@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — lists/sec of the LTR training hot path on B200 (BASELINE.json metric).
+"""bench.py — lists/sec of the LTR training hot path on H100 (BASELINE.json metric).
 
-Workloads (`--config`, BASELINE.json `configs[k - 1]`; the driver default is 2, the
+Workloads (`--config`, BASELINE.json `configs[k - 1]`; the default is 2, the
 configuration the metric is quoted on):
   2  ApproxNDCG + 3-layer MLP (256-128-64 relu), B=1024 N=200 D=136, fp32 (3xTF32)
   3  LambdaLoss (pairwise logistic + NDCGLambdaWeight), bf16 scorer, N=512 D=256,
@@ -22,6 +22,9 @@ synthetic data.  Prints ONE JSON line:
   cpu_baseline the reference algorithm's CPU step (oracle port) on the host cores
 `--impl reference` times the reference algorithm's CPU path on all host cores (oracle
 port: the reference needs TensorFlow, which cannot be installed here).
+`--dump-outputs DIR` writes what the last timed step computed (loss, scores, gradient,
+updated parameters; the last N's loss gradient for config 5) as DIR/<name>.npy, so that two
+builds can be compared output for output: inputs and parameters are seeded.
 """
 import argparse
 import json
@@ -32,6 +35,7 @@ import threading
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.dont_write_bytecode = True   # the tree may be read-only: no __pycache__ next to the sources
 if ROOT not in sys.path:
   sys.path.insert(0, ROOT)
 
@@ -57,7 +61,7 @@ WORKLOADS = {
             group_size=2, cpu_sample=256),
 }
 SWEEP_NS = (32, 64, 128, 256, 512, 1024)
-DTYPE_NAME = {'fp32': 'fp32', 'tf32x3': 'fp32 (3xTF32 on tcgen05)', 'tf32': 'tf32',
+DTYPE_NAME = {'fp32': 'fp32', 'tf32x3': 'fp32 (3xTF32 on wgmma)', 'tf32': 'tf32',
               'bf16': 'bf16 (fp32 accumulate, fp32 master weights)'}
 
 
@@ -94,8 +98,9 @@ def load_peaks():
             'bf16_tflops_sustained': p.get('bf16_tflops_sustained',
                                            p['bf16_tflops']),
             'source': 'measured'}
-  return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0,
-          'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+  # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+  return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0,
+          'bf16_tflops_sustained': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 class ClockSampler(threading.Thread):
@@ -406,6 +411,10 @@ def run_gpu(args):
   ms_step = float(t) / args.steps
   value = B * world / (ms_step * 1e-3)
   final_loss = float(loss)
+  if args.dump_outputs and rank == 0:   # before the phase / e2e runs move the parameters
+    dump_outputs(args.dump_outputs, {
+        'loss': loss.detach().reshape(1), 'scores': trainer.scores, 'grads': trainer.grads,
+        'params': tower.flat.data, 'adagrad_accum': trainer.accum})
 
   # ---- per-phase device time (same process, CUDA events on the launch stream) --
   phase = phase_times(trainer, resident, args.steps, stream)
@@ -440,11 +449,9 @@ def run_gpu(args):
     achieved = step_fl * B / (gemm_ms * 1e-3) / 1e12
     peak = peaks['bf16_tflops_sustained']
     # SURVEY.md §8(d): the algorithmic bytes of the scorer are X read twice (forward and
-    # dW_1); activations are recomputable on chip, so what the layer-by-layer plan moves
-    # beyond that is re-read traffic, reported as `traffic` / `traffic_ratio`.
+    # dW_1); activations are recomputable on chip.
     xbytes = 2 if precision == 'bf16' else 4
     alg_bytes = 2 * D * xbytes * N * B
-    traffic = load_traffic(cfg_id, precision)
     loss_bytes = (12 * N + 16) * B
     pair_evals = float(N) * N * B
     tf32_peak = measure_tf32_peak(dev) if precision in ('tf32x3', 'tf32') else None
@@ -453,12 +460,8 @@ def run_gpu(args):
         'bound': 'tensor', 'achieved': achieved, 'peak': peak,
         'unit': 'TFLOP/s', 'frac': achieved / peak,
         'peak_source': peaks['source'] + ' bf16 sustained',
-        'traffic': traffic['scorer_gemm_dram_bytes_per_step'] if traffic else None,
-        'traffic_source': traffic['source'] if traffic else None,
         'algorithmic_flops_per_step': step_fl * B,
         'algorithmic_bytes_per_step': alg_bytes,
-        'traffic_ratio': (traffic['scorer_gemm_dram_bytes_per_step'] / alg_bytes
-                          if traffic else None),
         'kernel_ms_per_step': gemm_ms,
     }
     if tf32_peak:
@@ -475,7 +478,6 @@ def run_gpu(args):
         'frac': alg_bytes / (gemm_ms * 1e-3) / 1e9 / peaks['hbm_gbs'],
         'algorithmic_bytes_per_step': alg_bytes,
         'note': 'SURVEY.md §8(d) bytes: X read twice',
-        'traffic': roof_gemm['traffic'], 'traffic_ratio': roof_gemm['traffic_ratio'],
     }
     roof_loss = {
         'kernel': {'approx_ndcg_loss': 'approx_loss_kernel',
@@ -534,16 +536,6 @@ def run_gpu(args):
     dist.destroy_process_group()
 
 
-def load_traffic(cfg_id, precision):
-  """dram__bytes_read + write of the scorer GEMM kernels per step, from the committed ncu
-  capture of this round (profiles/r02_traffic.json), if one exists for this workload."""
-  tpath = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-  if not os.path.exists(tpath):
-    return None
-  t = json.load(open(tpath))
-  return t.get('config%d_%s' % (cfg_id, precision))
-
-
 def ndcg10_parity(tfr, trainer, host_batch, dev, lists=64):
   """NDCG@10 of the scores the GPU scorer produces, computed by the CUDA metric kernel and
   by the oracle metric on the SAME scores (first `lists` lists of a batch): per-list max
@@ -577,7 +569,7 @@ def ndcg10_parity(tfr, trainer, host_batch, dev, lists=64):
 
 def measure_tf32_peak(dev, n=8192, reps=5):
   """Dense TF32 throughput of this GPU as cuBLAS reaches it (torch.matmul, 8192^3, best
-  of `reps`): the measured roof of `kind::tf32` MMAs — MEASURED_PEAKS.json only carries
+  of `reps`): the measured roof of TF32 tensor-core MMAs — MEASURED_PEAKS.json only carries
   the bf16 number.  Measurement aid outside every timed region; never on the product path."""
   try:
     prev = torch.backends.cuda.matmul.allow_tf32
@@ -709,6 +701,9 @@ def run_sweep(args):
                    'hbm_gbs_algorithmic': bytes_ / (ms * 1e-3) / 1e9,
                    'hbm_frac_per_gpu': bytes_ / world / (ms * 1e-3) / 1e9 / peaks['hbm_gbs'],
                    'pair_evals_per_s': float(n) * n * b * world / (ms * 1e-3)})
+      if args.dump_outputs and rank == 0 and lam_name == 'ndcg' and n == SWEEP_NS[-1]:
+        dump_outputs(args.dump_outputs, {'grad': grad, 'per_list': per_list,
+                                         'total': total2})
       del bufs
   if rank == 0:
     sampler.stop()
@@ -730,6 +725,20 @@ def run_sweep(args):
   if world > 1:
     dist.barrier()
     dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, arrays, limit_bytes=64 << 20):
+  """Writes each tensor as out_dir/<name>.npy in float32, flattened when it exceeds its share
+  of `limit_bytes` to a fixed, seeded sample of its elements."""
+  import numpy as np
+  os.makedirs(out_dir, exist_ok=True)
+  share = limit_bytes // max(len(arrays), 1) // 4
+  for name, t in arrays.items():
+    a = t.detach().float().cpu()
+    if a.numel() > share:
+      idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:share]
+      a = a.reshape(-1)[idx.sort().values]
+    np.save(os.path.join(out_dir, name + '.npy'), a.numpy())
 
 
 _REAL_STDOUT = None
@@ -757,11 +766,13 @@ def main():
   ap.add_argument('--precision', default=None,
                   choices=['fp32', 'tf32x3', 'tf32', 'bf16'],
                   help='scorer GEMM arithmetic (default: the workload\'s: tf32x3 = '
-                       'fp32-faithful 3xTF32 on tcgen05 for configs 2 / 4, bf16 for 3)')
+                       'fp32-faithful 3xTF32 on wgmma for configs 2 / 4, bf16 for 3)')
   ap.add_argument('--collective', default='fused', choices=['fused', 'nccl'])
   ap.add_argument('--cpu-sample-lists', type=int, default=0)
   ap.add_argument('--cpu-steps', type=int, default=3)
   ap.add_argument('--no-cpu-baseline', action='store_true')
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='write the outputs of the last timed step to DIR/<name>.npy')
   args = ap.parse_args()
   args.warmup = max(args.warmup, 3)
   # The contract is ONE JSON line on stdout.  Libraries print banners there (e.g.

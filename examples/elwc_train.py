@@ -1,5 +1,5 @@
 """Training on TFRecord files of ExampleListWithContext protos (the reference's
-`tfr.keras.pipeline` input format) with the fused B200 step.
+`tfr.keras.pipeline` input format) with the fused GPU step.
 
   python examples/elwc_train.py --train_path train.tfrecord --num_features 136 \
       --feature_name f --label_name utility --output_dir /tmp/out

@@ -1,4 +1,4 @@
-"""Training on LibSVM ranking files with the fused B200 step: the workflow of
+"""Training on LibSVM ranking files with the fused GPU step: the workflow of
 examples/tf_ranking_libsvm.py (hidden 256-128-64, pairwise_logistic_loss, Adagrad,
 list_size 100, 136 features) through `ranking_b200`.
 

@@ -1,5 +1,5 @@
 /*
- * tfr_b200.h — C ABI of the B200-native learning-to-rank hot path.
+ * tfr_b200.h — C ABI of the H100-native learning-to-rank hot path.
  *
  * The reference (tensorflow/ranking) has no FFI: its seam is the Python class
  * surface `tfr.keras.losses / tfr.keras.metrics / tfr.keras.model`
@@ -318,9 +318,9 @@ int tfr_weighted_sum(const float* v, const float* w, int n, float scale,
  * layout) then b_i [out].  Gradients use the same layout.
  * precision: how the GEMMs are evaluated
  *   TFR_PREC_FP32   fp32 CUDA-core FFMA
- *   TFR_PREC_TF32X3 tcgen05 kind::tf32, 3-pass error-compensated split (~fp32)
- *   TFR_PREC_TF32   tcgen05 kind::tf32, 1 pass
- *   TFR_PREC_BF16   tcgen05 kind::f16 (bf16 operands, fp32 accumulate)
+ *   TFR_PREC_TF32X3 wgmma tf32, 3-pass error-compensated split (~fp32)
+ *   TFR_PREC_TF32   wgmma tf32, 1 pass
+ *   TFR_PREC_BF16   wgmma bf16 (bf16 operands, fp32 accumulate)
  * ------------------------------------------------------------------------- */
 typedef enum {
   TFR_PREC_FP32 = 0,
@@ -427,7 +427,7 @@ int tfr_group_mlp_bwd(const float* X, int B, int N, int G, int gs, const int32_t
 int tfr_group_mlp_check(const tfr_mlp_cfg* cfg, int B, int N, int G, int gs,
                         void* workspace, void* stream);
 
-/* Parity helper: one GEMM through the tcgen05 TF32 engine that the scorer tower
+/* Parity helper: one GEMM through the wgmma TF32 engine that the scorer tower
  * uses (D[GM,GN] = A[GM,GK] * B[GK,GN]).  a_mn/b_mn select the operand storage
  * (0: K contiguous, i.e. A stored [GM,GK], B stored [GN,GK]; 1: M/N contiguous,
  * i.e. A stored [GK,GM], B stored [GK,GN]); passes 1 = TF32, 3 = 3xTF32 (fp32-
@@ -441,7 +441,7 @@ int tfr_tc_gemm(const float* A, int lda, const float* B, int ldb, const float* B
                 size_t split_stride, uint32_t* mask_bits_out,
                 const uint32_t* mask_bits_in, void* stream);
 
-/* Parity helper for the bf16 engine (tcgen05 kind::f16, csrc/tc_gemm_bf16.cuh):
+/* Parity helper for the bf16 engine (Hopper wgmma, csrc/tc_gemm_bf16.cuh):
  * D[GM,GN] = A[GM,GK] * B[GK,GN] with bf16 operands and fp32 accumulation.
  *   mn = 0: A stored [GM,GK], B stored [GN,GK]; C bf16 [GM,GN]; epi 0 store, 1 bias+act
  *           (+ ReLU sign bits to mask_bits_out), 3 mask by mask_bits_in (+ fp32 column sums
@@ -455,10 +455,6 @@ int tfr_tc_gemm_bf16(const void* A, int lda, const void* B, int ldb, void* C, in
                      uint32_t* mask_bits_out, const uint32_t* mask_bits_in,
                      float* colsum, int colsum_stride, int* colsum_slots_out,
                      int splits, size_t split_stride, void* stream);
-
-/* Profiling aid for the engine above: device buffer [num_SMs][12] of int64 that each
- * GEMM launch fills with per-warp-role mbarrier wait cycles (NULL disables). */
-int tfr_tc_set_debug(long long* buf);
 
 /* ---------------------------------------------------------------------------
  * Input side (host code, no device work): a batch of serialized

@@ -113,7 +113,6 @@ _SIGNATURES = {
                          _P, _P, _I, _I, _I, C.c_size_t, _P, _P, _P]),
     'tfr_tc_gemm_bf16': (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P,
                               _I, _P, _I, C.c_size_t, _P]),
-    'tfr_tc_set_debug': (_I, [_P]),
     'tfr_dp_alloc': (_I, [C.c_size_t, C.POINTER(C.c_void_p), C.POINTER(C.c_ubyte * 64)]),
     'tfr_dp_open': (_I, [C.POINTER(C.c_ubyte * 64), C.POINTER(C.c_void_p)]),
     'tfr_dp_close': (_I, [_P]),

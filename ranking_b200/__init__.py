@@ -1,9 +1,9 @@
-"""ranking_b200 — B200-native learning-to-rank training path.
+"""ranking_b200 — H100-native learning-to-rank training path.
 
 Drop-in for the hot path of tensorflow/ranking: `keras.losses`, `keras.metrics`,
 `keras.model` / `keras.layers` scorer, plus the numeric cores `losses_impl`,
 `metrics_impl`, `utils`.  Host code is Python over torch tensors; all arithmetic
-runs in hand-written sm_100a CUDA kernels behind the C ABI in
+runs in hand-written sm_90a CUDA kernels behind the C ABI in
 `include/tfr_b200.h` (loaded by `ranking_b200._C`; importing this package
 without the built library raises).
 """

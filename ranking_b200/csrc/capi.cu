@@ -18,6 +18,17 @@ void set_error(const char* fmt, ...) {
 static unsigned long long g_launches = 0;
 void count_launch() { __atomic_add_fetch(&g_launches, 1ull, __ATOMIC_RELAXED); }
 
+int num_sms() {
+  static int n = 0;
+  if (n <= 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+      return 132;   // no device to ask (e.g. planning on a CPU-only build machine)
+  }
+  return n;
+}
+
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 int make_mlp_plan(const tfr_mlp_cfg* cfg, int M, MlpPlan* p) {
@@ -114,18 +125,11 @@ int make_mlp_plan(const tfr_mlp_cfg* cfg, int M, MlpPlan* p) {
     p->dz_off[i] = w;
     w += align_up((size_t)M * max_hidden, 64);
   }
-  // Row splits of the dW GEMMs / bias partials: about one per SM, so that the
-  // persistent GEMM's tile list (m_tiles x splits) divides evenly over the SMs.
+  const int sms = num_sms();
+  // Row splits of the dW GEMMs / bias partials: about one per SM, so that the persistent
+  // GEMM has a split for every SM even when the dW output is one or two 128 x 128 tiles.
   {
-    static int num_sms = 0;
-    if (num_sms == 0) {
-      int dev = 0;
-      if (cudaGetDevice(&dev) != cudaSuccess ||
-          cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-          num_sms <= 0)
-        num_sms = 148;   // B200 (also the answer on a CPU-only build box)
-    }
-    const int per = (M + num_sms - 1) / num_sms;
+    const int per = (M + sms - 1) / sms;
     p->rows_per_split = per < 256 ? 256 : ((per + 127) / 128) * 128;
     p->splits = M > 0 ? (M + p->rows_per_split - 1) / p->rows_per_split : 1;
   }
@@ -140,12 +144,14 @@ int make_mlp_plan(const tfr_mlp_cfg* cfg, int M, MlpPlan* p) {
   w += align_up(p->n_params, 64);
   p->wtlo_off = w;
   w += align_up(p->n_params, 64);
-  p->tile_slots = 4 * 1024;   // upper bound: 4 quarters x persistent CTAs (<= SM count)
+  // column-sum slots: 8 warps x persistent GEMM CTAs (one per SM; room for 512 SMs), or one
+  // per row split (about one per SM)
+  p->tile_slots = 4 * 1024;
   p->tile_stride = align_up((size_t)max_hidden, 64);
   p->tile_off = w;
   w += (size_t)p->tile_slots * p->tile_stride;
   // output-layer backward: about 4 blocks per SM, each owning one slot
-  p->out_rows = M > 0 ? ((M + 591) / 592 + 3) / 4 * 4 : 4;
+  p->out_rows = M > 0 ? ((M + 4 * sms - 1) / (4 * sms) + 3) / 4 * 4 : 4;
   if (p->out_rows < 16) p->out_rows = 16;
   p->out_slots = (M + p->out_rows - 1) / p->out_rows;
   p->oslot_stride = align_up((size_t)p->dims[L] * (p->dims[L + 1] + 1) + p->dims[L + 1] + 4, 64);

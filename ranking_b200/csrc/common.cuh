@@ -1,4 +1,4 @@
-// Shared helpers for the tfr_b200 kernels (sm_100a).
+// Shared helpers for the tfr_b200 kernels (sm_90a).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -14,6 +14,7 @@ namespace tfr {
 // ---- error plumbing (host) -------------------------------------------------
 void set_error(const char* fmt, ...);
 void count_launch();   // bumps the host-side launch counter (tfr_launch_count)
+int num_sms();         // SM count of the current device; 132 (H100 SXM) when none can be queried
 
 #define TFR_REQUIRE(cond, ...)              \
   do {                                      \

@@ -177,7 +177,8 @@ extern "C" int tfr_allreduce_optimizer_step(const void* const* grad_ptrs,
   const size_t n4 = n / 4;
   size_t blocks = (n4 + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 296) blocks = 296;   // <= 2 CTAs per SM: every CTA is resident while it spins
+  // <= 2 CTAs per SM: every CTA is resident while it spins
+  if (blocks > (size_t)(2 * num_sms())) blocks = (size_t)(2 * num_sms());
   allreduce_optimizer_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       t, rank, world, epoch, params, accum, summed_out, n4, n, kind, lr, eps, grad_scale);
   TFR_LAUNCH_OK();

@@ -70,14 +70,14 @@ int mlp_simt_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                  const float* dscores, const uint8_t* mask, float* ws, float* grads,
                  cudaStream_t st);
 
-// tensor-core (tcgen05) path; passes = 1 (TF32) or 3 (3xTF32, fp32-faithful)
+// tensor-core (wgmma) path; passes = 1 (TF32) or 3 (3xTF32, fp32-faithful)
 int mlp_tc_fwd(const float* X, int M, const MlpPlan& p, const float* params,
                const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st);
 int mlp_tc_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                const float* dscores, const uint8_t* mask, float* ws, float* grads,
                int passes, cudaStream_t st);
 
-// bf16 tensor-core path (tcgen05 kind::f16): X and all activations are bf16 in HBM
+// bf16 tensor-core path (wgmma bf16): X and all activations are bf16 in HBM
 int mlp_bf16_fwd(const void* X, int M, const MlpPlan& p, const float* params,
                  const uint8_t* mask, float* ws, float* scores, cudaStream_t st);
 int mlp_bf16_bwd(const void* X, int M, const MlpPlan& p, const float* params,

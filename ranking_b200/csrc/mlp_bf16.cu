@@ -1,5 +1,5 @@
 // K5/K6, bf16 mode (TFR_PREC_BF16, BASELINE config 3): the scorer tower's Dense layers on
-// the tcgen05 kind::f16 engine (tc_gemm_bf16.cu).
+// the Hopper wgmma bf16 engine (tc_gemm_bf16.cu).
 //
 //   storage   X, hidden activations H_d and the backward signals dZ_d are bf16 in HBM
 //             (half the bytes of every activation term); parameters stay fp32 (master
@@ -168,7 +168,7 @@ out_bwd_bf16_kernel(const __nv_bfloat162* __restrict__ H2, int M, int K, int O,
 // Eight lanes share a row: a lane owns 8 consecutive k (one 16-byte load) per 64-wide chunk,
 // a warp instruction covers four rows and the loop is unrolled over four of them, so a warp
 // keeps 16 rows (2 KB) in flight.  The row-per-warp kernels above move 128 B per warp and
-// load round trip: 58 us / 97 us for 34 MB at config 3 (profiles/r02_launches_c3.txt).
+// load round trip.
 constexpr int kFastK = 128, kFastO = 2;
 
 __device__ __forceinline__ void unpack8(const uint4& v, float (&h)[8]) {
@@ -392,7 +392,8 @@ int mlp_bf16_fwd(const void* X, int M, const MlpPlan& p, const float* params,
   }
   const int K = p.dims[L], O = p.dims[L + 1];
   if (K <= kFastK && O <= kFastO) {
-    const int nb = (M + 31) / 32 < 148 * 8 ? (M + 31) / 32 : 148 * 8;   // 32 rows per block pass
+    const int cap = 8 * num_sms();
+    const int nb = (M + 31) / 32 < cap ? (M + 31) / 32 : cap;   // 32 rows per block pass
     const uint4* H8 = reinterpret_cast<const uint4*>(in);
     const float* Wl = params + p.w_off[L];
     const float* bl = params + p.b_off[L];
@@ -406,7 +407,8 @@ int mlp_bf16_fwd(const void* X, int M, const MlpPlan& p, const float* params,
     TFR_LAUNCH_OK();
     return TFR_OK;
   }
-  const int blocks = (M + 7) / 8 < 148 * 16 ? (M + 7) / 8 : 148 * 16;
+  const int bcap = 16 * num_sms();
+  const int blocks = (M + 7) / 8 < bcap ? (M + 7) / 8 : bcap;
   out_fwd_bf16_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat162*>(in), M,
                                               K / 2, O, params + p.w_off[L], params + p.b_off[L],
                                               mask, scores);

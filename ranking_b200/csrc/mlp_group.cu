@@ -331,7 +331,8 @@ extern "C" int tfr_circular_pad_gather(const void* x, const uint8_t* is_valid, i
   const int row_vecs = row_bytes / 16;
   const size_t total = (size_t)B * N * row_vecs;
   size_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  const size_t cap = 16 * (size_t)num_sms();   // 16 blocks per SM
+  if (blocks > cap) blocks = cap;
   gather_rows_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const uint4*>(x), idx_out, N,
                                                       row_vecs, total, static_cast<uint4*>(out));
   TFR_LAUNCH_OK();
@@ -464,7 +465,8 @@ extern "C" int tfr_group_mlp_bwd(const float* X, int B, int N, int G, int gs, co
   rc = mlp_tc_bwd_until(1, &tail, nullptr, M, p, params, gw.gscore, nullptr, ws, grads, passes, st);
   if (rc) return rc;
   // first layer: dP_j by the inverse index, dW_1^(j) = X^T dP_j (rows split over CTAs)
-  const int per = (int)((bn + 147) / 148);
+  const int sms = num_sms();
+  const int per = (int)((bn + sms - 1) / sms);   // about one split per SM
   const int rows_per = per < 256 ? 256 : ((per + 127) / 128) * 128;
   int splits = (int)((bn + rows_per - 1) / rows_per);
   if (splits > p.splits) splits = p.splits;
@@ -474,16 +476,9 @@ extern "C" int tfr_group_mlp_bwd(const float* X, int B, int N, int G, int gs, co
     group_gather_bwd_kernel<<<(unsigned)((t + 255) / 256), 256, 0, st>>>(tail.dz, gw.inv, S, B, N,
                                                                          G, gs, j, H, dP);
     TFR_LAUNCH_OK();
-    // dW^(j)^T [H, D] = dP_j^T X, stored transposed (the orientation of mlp_tc_bwd when the
-    // output width is the larger side is decided the same way: fewer UMMA tiles)
-    auto cost = [](int gm, int gn) {
-      const int n16 = (gn + 15) / 16 * 16;
-      const int ntiles = (n16 + 255) / 256;
-      const int n_umma = n16 < 256 ? n16 : 256;
-      const long long mmas = (long long)((gm + 127) / 128) * ntiles;
-      return mmas * (1 << 20) + mmas * (16384 + 128 * n_umma);
-    };
-    const bool swapped = cost(H, D) < cost(D, H);
+    // dW^(j) [D, H] = X^T dP_j, or its transpose when that orientation has fewer tile units
+    // (decided as in mlp_tc_bwd)
+    const bool swapped = tc::tile_units(H, D) < tc::tile_units(D, H);
     tc::GemmDesc g{};
     if (!swapped) {
       g.A = X; g.lda = D; g.B = dP; g.ldb = H;

@@ -1,4 +1,4 @@
-// K5/K6 tensor-core path: the scorer tower's Dense layers on the tcgen05 TF32
+// K5/K6 tensor-core path: the scorer tower's Dense layers on the Hopper wgmma TF32
 // engine (tc_gemm.cu).  passes = 3 is the fp32-faithful 3xTF32 mode used for the
 // fp32 configuration; passes = 1 is plain TF32.
 //
@@ -22,8 +22,7 @@ struct SplitTable {
 
 // hi = round-to-nearest TF32 of every parameter, lo = the fp32 residual; blockIdx.y = 1 + d
 // additionally writes the transposes W_d^T [out, in] of the hidden kernels (hi / lo), the
-// K-major B operand of the forward GEMMs: one TMA box per stage instead of one per 32
-// output columns.
+// K-major B operand of the forward GEMMs: the engine stages it without a transpose.
 __global__ void __launch_bounds__(256)
 split_params_kernel(const float* __restrict__ p, size_t n, SplitTable t, float* __restrict__ hi,
                     float* __restrict__ lo, float* __restrict__ thi, float* __restrict__ tlo) {
@@ -210,24 +209,7 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
       // dW[Kin, Nout] = A^T dZ in one of two orientations:
       //   direct : GM = Kin (tiles of 128), GN = Nout
       //   swapped: GM = Nout,               GN = Kin, stored transposed
-      // Cost of one 32-row k block (tools/mma_rate.cu: a 128 x N x 8 TF32 MMA takes N / 2
-      // cycles; profiles/r02_tc_gemm_wait_cycles.txt: the dW GEMMs are bound by shared-memory
-      // traffic, 128 B / cycle): per 128-row block of the M side the stage is written by TMA,
-      // read by the splitters (the M side goes to tensor memory), the N side is rewritten as
-      // hi / lo and read by 12 MMAs.  Fewer than 3 pipeline stages expose the load latency.
-      auto cost = [](int gm, int gn) {
-        const int n16 = (gn + 15) / 16 * 16;
-        const int ntiles = (n16 + 255) / 256;
-        const int n_umma = n16 < 256 ? n16 : 256;
-        const long long tiles = (long long)((gm + 127) / 128) * ntiles;
-        const long long mma = tiles * 12 * (n_umma / 2);
-        const long long smem = tiles * (32768 + 896LL * n_umma) / 128;
-        const long long stage = 16384 + 256LL * n_umma;
-        long long c = mma > smem ? mma : smem;
-        if (200 * 1024 / stage < 3) c = c * 3 / 2;
-        return c;
-      };
-      const bool swapped = cost(Nout, Kin) < cost(Kin, Nout);
+      const bool swapped = tc::tile_units(Nout, Kin) < tc::tile_units(Kin, Nout);
       tc::GemmDesc g{};
       if (!swapped) {
         g.A = A; g.lda = Kin; g.B = dz_cur; g.ldb = Nout;

@@ -1,4 +1,4 @@
-// tcgen05 (UMMA) TF32 GEMM engine for the scorer tower — declarations.
+// Hopper wgmma TF32 / 3xTF32 GEMM engine for the scorer tower — declarations.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -12,8 +12,8 @@ enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 
 // D[GM, GN] = A[GM, GK] * B[GK, GN]  (fp32 in / fp32 out, TF32 tensor cores)
 //
 // Operand storage (all row-major fp32 in global memory):
-//   a_mn == 0 : A stored [GM, GK]  (K contiguous  -> UMMA K-major)
-//   a_mn == 1 : A stored [GK, GM]  (GM contiguous -> UMMA MN-major)
+//   a_mn == 0 : A stored [GM, GK]  (K contiguous  -> K-major)
+//   a_mn == 1 : A stored [GK, GM]  (GM contiguous -> MN-major)
 //   b_mn == 0 : B stored [GN, GK]  (K contiguous  -> K-major)
 //   b_mn == 1 : B stored [GK, GN]  (GN contiguous -> MN-major)
 // passes == 1 : one TF32 product (operands truncated to TF32)
@@ -36,7 +36,7 @@ struct GemmDesc {
   int splits;                    // split the GK loop over blockIdx.z; split z writes to
   size_t split_stride;           //   C + z * split_stride (floats); k range rounded to 32
   float* colsum;                 // optional: column sums of everything each CTA stored, slot
-  int colsum_stride;             //   (cta * 8 + epilogue warp), row pitch in floats;
+  int colsum_stride;             //   (cta * 8 + warp), row pitch in floats;
   int* colsum_slots_out;         //   receives the number of slots written (8 * CTAs)
   // ReLU sign bits, word [(col / 32) * GM + row] (bit j = column 32 * (col / 32) + j):
   uint32_t* mask_bits_out;       //   EPI_BIAS_ACT: written next to C (stored value > 0)
@@ -44,8 +44,12 @@ struct GemmDesc {
 };
 
 // Returns a tfr_status.  Requirements (checked): lda/ldb multiples of 4 floats,
-// 16-byte aligned base pointers, GN <= 256 per tile handled internally by tiling.
+// 16-byte aligned base pointers, any GN (128-column output tiles).
 int gemm(const GemmDesc& g, cudaStream_t stream);
+
+// Work units of a GM x GN output: 128-row tiles of one or two 64-column MMA halves, each
+// walking the whole k range.  Picks the cheaper orientation of a dW GEMM.
+inline int tile_units(int gm, int gn) { return ((gm + 127) / 128) * ((gn + 63) / 64); }
 
 // True if a layer shape can run on this engine (alignment constraints).
 bool shape_supported(int rows_ld_a, int rows_ld_b);

@@ -1,4 +1,4 @@
-// tcgen05 (UMMA) bf16 GEMM engine for the scorer tower (TFR_PREC_BF16) — declarations.
+// Hopper wgmma bf16 GEMM engine for the scorer tower (TFR_PREC_BF16) — declarations.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -9,14 +9,14 @@ namespace tcb {
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_BITS = 3 };
 
-// D[GM, GN] = A[GM, GK] * B[GK, GN], bf16 operands, fp32 accumulation in tensor memory.
+// D[GM, GN] = A[GM, GK] * B[GK, GN], bf16 operands, fp32 accumulation.
 //
 //   mn == 0 (forward / dZ GEMMs): A stored [GM, GK], B stored [GN, GK] (K contiguous);
-//           C is bf16 [GM, GN] row-major, written by TMA stores; epilogues:
+//           C is bf16 [GM, GN] row-major; epilogues:
 //             EPI_BIAS_ACT  C = act(D + bias), optionally the ReLU sign bits of the stored
 //                           values to mask_bits_out, word [(col / 32) * GM + row]
 //             EPI_MASK_BITS C = bit ? D : 0 with bits from mask_bits_in; optionally the
-//                           column sums of C (fp32, before rounding) per CTA and epilogue
+//                           column sums of C (fp32, before rounding) per CTA and
 //                           warp to `colsum` (bias gradients)
 //             EPI_STORE     C = D
 //   mn == 1 (dW GEMMs): A stored [GK, GM], B stored [GK, GN] (M / N contiguous), i.e.

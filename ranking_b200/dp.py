@@ -5,7 +5,7 @@ lists across ranks (one process per GPU) and the ONLY data-path collective per
 training step is one all-reduce(SUM) of the flat fp32 scorer gradient, with the
 1/num_replicas factor of the reference (extension/task.py:256-262) folded into
 the optimizer kernel.  Metric means all-reduce their (sum v*w, sum w) state.
-Works on any backend: NCCL over NVLink on B200 boxes, gloo in the CPU tests.
+Works on any backend: NCCL over NVLink on H100 boxes, gloo in the CPU tests.
 """
 import torch
 import torch.distributed as dist

@@ -226,7 +226,7 @@ def create_tower(hidden_layer_dims, output_units, activation=None,
                  input_dim=None, precision=None, seed=None, **kwargs):
   """keras/layers.py:26-77.  Same arguments and defaults as the reference.
 
-  `precision`: None (default) = 'tf32x3' (tcgen05, fp32-faithful) when every Dense input
+  `precision`: None (default) = 'tf32x3' (wgmma, fp32-faithful) when every Dense input
   width is a multiple of 4, else 'fp32' (FFMA); 'tf32', 'bf16' on request.
 
   BatchNormalization (batch statistics in `train()` mode, moving statistics in

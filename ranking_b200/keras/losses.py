@@ -590,6 +590,6 @@ def get(loss, reduction=Reduction.AUTO, lambda_weight=None, name=None, **kwargs)
     return _KEY_TO_CLS_WITH_LAMBDA[loss](lambda_weight=lambda_weight,
                                          **loss_kwargs)
   if loss in RankingLossKey.all_keys():
-    raise ValueError('unsupported loss: {} (not on the B200 hot path yet; see '
+    raise ValueError('unsupported loss: {} (not on the GPU hot path yet; see '
                      'DESIGN.md scope)'.format(loss))
   raise ValueError('unsupported loss: {}'.format(loss))

@@ -225,7 +225,7 @@ def get(key, name=None, dtype=None, topn=None, **kwargs):
   if key in _KEY_TO_CLS:
     return _KEY_TO_CLS[key](**metric_kwargs)
   if key in _ALL_KEYS:
-    raise ValueError('Unsupported metric: {} (not on the B200 hot path yet; see '
+    raise ValueError('Unsupported metric: {} (not on the GPU hot path yet; see '
                      'DESIGN.md scope)'.format(key))
   raise ValueError('Unsupported metric: {}'.format(key))
 

@@ -2,7 +2,7 @@
 
 Golden-vector tests are written once against a small namespace (`api`) and run
 against (a) the CPU oracle (always, `-m "not gpu"`) and (b) the CUDA product
-path through the C-ABI (`-m gpu`, on a B200).
+path through the C-ABI (`-m gpu`, on an H100).
 """
 import os
 import sys
@@ -17,7 +17,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: needs a CUDA device (B200)')
+  config.addinivalue_line('markers', 'gpu: needs a CUDA device (H100)')
 
 
 def _oracle_api():

@@ -575,7 +575,7 @@ def test_tower_forward_backward(oracle_api, shape):
     (6400, 256, [512, 64], 1, None),
 ])
 def test_tower_tensor_core_path(oracle_api, shape, precision, tol_fwd, tol_bwd):
-  """tcgen05 scorer path: 3xTF32 must stay fp32-faithful (1e-5), TF32 is looser.
+  """Tensor-core scorer path: 3xTF32 must stay fp32-faithful (1e-5), TF32 is looser.
 
   With ReLU, a hidden pre-activation that lies within rounding distance of zero
   can take the other branch than in the fp64 oracle; that moves a handful of

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 bf16 GEMM engine (csrc/tc_gemm_bf16.cu) through the C ABI,
+"""GPU tests of the wgmma bf16 GEMM engine (csrc/tc_gemm_bf16.cu) through the C ABI,
 against a torch fp64 matmul of the SAME bf16-rounded inputs (so only the fp32
 accumulation order and the bf16 rounding of the output differ).
 

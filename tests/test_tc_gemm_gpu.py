@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 TF32 GEMM engine (csrc/tc_gemm.cu) through the C ABI,
+"""GPU tests of the wgmma TF32 GEMM engine (csrc/tc_gemm.cu) through the C ABI,
 against a torch fp64 matmul of the same fp32 inputs.
 
 Tolerance: 3xTF32 (passes=3) must be fp32-faithful: <= 2e-6 of |A||B| row/col
@@ -29,8 +29,15 @@ def _pack_bits(keep):
   return words.t().contiguous().to(torch.int32)
 
 
+def C_ptr(buf, offset):
+  import ctypes
+  return ctypes.c_void_p(buf.data_ptr() + 4 * offset)
+
+
 def run_gemm(gm, gn, gk, a_mn, b_mn, passes, split_b, epi=0, act=0, transposed=0,
-             splits=1, seed=0, want_bits=False):
+             splits=1, seed=0, want_bits=False, c_pad=0):
+  """c_pad > 0: C starts c_pad floats into its buffer and split partials lie c_pad floats
+  further apart than gm * gn (4-byte aligned C, odd split strides)."""
   import ranking_b200  # noqa: F401
   from ranking_b200 import _C
   g = torch.Generator().manual_seed(seed)
@@ -55,13 +62,9 @@ def run_gemm(gm, gn, gk, a_mn, b_mn, passes, split_b, epi=0, act=0, transposed=0
   lay = (lambda t: t.contiguous()) if b_mn else (lambda t: t.t().contiguous())
   b_store = lay(b_hi).cuda()
   b_lo_store = None if b_lo is None else lay(b_lo).cuda()
-  if splits > 1:
-    stride = gm * gn
-    C = torch.full((splits, gn, gm) if transposed else (splits, gm, gn), float('nan'),
-                   device='cuda')
-  else:
-    stride = 0
-    C = torch.full((gn, gm) if transposed else (gm, gn), float('nan'), device='cuda')
+  shape = (gn, gm) if transposed else (gm, gn)
+  stride = gm * gn + c_pad if splits > 1 else 0
+  buf = torch.full((c_pad + max(splits, 1) * (gm * gn + c_pad),), float('nan'), device='cuda')
   ldc = gm if transposed else gn
   bias_d, aux_d = bias.cuda(), aux.cuda()    # keep alive until the sync below
   bits_out = bits_in = None
@@ -71,11 +74,13 @@ def run_gemm(gm, gn, gk, a_mn, b_mn, passes, split_b, epi=0, act=0, transposed=0
     bits_in = _pack_bits(aux > 0).cuda()
   rc = _C.lib.tfr_tc_gemm(
       _C.ptr(a_store), a_store.shape[1], _C.ptr(b_store), b_store.shape[1],
-      _C.ptr(b_lo_store), _C.ptr(C), ldc, gm, gn, gk, a_mn, b_mn, passes, split_b,
+      _C.ptr(b_lo_store), C_ptr(buf, c_pad), ldc, gm, gn, gk, a_mn, b_mn, passes, split_b,
       epi, _C.ptr(bias_d), _C.ptr(aux_d), act, transposed, splits, stride,
       _C.ptr(bits_out), _C.ptr(bits_in), _C.stream())
   _C.check(rc)
   torch.cuda.synchronize()
+  C = torch.stack([buf[c_pad + z * stride:c_pad + z * stride + gm * gn].view(shape)
+                   for z in range(splits)]) if splits > 1 else buf[c_pad:c_pad + gm * gn].view(shape)
   out = C.double().cpu()
   if want_bits:
     assert torch.equal(bits_out.cpu(), _pack_bits(C.cpu() > 0))
@@ -125,13 +130,21 @@ def test_tc_gemm_epilogues_and_splits():
   assert err <= 2e-6, err
 
 
+def test_tc_gemm_unaligned_output():
+  """C only 4-byte aligned, and split-K partials an odd number of floats apart: the paired
+  stores of the epilogue must fall back to single ones."""
+  err, _, _ = run_gemm(300, 136, 136, 0, 1, 3, 0, epi=1, act=1, c_pad=1)
+  assert err <= 2e-6, err
+  err, _, _ = run_gemm(256, 136, 2048, 1, 1, 3, 1, splits=3, c_pad=1)
+  assert err <= 2e-6, err
+
+
 @pytest.mark.parametrize('gm', [512, 600, 657, 1280])
 @pytest.mark.parametrize('gn,gk', [(256, 136), (128, 256), (64, 128)])
 def test_tc_gemm_cta_pairs_kmajor(gm, gn, gk):
-  """Forward / dZ GEMM shapes that run as CTA pairs (cta_group::2, K-major pre-split weights,
-  >= 4 row blocks): even and odd block counts (600 rows = 5 blocks: the last pair has a
-  phantom half), ragged last blocks (657), every compile-time epilogue (store, bias + ReLU +
-  sign bits, mask from sign bits)."""
+  """Forward / dZ GEMM shapes (K-major pre-split weights, >= 4 row blocks): even and odd
+  block counts (600 rows = 5 blocks), ragged last blocks (657), every epilogue (store,
+  bias + ReLU + sign bits, mask from sign bits)."""
   for epi, act, bits in ((0, 0, False), (1, 1, True), (3, 1, False)):
     err, _, _ = run_gemm(gm, gn, gk, 0, 0, 3, 0, epi=epi, act=act, want_bits=bits, seed=gm + gn)
     assert err <= 2e-6, (gm, gn, gk, epi, err)
@@ -140,9 +153,8 @@ def test_tc_gemm_cta_pairs_kmajor(gm, gn, gk):
 @pytest.mark.parametrize('shape', [(256, 136, 4096, 1, 4), (256, 128, 4096, 0, 8),
                                    (384, 136, 2048, 1, 3), (640, 64, 1536, 0, 5)])
 def test_tc_gemm_cta_pairs_dw(shape):
-  """dW GEMM shapes that run as CTA pairs (MN-major operands split on the fly, M side through
-  tensor memory, N rounded up to 64): 2, 3 (phantom half) and 5 row blocks, split-K partials,
-  transposed and direct stores."""
+  """dW GEMM shapes (MN-major operands split on the fly): 2, 3 and 5 row blocks, split-K
+  partials, transposed and direct stores."""
   gm, gn, gk, transposed, splits = shape
   err, _, _ = run_gemm(gm, gn, gk, 1, 1, 3, 1, transposed=transposed, splits=splits, seed=gm)
   assert err <= 2e-6, (shape, err)

@@ -1,5 +1,5 @@
 """Runs ONE scorer GEMM shape of the bench configuration through the TF32 engine, a few times,
-for `ncu --set full --import-source on -k regex:tc_gemm -c 1` captures (no debug counters).
+for `ncu --set full --import-source on -k regex:gemm_kernel -c 1` captures.
 usage: gemm_only.py {fwd1|fwd2|fwd3|dz1|dz2|dw1|dw2|dw3}"""
 import os
 import sys
