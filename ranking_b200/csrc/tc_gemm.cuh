@@ -18,7 +18,7 @@ enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 
 //   b_mn == 1 : B stored [GK, GN]  (GN contiguous -> MN-major)
 // passes == 1 : one TF32 product (operands truncated to TF32)
 // passes == 3 : error-compensated 3xTF32: x = hi + lo, D = Ahi*Bhi + Alo*Bhi + Ahi*Blo.
-//               A is always split on the fly in shared memory.  B is split on the
+//               A is always split on the fly, in registers.  B is split on the
 //               fly too when split_b != 0, otherwise `B` must hold the hi parts
 //               and `B_lo` the lo parts (weights, pre-split once per step).
 struct GemmDesc {
@@ -47,7 +47,8 @@ struct GemmDesc {
 // 16-byte aligned base pointers, any GN (128-column output tiles).
 int gemm(const GemmDesc& g, cudaStream_t stream);
 
-// Work units of a GM x GN output: 128-row tiles of one or two 64-column MMA halves, each
+// Work units of a GM x GN output: 128-row tiles of one m64n128 (two units) or, when the
+// tile's live columns fit in 64, one m64n64 (one unit) per warpgroup and k step, each
 // walking the whole k range.  Picks the cheaper orientation of a dW GEMM.
 inline int tile_units(int gm, int gn) { return ((gm + 127) / 128) * ((gn + 63) / 64); }
 

@@ -1,14 +1,18 @@
 // Hopper (sm_90a) warpgroup-MMA GEMM core shared by the TF32 / 3xTF32 engine (tc_gemm.cu) and
 // the bf16 engine (tc_gemm_bf16.cu).
 //
-//   * a CTA owns a 128 x 128 output tile: two consumer warpgroups of 64 rows, each issuing
-//     wgmma.mma_async m64n64 instructions (two per k step for the full 128 columns);
-//   * operands go global -> registers -> shared memory, always written K-major with the
-//     128-byte swizzle that the wgmma descriptors address.  TF32 wgmma only reads K-major
-//     operands, so MN-major storage (the dW GEMMs) is transposed on that way, and the 3xTF32
-//     hi / lo split of A (and of B when it is not pre-split) happens there too;
-//   * the next k block is loaded into registers while the tensor cores work on the current
-//     one (two shared-memory stages);
+//   * a CTA owns a 128 x 128 output tile: two consumer warpgroups of 64 rows, each issuing one
+//     wgmma.mma_async m64n128 per k step (m64n64 when the tile's live columns fit in 64);
+//   * A comes from registers: each warpgroup loads its fragments from a plain (unswizzled,
+//     padded) fp32 / bf16 tile in shared memory, at transposed addresses when A is MN-major.
+//     The 3xTF32 hi / lo split of A happens there, in registers;
+//   * operands that need no arithmetic (A in both layouts, K-major B and its pre-split lo part,
+//     every bf16 B) are copied global -> shared by cp.async 16-byte copies into a ring of 3-4
+//     stages; the 128-byte swizzle of B is applied in the destination address.  bf16 MN-major
+//     B is read by the wgmma through the descriptor's transpose bit.  Only the MN-major TF32 B
+//     of the dW GEMMs (TF32 wgmma reads K-major B only) is staged through registers, where it
+//     is transposed and, for 3xTF32, split;
+//   * the copies for the next tile start before the epilogue of the current one;
 //   * the epilogue runs on the accumulator registers: bias / activation, ReLU masks (from an
 //     fp32 array or from 1-bit sign words), ReLU sign words out, per-warp column sums,
 //     row-major, transposed or split-K partial stores, fp32 or bf16 output.
@@ -19,17 +23,26 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace tfr {
 namespace wg {
 
 constexpr int BM = 128;          // rows of an output tile (two warpgroups of 64)
-constexpr int BN = 128;          // columns of an output tile (two m64n64 instructions)
+constexpr int BN = 128;          // columns of an output tile (one m64n128 instruction)
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kTileBytes = 128 * 128;   // one operand tile: 128 rows x 128 bytes of k
-constexpr int kStages = 2;
+constexpr int kTileBytes = 128 * 128;   // one swizzled B tile: 128 rows x 128 bytes of k
+// A tile: 128 rows x 128 bytes of k.  K-major rows are padded to 144 B, MN-major k rows
+// (512 B of m) to 544 B (fp32, 32 rows) / 272 B (bf16, 64 rows): either way the fragment
+// loads of a warp hit 32 different banks.
+constexpr int kAPitchK = 144;
+constexpr int kAPitchMN = 4 * (128 + 8);   // bytes per k row (fp32); bf16 uses half of it
+constexpr int kATileBytes = 128 * kAPitchK;
+constexpr int kMaxStages = 4;
+constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory of one CTA on sm_90
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 };
 
@@ -51,6 +64,23 @@ struct Args {
   float* colsum; int colsum_stride;  // slot (cta * 8 + warp): column sums of what it stored
   int colsum_cols;                   // shared-memory accumulator width (0: off)
 };
+
+// Bytes of one pipeline stage: the B tile (plus its lo tile for 3xTF32), then the A tile.
+__host__ __device__ constexpr int stage_bytes(int passes) {
+  return (passes == 3 ? 2 : 1) * kTileBytes + kATileBytes;
+}
+// Stages that fit beside the [8][colsum_cols] column-sum accumulator and the 1 KB alignment
+// slack; at most kMaxStages.  The one place that sizes the shared memory of a launch.
+__host__ __device__ constexpr int num_stages(int passes, int colsum_cols) {
+  return (kSmemLimit - 1024 - kWarps * colsum_cols * 4) / stage_bytes(passes) < kMaxStages
+             ? (kSmemLimit - 1024 - kWarps * colsum_cols * 4) / stage_bytes(passes)
+             : kMaxStages;
+}
+static_assert(num_stages(3, 1024) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
+inline size_t smem_bytes(int passes, int colsum_cols) {
+  return (size_t)num_stages(passes, colsum_cols) * stage_bytes(passes) +
+         (size_t)kWarps * colsum_cols * sizeof(float) + 1024;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -74,6 +104,16 @@ __device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
   d |= static_cast<uint64_t>(1) << 62;                 // SWIZZLE_128B
   return d;
 }
+// MN-major, 128-byte swizzle (bf16 B read with the transpose bit): 64 columns (128 B) per
+// swizzle atom, 8 k rows per 1024 B; the next 64 columns start `atom_stride` bytes further.
+__device__ __forceinline__ uint64_t desc_sw128_mn(uint32_t saddr, uint32_t atom_stride) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(atom_stride >> 4) << 16;  // leading byte offset: next 64 columns
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;         // stride byte offset: next 8 k rows
+  d |= static_cast<uint64_t>(1) << 62;                 // SWIZZLE_128B
+  return d;
+}
 
 __device__ __forceinline__ void wgmma_fence() {
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
@@ -89,9 +129,27 @@ __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// 16-byte global -> shared copy; the `bytes` (0..16) first bytes are read, the rest zero-filled.
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() {
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
 #define TFR_WG_D32                                                                           \
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, "  \
   "%19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define TFR_WG_D64                                                                           \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, "  \
+  "%19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, "   \
+  "%36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, "   \
+  "%53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
 #define TFR_WG_OUT32(d)                                                                      \
   "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),       \
       "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]),             \
@@ -99,120 +157,93 @@ __device__ __forceinline__ void fence_proxy_async() {
       "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),          \
       "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
 
-// D[64 x 64] += A[64 x 8] B[8 x 64], TF32 operands (fp32 bits; the low 13 are ignored)
-__device__ __forceinline__ void mma_tf32(float (&d)[32], uint64_t da, uint64_t db) {
+// D[64 x N] += A[64 x k] B[k x N]; A: four registers of this thread's fragment, B: descriptor.
+// acc[0] holds columns 0..63, acc[1] columns 64..127 (the m64n128 accumulator layout).
+// TF32 (k = 8): fp32 bits, the low 13 are ignored.
+__device__ __forceinline__ void mma_tf32_n64(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile("wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " TFR_WG_D32
-               ", %32, %33, 1, 1, 1;"
-               : TFR_WG_OUT32(d)
-               : "l"(da), "l"(db));
+               ", {%32, %33, %34, %35}, %36, 1, 1, 1;"
+               : TFR_WG_OUT32(d[0])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
-// D[64 x 64] += A[64 x 16] B[16 x 64], bf16 operands, both K-major
-__device__ __forceinline__ void mma_bf16(float (&d)[32], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void mma_tf32_n128(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " TFR_WG_D64
+               ", {%64, %65, %66, %67}, %68, 1, 1, 1;"
+               : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+// bf16 (k = 16): two bf16 per register.  TRANS_B: B is MN-major in shared memory.
+template <int TRANS_B>
+__device__ __forceinline__ void mma_bf16_n64(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " TFR_WG_D32
-               ", %32, %33, 1, 1, 1, 0, 0;"
-               : TFR_WG_OUT32(d)
-               : "l"(da), "l"(db));
+               ", {%32, %33, %34, %35}, %36, 1, 1, 1, %37;"
+               : TFR_WG_OUT32(d[0])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
+}
+template <int TRANS_B>
+__device__ __forceinline__ void mma_bf16_n128(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " TFR_WG_D64
+               ", {%64, %65, %66, %67}, %68, 1, 1, 1, %69;"
+               : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
 }
 #undef TFR_WG_D32
+#undef TFR_WG_D64
 #undef TFR_WG_OUT32
 
-// Element traits: a 16-byte chunk holds EPC elements; a 128-byte swizzle row holds BK of k.
+// Element traits: a 16-byte chunk holds EPC elements; a 128-byte row holds BK of k.
 template <typename T> struct Elem;
 template <> struct Elem<float> { static constexpr int EPC = 4; static constexpr int BK = 32; };
 template <> struct Elem<__nv_bfloat16> { static constexpr int EPC = 8; static constexpr int BK = 64; };
 
-// One 16-byte chunk of an operand tile, zero past the matrix edge.  `p` points at the first
-// element; `n` elements of the chunk lie inside the matrix (the chunk is aligned when n == EPC).
-template <typename T>
-__device__ __forceinline__ uint4 load_chunk(const T* p, int n) {
-  constexpr int EPC = Elem<T>::EPC;
-  if (n >= EPC) return __ldg(reinterpret_cast<const uint4*>(p));
-  union { uint4 v; T e[EPC]; } u;
-  u.v = make_uint4(0u, 0u, 0u, 0u);
-  for (int i = 0; i < n; ++i) u.e[i] = p[i];
-  return u.v;
-}
+// Byte offset of 16-byte chunk `kc` of row `row` in a K-major 128B-swizzled tile.
+__device__ __forceinline__ int swz_chunk(int row, int kc) { return row * 128 + (((kc ^ row) & 7) << 4); }
 
-// Byte offset of element (row, k) in a K-major 128B-swizzled tile (row pitch 128 B).
-template <typename T>
-__device__ __forceinline__ int swz(int row, int k) {
-  const int byte = k * static_cast<int>(sizeof(T));
-  return row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15);
-}
-
-// Chunk i (0..3) of this thread in an MN-major tile ([k][rows], rows contiguous): a warp takes
-// 8 consecutive row chunks (one 128-byte line per k row) of 4 consecutive k rows.  Spreading a
-// warp over k keeps the scalar K-major stores of the transpose on 4 (TF32) / 8 (bf16) ways of
-// bank conflict instead of 16: within one k row every lane's rows share their swizzle phase.
-template <typename T>
-__device__ __forceinline__ void mn_chunk(int i, int& k, int& r) {
-  constexpr int EPC = Elem<T>::EPC, RG = 128 / EPC / 8;   // groups of 8 row chunks
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  k = (lane >> 3) + 4 * (warp / RG) + (Elem<T>::BK / 4) * i;
-  r = ((lane & 7) + 8 * (warp % RG)) * EPC;
-}
-
-// Register-staged operand tile: 128 rows (m or n) x BK of k, 4 chunks per thread.
-//   MN == false: stored [rows][k] (k contiguous); chunk c = row * 8 + k chunk
-//   MN == true : stored [k][rows] (rows contiguous); chunks as in mn_chunk
-template <typename T, bool MN>
-struct Tile {
-  uint4 v[4];
-  __device__ __forceinline__ void load(const T* base, int ld, int r0, int rows, int k0, int ks) {
-    constexpr int EPC = Elem<T>::EPC;
+// The register-staged operand: an MN-major fp32 B tile ([k][n], n contiguous) of 128 columns
+// x 32 k, transposed into the K-major swizzled tile(s) and, for 3xTF32, split into hi / lo.
+// A warp takes 8 consecutive column chunks (one 128-byte line per k row) of 4 consecutive k
+// rows: within one k row every lane's columns share their swizzle phase, which keeps the
+// scalar K-major stores on 4 ways of bank conflict instead of 16.
+struct BTileMN {
+  float4 v[4];
+  __device__ __forceinline__ static void chunk(int i, int& k, int& r) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    k = (lane >> 3) + 4 * (warp / 4) + 8 * i;
+    r = ((lane & 7) + 8 * (warp % 4)) * 4;
+  }
+  __device__ __forceinline__ void load(const float* base, int ld, int r0, int rows, int k0, int ks) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int c = threadIdx.x + i * kThreads;
-      if (!MN) {
-        const int r = c >> 3, k = (c & 7) * EPC;
-        const int n = (r < rows) ? min(EPC, ks - (k0 + k)) : 0;
-        v[i] = n > 0 ? load_chunk(base + static_cast<size_t>(r0 + r) * ld + k0 + k, n)
-                     : make_uint4(0u, 0u, 0u, 0u);
+      int k, r;
+      chunk(i, k, r);
+      const int n = (k0 + k < ks) ? min(4, rows - r) : 0;
+      const float* p = base + static_cast<size_t>(k0 + k) * ld + r0 + r;
+      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (n >= 4) {
+        v[i] = __ldg(reinterpret_cast<const float4*>(p));
       } else {
-        int k, r;
-        mn_chunk<T>(i, k, r);
-        const int n = (k0 + k < ks) ? min(EPC, rows - r) : 0;
-        v[i] = n > 0 ? load_chunk(base + static_cast<size_t>(k0 + k) * ld + r0 + r, n)
-                     : make_uint4(0u, 0u, 0u, 0u);
+        if (n > 0) v[i].x = p[0];
+        if (n > 1) v[i].y = p[1];
+        if (n > 2) v[i].z = p[2];
       }
     }
   }
-  // Write into the K-major swizzled tile(s).  SPLIT: hi = RN-TF32(x) to `hi`, x - hi to `lo`.
   template <bool SPLIT>
   __device__ __forceinline__ void store(unsigned char* hi, unsigned char* lo) const {
-    constexpr int EPC = Elem<T>::EPC;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int c = threadIdx.x + i * kThreads;
-      union { uint4 v; T e[EPC]; } u;
-      u.v = v[i];
-      if (!MN) {
-        const int r = c >> 3, k = (c & 7) * EPC;
-        const int off = swz<T>(r, k);
-        if (SPLIT) {
-          float4 h, l;
-          const float4 x = *reinterpret_cast<const float4*>(&u.v);
-          h.x = tf32_rn(x.x); h.y = tf32_rn(x.y); h.z = tf32_rn(x.z); h.w = tf32_rn(x.w);
-          l.x = x.x - h.x; l.y = x.y - h.y; l.z = x.z - h.z; l.w = x.w - h.w;
-          *reinterpret_cast<float4*>(hi + off) = h;
-          *reinterpret_cast<float4*>(lo + off) = l;
-        } else {
-          *reinterpret_cast<uint4*>(hi + off) = u.v;
-        }
-      } else {
-        int k, r;
-        mn_chunk<T>(i, k, r);
+      int k, r;
+      chunk(i, k, r);
+      const float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
 #pragma unroll
-        for (int e = 0; e < EPC; ++e) {
-          const int off = swz<T>(r + e, k);
-          if (SPLIT) {
-            const float x = static_cast<float>(u.e[e]);
-            const float h = tf32_rn(x);
-            *reinterpret_cast<float*>(hi + off) = h;
-            *reinterpret_cast<float*>(lo + off) = x - h;
-          } else {
-            *reinterpret_cast<T*>(hi + off) = u.e[e];
-          }
+      for (int j = 0; j < 4; ++j) {
+        const int off = swz_chunk(r + j, k >> 2) + (k & 3) * 4;
+        if (SPLIT) {
+          const float h = tf32_rn(e[j]);
+          *reinterpret_cast<float*>(hi + off) = h;
+          *reinterpret_cast<float*>(lo + off) = e[j] - h;
+        } else {
+          *reinterpret_cast<float*>(hi + off) = e[j];
         }
       }
     }
@@ -227,17 +258,25 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 
 // PASSES: 1 (one product) or 3 (3xTF32: Ahi Bhi + Alo Bhi + Ahi Blo; float only).
 // PRE_B: B comes pre-split (B = hi parts, B_lo = lo parts).  OUT_BF16: C is bf16 (row-major).
-// Shared memory: kStages x {A hi, A lo, B hi, B lo} tiles, then [8][colsum_cols] floats.
+// Shared memory: num_stages x {B hi, [B lo,] A}, then [8][colsum_cols] floats.
 template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
 __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
+  constexpr bool F32 = sizeof(T) == 4;
+  constexpr int EPC = Elem<T>::EPC;
   constexpr int BK = Elem<T>::BK;
-  constexpr int KSTEP = sizeof(T) == 4 ? 8 : 16;   // k of one wgmma
+  constexpr int KSTEP = F32 ? 8 : 16;   // k of one wgmma
+  constexpr int NKS = BK / KSTEP;
   constexpr bool P3 = PASSES == 3;
-  constexpr int kCopies = P3 ? 2 : 1;
-  constexpr int kStageBytes = 2 * kCopies * kTileBytes;
+  constexpr bool REG_B = F32 && B_MN;   // TF32 MN-major B: transposed through registers
+  constexpr int kStage = stage_bytes(PASSES);
+  constexpr int kAOff = (P3 ? 2 : 1) * kTileBytes;
+  constexpr int kAPitch = A_MN ? kAPitchMN * static_cast<int>(sizeof(T)) / 4 : kAPitchK;
+  static_assert(!P3 || F32, "3xTF32 is float only");
+  static_assert(!PRE_B || P3, "pre-split B is 3xTF32");
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* cacc = reinterpret_cast<float*>(smem + kStages * kStageBytes);
+  const int stages = num_stages(PASSES, args.colsum_cols);
+  float* cacc = reinterpret_cast<float*>(smem + stages * kStage);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2, wq = warp & 3;   // warpgroup, warp within it
@@ -247,19 +286,81 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
   const int nkb_total = (args.GK + BK - 1) / BK;
   const int tiles_mn = args.m_tiles * args.n_tiles;
   const int total = tiles_mn * args.splits;
+  const uint32_t smem_base = smem_u32(smem);
 
   for (int c = threadIdx.x; c < kWarps * args.colsum_cols; c += kThreads) cacc[c] = 0.f;
 
-  auto sA = [&](int s, int lo) { return smem + s * kStageBytes + lo * kTileBytes; };
-  auto sB = [&](int s, int lo) { return smem + s * kStageBytes + (kCopies + lo) * kTileBytes; };
+  // Issues the cp.async copies of k block kb (relative to the split) of the tile at (m0, n0)
+  // into stage s: 4 chunks of A and, unless register-staged, 4 chunks of B (and 4 of B lo).
+  auto copy_block = [&](int m0, int n0, int kb0, int kb, int s) {
+    const int k0 = (kb0 + kb) * BK;
+    const uint32_t st = smem_base + s * kStage;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = threadIdx.x + i * kThreads;
+      if (!A_MN) {   // [128 rows of m][8 chunks of k]
+        const int r = c >> 3, kc = c & 7, k = k0 + kc * EPC;
+        const int n = (m0 + r < args.GM && k < args.GK) ? min(EPC, args.GK - k) : 0;
+        const T* src = n > 0 ? A + static_cast<size_t>(m0 + r) * args.lda + k : A;
+        cp_async16(st + kAOff + r * kAPitch + kc * 16, src, n * static_cast<int>(sizeof(T)));
+      } else {       // [BK k rows][128 / EPC chunks of m]
+        const int k = c / (128 / EPC), mc = c % (128 / EPC), m = m0 + mc * EPC;
+        const int n = (k0 + k < args.GK && m < args.GM) ? min(EPC, args.GM - m) : 0;
+        const T* src = n > 0 ? A + static_cast<size_t>(k0 + k) * args.lda + m : A;
+        cp_async16(st + kAOff + k * kAPitch + mc * 16, src, n * static_cast<int>(sizeof(T)));
+      }
+    }
+    if (!B_MN) {     // [128 rows of n][8 chunks of k], swizzled
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = threadIdx.x + i * kThreads;
+        const int r = c >> 3, kc = c & 7, k = k0 + kc * EPC;
+        const int n = (n0 + r < args.GN && k < args.GK) ? min(EPC, args.GK - k) : 0;
+        const size_t off = n > 0 ? static_cast<size_t>(n0 + r) * args.ldb + k : 0;
+        cp_async16(st + swz_chunk(r, kc), B + off, n * static_cast<int>(sizeof(T)));
+        if (PRE_B) cp_async16(st + kTileBytes + swz_chunk(r, kc), Blo + off, n * static_cast<int>(sizeof(T)));
+      }
+    } else if (!F32) {   // bf16 [2 atoms of 64 n][64 k rows][8 chunks of n], swizzled
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = threadIdx.x + i * kThreads;
+        const int k = c >> 4, nc = c & 15, n = n0 + nc * 8;
+        const int cnt = (k0 + k < args.GK && n < args.GN) ? min(8, args.GN - n) : 0;
+        const T* src = cnt > 0 ? B + static_cast<size_t>(k0 + k) * args.ldb + n : B;
+        cp_async16(st + (nc >> 3) * (BK * 128) + swz_chunk(k, nc & 7), src, cnt * 2);
+      }
+    }
+  };
 
+  // cp.async groups: a tile's prologue commits stages - 1 groups (blocks 0 .. stages - 2),
+  // every k block one more (block kb + stages - 1), empty ones included, so that block kb's
+  // group is complete once at most stages - 2 younger groups are pending.
+  BTileMN tb, tbl;
+  auto load_b = [&](int n0, int kb) {
+    tb.load(reinterpret_cast<const float*>(B), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
+    if (PRE_B) tbl.load(reinterpret_cast<const float*>(Blo), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
+  };
+  auto prologue = [&](int tile) {
+    const int z = tile / tiles_mn;
+    const int r = tile - z * tiles_mn;
+    const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
+    const int kb0 = z * args.kb_per_split;
+    const int nkb = max(min(nkb_total, kb0 + args.kb_per_split) - kb0, 0);
+    for (int p = 0; p < stages - 1; ++p) {
+      if (p < nkb) copy_block(m0, n0, kb0, p, p);
+      cp_async_commit();
+    }
+    if (REG_B && nkb > 0) load_b(n0, kb0);
+  };
+
+  if (blockIdx.x < total) prologue(blockIdx.x);
   for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int z = tile / tiles_mn;
     const int r = tile - z * tiles_mn;
     const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
     const int kb0 = z * args.kb_per_split;
     const int nkb = max(min(nkb_total, kb0 + args.kb_per_split) - kb0, 0);
-    const bool two_n = n0 + 64 < args.GN;   // the second 64-column half holds live columns
+    const bool two_n = n0 + 64 < args.GN;           // the second 64 columns hold live columns
 
     float acc[2][32];
 #pragma unroll
@@ -267,59 +368,142 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
 
-    Tile<T, A_MN> ta;
-    Tile<T, B_MN> tb, tbl;
-    auto load = [&](int kb) {
-      const int k0 = (kb0 + kb) * BK;
-      ta.load(A, args.lda, m0, args.GM - m0, k0, args.GK);
-      tb.load(B, args.ldb, n0, args.GN - n0, k0, args.GK);
-      if (PRE_B) tbl.load(Blo, args.ldb, n0, args.GN - n0, k0, args.GK);
-    };
-    if (nkb > 0) load(0);
+    int s = 0;
     for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % kStages;
-      // the wgmma groups that read this stage (issued kStages k blocks ago) have retired in
-      // every warpgroup once all threads pass this barrier
-      __syncthreads();
-      ta.template store<P3>(sA(s, 0), sA(s, 1));
-      if (PRE_B) {
-        tb.template store<false>(sB(s, 0), nullptr);
-        tbl.template store<false>(sB(s, 1), nullptr);
-      } else {
-        tb.template store<P3>(sB(s, 0), sB(s, 1));
-      }
-      fence_proxy_async();   // generic-proxy stores -> visible to the tensor cores
-      __syncthreads();
-      if (kb + 1 < nkb) load(kb + 1);   // in flight while the tensor cores run
-      // a K tail that is no multiple of BK is zero-filled: skip its all-zero k steps
-      const int krem = args.GK - (kb0 + kb) * BK;
-      const int ksteps = krem >= BK ? BK / KSTEP : (krem + KSTEP - 1) / KSTEP;
-      const uint32_t a_hi = smem_u32(sA(s, 0)) + wg * 64 * 128, a_lo = a_hi + kTileBytes;
-      const uint32_t b_hi = smem_u32(sB(s, 0)), b_lo = b_hi + kTileBytes;
-      wgmma_fence();
-#pragma unroll 1
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const uint32_t kofs = ks * 32;   // 32 bytes of k per wgmma
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (h == 1 && !two_n) break;
-          const uint64_t dah = desc_sw128(a_hi + kofs);
-          const uint64_t dbh = desc_sw128(b_hi + h * 64 * 128 + kofs);
-          if (sizeof(T) == 4) {
-            mma_tf32(acc[h], dah, dbh);
-            if (P3) {
-              mma_tf32(acc[h], desc_sw128(a_lo + kofs), dbh);
-              mma_tf32(acc[h], dah, desc_sw128(b_lo + h * 64 * 128 + kofs));
-            }
-          } else {
-            mma_bf16(acc[h], dah, dbh);
-          }
+      const uint32_t st = smem_base + s * kStage;
+      // stage s was last read by the MMAs of block kb - stages, retired before the barrier
+      // of block kb - stages + 1
+      if (REG_B) {
+        unsigned char* sb = smem + s * kStage;
+        if (PRE_B) {
+          tb.template store<false>(sb, nullptr);
+          tbl.template store<false>(sb + kTileBytes, nullptr);
+        } else {
+          tb.template store<P3>(sb, sb + kTileBytes);
         }
       }
-      wgmma_commit();
-      wgmma_wait<1>();
+      if (stages == 4) cp_async_wait<2>(); else cp_async_wait<1>();
+      if (P3 && !B_MN && !PRE_B) {   // K-major B split on the fly: each thread its own chunks
+        unsigned char* sb = smem + s * kStage;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int c = threadIdx.x + i * kThreads;
+          const int off = swz_chunk(c >> 3, c & 7);
+          const float4 x = *reinterpret_cast<const float4*>(sb + off);
+          const float4 h = make_float4(tf32_rn(x.x), tf32_rn(x.y), tf32_rn(x.z), tf32_rn(x.w));
+          *reinterpret_cast<float4*>(sb + off) = h;
+          *reinterpret_cast<float4*>(sb + kTileBytes + off) =
+              make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+        }
+      }
+      fence_proxy_async();   // cp.async and st.shared writes -> visible to the tensor cores
+      __syncthreads();
+      // refill the stage of block kb - 1, whose MMAs every warpgroup retired before the barrier
+      {
+        const int nb = kb + stages - 1;
+        if (nb < nkb) copy_block(m0, n0, kb0, nb, nb % stages);
+        cp_async_commit();
+      }
+      if (REG_B && kb + 1 < nkb) load_b(n0, kb0 + kb + 1);   // in flight while the tensor cores run
+      {
+        // a K tail that is no multiple of BK is zero-filled: skip its all-zero k steps
+        const int krem = args.GK - (kb0 + kb) * BK;
+        const int ksteps = krem >= BK ? NKS : (krem + KSTEP - 1) / KSTEP;
+        // A fragments of every k step (m64 x k, per warp 16 rows): register i holds row
+        // g + 8 (i % 2), k t + 4 (i / 2) (TF32) / k pair 2t + 8 (i / 2) (bf16)
+        const int g = lane >> 2, t = lane & 3;
+        const int row = wg * 64 + wq * 16 + g;
+        const unsigned char* sa = smem + s * kStage + kAOff;
+        uint32_t ahi[NKS][4], alo[NKS][4];
+#pragma unroll
+        for (int ks = 0; ks < NKS; ++ks) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int rr = row + 8 * (i & 1);
+            if (F32) {
+              const int k = ks * KSTEP + t + 4 * (i >> 1);
+              const float x = *reinterpret_cast<const float*>(
+                  sa + (A_MN ? k * kAPitch + rr * 4 : rr * kAPitch + k * 4));
+              if (P3) {
+                const float h = tf32_rn(x);
+                ahi[ks][i] = __float_as_uint(h);
+                alo[ks][i] = __float_as_uint(x - h);
+              } else {
+                ahi[ks][i] = __float_as_uint(x);
+              }
+            } else {
+              const int k = ks * KSTEP + 2 * t + 8 * (i >> 1);
+              if (A_MN) {
+                const uint32_t e0 = *reinterpret_cast<const unsigned short*>(sa + k * kAPitch + rr * 2);
+                const uint32_t e1 = *reinterpret_cast<const unsigned short*>(sa + (k + 1) * kAPitch + rr * 2);
+                ahi[ks][i] = e0 | (e1 << 16);
+              } else {
+                ahi[ks][i] = *reinterpret_cast<const uint32_t*>(sa + rr * kAPitch + k * 2);
+              }
+            }
+          }
+        }
+        // one wgmma group per block.  Its width and k-step count are chosen outside it so
+        // that the group is straight-line code: a branch inside makes ptxas fence every k step.
+        auto mmas = [&](auto wide, auto nk) {
+          constexpr bool W = decltype(wide)::value;
+          constexpr int NK = decltype(nk)::value;
+          // the fragments are final before the fence: keeps their computation from sinking
+          // past it, where ptxas would fence each wgmma that reads them
+#pragma unroll
+          for (int ks = 0; ks < NKS; ++ks)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              asm volatile("" : "+r"(ahi[ks][i]));
+              if (P3) asm volatile("" : "+r"(alo[ks][i]));
+            }
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < NK; ++ks) {
+            if (F32) {
+              const uint64_t dbh = desc_sw128(st + ks * 32);   // 32 bytes of k per wgmma
+              const uint64_t dbl = desc_sw128(st + kTileBytes + ks * 32);
+              if (W) {
+                mma_tf32_n128(acc, ahi[ks], dbh);
+                if (P3) {
+                  mma_tf32_n128(acc, alo[ks], dbh);
+                  mma_tf32_n128(acc, ahi[ks], dbl);
+                }
+              } else {
+                mma_tf32_n64(acc, ahi[ks], dbh);
+                if (P3) {
+                  mma_tf32_n64(acc, alo[ks], dbh);
+                  mma_tf32_n64(acc, ahi[ks], dbl);
+                }
+              }
+            } else if (B_MN) {   // 16 k rows (2 KB) per wgmma
+              const uint64_t db = desc_sw128_mn(st + ks * 2048, BK * 128);
+              if (W) mma_bf16_n128<1>(acc, ahi[ks], db);
+              else mma_bf16_n64<1>(acc, ahi[ks], db);
+            } else {
+              const uint64_t db = desc_sw128(st + ks * 32);
+              if (W) mma_bf16_n128<0>(acc, ahi[ks], db);
+              else mma_bf16_n64<0>(acc, ahi[ks], db);
+            }
+          }
+          wgmma_commit();
+        };
+        auto by_width = [&](auto nk) {
+          if (two_n) mmas(std::true_type{}, nk);
+          else mmas(std::false_type{}, nk);
+        };
+        static_assert(NKS == 4, "k steps per block");
+        if (ksteps == 4) by_width(std::integral_constant<int, 4>{});
+        else if (ksteps == 3) by_width(std::integral_constant<int, 3>{});
+        else if (ksteps == 2) by_width(std::integral_constant<int, 2>{});
+        else by_width(std::integral_constant<int, 1>{});
+        wgmma_wait<0>();
+      }
+      s = s + 1 == stages ? 0 : s + 1;
     }
-    wgmma_wait<0>();
+    // every warpgroup is done with the stages: start the next tile's copies, then the epilogue
+    __syncthreads();
+    if (tile + gridDim.x < total) prologue(tile + gridDim.x);
 
     // ---------------------------------------------------------------- epilogue ----
     // accumulator element j of half h: row = 16 wq + lane / 4 + 8 ((j / 2) % 2),
@@ -436,12 +620,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
     float* dst = args.colsum + static_cast<size_t>(blockIdx.x * kWarps + warp) * args.colsum_stride;
     for (int c = lane; c < args.GN; c += 32) dst[c] = cacc[warp * args.colsum_cols + c];
   }
-}
-
-// Shared memory of one instantiation (dynamic, including the 1 KB alignment slack).
-inline size_t smem_bytes(int passes, int colsum_cols) {
-  return (size_t)kStages * 2 * (passes == 3 ? 2 : 1) * kTileBytes +
-         (size_t)kWarps * colsum_cols * sizeof(float) + 1024;
 }
 
 // Launches the persistent grid; *ctas receives its size (column-sum slots = 8 x ctas).
