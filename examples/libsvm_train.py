@@ -4,6 +4,10 @@ list_size 100, 136 features) through `ranking_b200`.
 
   python examples/libsvm_train.py --train_path train.txt --vali_path vali.txt \
       --output_dir /tmp/out --num_train_steps 1000
+
+`--scorer gam` trains the neural additive model of examples/tf_ranking_canned_gam.py
+instead: one tower per scalar feature (`--hidden_layer_dims 16,8` for that recipe), relu,
+batch norm and `--dropout_rate`; the loss still comes from `--loss`.
 """
 import argparse
 import os
@@ -29,17 +33,25 @@ def main():
   ap.add_argument('--list_size', type=int, default=100)
   ap.add_argument('--loss', default='pairwise_logistic_loss')
   ap.add_argument('--precision', default='tf32x3')
+  ap.add_argument('--scorer', choices=('dnn', 'gam'), default='dnn')
   args = ap.parse_args()
 
   hidden = [int(h) for h in args.hidden_layer_dims.split(',')]
   x, y, info = data.load_libsvm_data(args.train_path, args.list_size, args.num_features)
   print('train:', info)
-  tower = tfr.keras.layers.create_tower(
-      hidden, 1, activation='relu', use_batch_norm=True, input_batch_norm=True,
-      dropout=args.dropout_rate, input_dim=args.num_features, precision=args.precision)
-  trainer = tfr.train.RankingTrainer(tower, tfr.keras.losses.get(args.loss),
-                                     optimizer='adagrad',
-                                     learning_rate=args.learning_rate)
+  loss = tfr.keras.losses.get(args.loss)
+  if args.scorer == 'gam':
+    tower = tfr.keras.layers.GAMLayer(args.num_features, hidden, activation='relu',
+                                      use_batch_norm=True, dropout=args.dropout_rate)
+    trainer = tfr.train.GAMRankingTrainer(tower, loss, [1] * args.num_features,
+                                          optimizer='adagrad',
+                                          learning_rate=args.learning_rate)
+  else:
+    tower = tfr.keras.layers.create_tower(
+        hidden, 1, activation='relu', use_batch_norm=True, input_batch_norm=True,
+        dropout=args.dropout_rate, input_dim=args.num_features, precision=args.precision)
+    trainer = tfr.train.RankingTrainer(tower, loss, optimizer='adagrad',
+                                       learning_rate=args.learning_rate)
   eval_fn = None
   if args.vali_path:
     vx, vy, vinfo = data.load_libsvm_data(args.vali_path, args.list_size,

@@ -383,6 +383,74 @@ int tfr_mlp_bwd(const void* X, int M, const tfr_mlp_cfg* cfg,
                 void* workspace, float* grads, int precision, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K10  neural additive ranking model: GAMLayer (keras/layers.py:591-803) over the
+ * flattened [M = B*N] rows.  Example feature f owns columns [feature_offsets[f],
+ * feature_offsets[f + 1]) of X [M, D] (D = feature_offsets[F], feature_offsets[0] = 0,
+ * width d_f in [1, 32]) and has its own tower create_tower(hidden, 1): Dense -> [BN] ->
+ * activation -> [Dropout] per hidden layer, then Dense(1); s_f = tower_f(x_f).
+ * Context feature j (input [M, context_dims[j]]) has a tower create_tower(context_hidden,
+ * F) followed by a softmax over its F outputs; w = sum_j softmax_j and
+ *   logits = sum_f s_f w_f      (with context inputs)
+ *   logits = sum_f s_f          (without; also when n_context > 0 and none are passed)
+ * Limits: F <= TFR_GAM_MAX_FEATURES, 0..4 example hidden layers of width 1..64, d_f <= 32;
+ * context towers need F <= 8 (the tower kernels' output_units limit).
+ *
+ * Flat parameter layout: example towers 0..F-1, then context towers 0..C-1; every tower's
+ * slice is exactly the tfr_mlp layout of its dims (W_0, b_0, ..., W_L, b_L, then BN
+ * gamma / beta per hidden layer).  bn_state is concatenated in the same tower order, each
+ * slice the tfr_mlp bn_state layout.  Gradients use the parameter layout.
+ * Dropout: example tower f, hidden layer d (width h) drops (row m, unit u) iff the
+ * tfr_mlp mask of the block-diagonal layer of width F*h drops element m*(F*h) + f*h + u
+ * (same seed s = dropout_seed * 0x100000001B3 + d + 1); a one-feature GAM without context
+ * therefore draws exactly the mask of the equivalent tower.  Context tower j draws the
+ * tfr_mlp mask of its own dims with dropout_seed + (j + 1) * 0xD1B54A32D192ED03.
+ * Example towers are evaluated on chip, one (row, feature) tower per thread, recomputed
+ * from X in every sweep: no per-feature hidden activation is ever written to memory.
+ * ------------------------------------------------------------------------- */
+#define TFR_GAM_MAX_FEATURES 512
+#define TFR_GAM_MAX_HIDDEN 4
+#define TFR_GAM_MAX_CONTEXT 16
+
+typedef struct {
+  int32_t n_features;                                  /* F >= 1 */
+  int32_t feature_offsets[TFR_GAM_MAX_FEATURES + 1];   /* column offsets into X, F + 1 */
+  int32_t n_hidden;                                    /* example hidden layers, 0..4 */
+  int32_t hidden[TFR_GAM_MAX_HIDDEN];                  /* shared example hidden widths */
+  int32_t n_context;                                   /* C, 0..TFR_GAM_MAX_CONTEXT */
+  int32_t context_dims[TFR_GAM_MAX_CONTEXT];           /* input width of context tower j */
+  int32_t n_context_hidden;                            /* >= 0 */
+  int32_t context_hidden[TFR_MLP_MAX_LAYERS - 1];
+  /* create_tower options, as in tfr_mlp_cfg (no input BN) */
+  int32_t activation;
+  int32_t use_batch_norm;
+  float bn_epsilon;
+  float bn_momentum;
+  float dropout;
+  int32_t training;
+  uint64_t dropout_seed;
+  float* bn_state;                                     /* device, tfr_gam_bn_state_count */
+} tfr_gam_cfg;
+
+/* 0 when the configuration is out of range (tfr_last_error says why) */
+size_t tfr_gam_param_count(const tfr_gam_cfg* cfg);
+size_t tfr_gam_bn_state_count(const tfr_gam_cfg* cfg);
+size_t tfr_gam_workspace_bytes(const tfr_gam_cfg* cfg, int M);
+
+/* X [M, D] fp32; context_host: NULL (no context) or a HOST array of n_context device
+ * pointers, context j fp32 [M, context_dims[j]].  logits [M] with the RestoreList
+ * ln(1e-10) fill where mask (uint8 [M], optional) is 0; sublogits [M, F] and subweights
+ * [C, M, F] (the per-context-tower softmax outputs) are optional. */
+int tfr_gam_fwd(const float* X, const float* const* context_host, int M,
+                const tfr_gam_cfg* cfg, const float* params, const uint8_t* mask,
+                void* workspace, float* logits, float* sublogits, float* subweights,
+                void* stream);
+/* dlogits [M] -> grads (flat, parameter layout; context towers get 0 when no context is
+ * passed).  Must follow a tfr_gam_fwd with the same inputs, cfg and workspace. */
+int tfr_gam_bwd(const float* X, const float* const* context_host, int M,
+                const tfr_gam_cfg* cfg, const float* params, const float* dlogits,
+                const uint8_t* mask, void* workspace, float* grads, void* stream);
+
+/* ---------------------------------------------------------------------------
  * K8  groupwise scoring folded into the tower (tfr.model._GroupwiseRankingModel,
  * model.py:273-421; group formation model.py:164-244 stays with the caller).
  *   X      [B * N, D] fp32 item features (NOT gathered)

@@ -28,6 +28,7 @@ DISC_INVERSE, DISC_LOG2_INVERSE, DISC_LOG1P_INVERSE, DISC_TABLE = 0, 1, 2, 3
 PREC_FP32, PREC_TF32X3, PREC_TF32, PREC_BF16 = 0, 1, 2, 3
 ACT_NONE, ACT_RELU = 0, 1
 MLP_MAX_LAYERS = 8
+GAM_MAX_FEATURES, GAM_MAX_HIDDEN, GAM_MAX_CONTEXT = 512, 4, 16
 
 
 class LambdaCfg(C.Structure):
@@ -50,6 +51,19 @@ class MlpCfg(C.Structure):
   _fields_ = [('n_dense', C.c_int32), ('dims', C.c_int32 * (MLP_MAX_LAYERS + 1)),
               ('activation', C.c_int32),
               ('use_batch_norm', C.c_int32), ('input_batch_norm', C.c_int32),
+              ('bn_epsilon', C.c_float), ('bn_momentum', C.c_float),
+              ('dropout', C.c_float), ('training', C.c_int32),
+              ('dropout_seed', C.c_uint64), ('bn_state', C.c_void_p)]
+
+
+class GamCfg(C.Structure):
+  _fields_ = [('n_features', C.c_int32),
+              ('feature_offsets', C.c_int32 * (GAM_MAX_FEATURES + 1)),
+              ('n_hidden', C.c_int32), ('hidden', C.c_int32 * GAM_MAX_HIDDEN),
+              ('n_context', C.c_int32), ('context_dims', C.c_int32 * GAM_MAX_CONTEXT),
+              ('n_context_hidden', C.c_int32),
+              ('context_hidden', C.c_int32 * (MLP_MAX_LAYERS - 1)),
+              ('activation', C.c_int32), ('use_batch_norm', C.c_int32),
               ('bn_epsilon', C.c_float), ('bn_momentum', C.c_float),
               ('dropout', C.c_float), ('training', C.c_int32),
               ('dropout_seed', C.c_uint64), ('bn_state', C.c_void_p)]
@@ -101,6 +115,11 @@ _SIGNATURES = {
     'tfr_mlp_workspace_bytes': (C.c_size_t, [C.POINTER(MlpCfg), _I]),
     'tfr_mlp_fwd': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _I, _P]),
     'tfr_mlp_bwd': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _P, _I, _P]),
+    'tfr_gam_param_count': (C.c_size_t, [C.POINTER(GamCfg)]),
+    'tfr_gam_bn_state_count': (C.c_size_t, [C.POINTER(GamCfg)]),
+    'tfr_gam_workspace_bytes': (C.c_size_t, [C.POINTER(GamCfg), _I]),
+    'tfr_gam_fwd': (_I, [_P, _P, _I, C.POINTER(GamCfg), _P, _P, _P, _P, _P, _P, _P]),
+    'tfr_gam_bwd': (_I, [_P, _P, _I, C.POINTER(GamCfg), _P, _P, _P, _P, _P, _P]),
     'tfr_circular_pad_gather': (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     'tfr_group_indices': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'tfr_group_mlp_workspace_bytes': (C.c_size_t, [C.POINTER(MlpCfg), _I, _I, _I, _I]),

@@ -1,5 +1,5 @@
-"""The scorer part of `tfr.keras.model` (keras/model.py:668-817): `Scorer`,
-`UnivariateScorer`, `DNNScorer`.
+"""The scorer part of `tfr.keras.model` (keras/model.py:668-865): `Scorer`,
+`UnivariateScorer`, `DNNScorer`, `GAMScorer`.
 
 `scorer(context_features, example_features, mask) -> [batch_size, list_size]`
 with `context_features: {name: [B, Dc]}`, `example_features: {name: [B, N, Dk]}`,
@@ -61,3 +61,26 @@ class DNNScorer(UnivariateScorer):
       kw['input_dim'] = input_layer.shape[1]
       self.tower = layers.create_tower(**kw)
     return self.tower(input_layer)
+
+
+class GAMScorer(UnivariateScorer):
+  """keras/model.py:820-865: `GAMScorer(**GAMLayer kwargs)`.  Both feature counts come
+  from the inputs; every feature is flattened and features go in sorted key order."""
+
+  def __init__(self, **gam_kwargs):
+    super().__init__()
+    self._gam_kwargs = gam_kwargs
+    self.gam = None
+
+  def _score_flattened(self, context_features, example_features):
+    context_inputs = [context_features[k].reshape(context_features[k].shape[0], -1)
+                      for k in sorted(context_features)]
+    example_inputs = [example_features[k].reshape(example_features[k].shape[0], -1)
+                      for k in sorted(example_features)]
+    if self.gam is None:   # built at first call, like a Keras layer
+      kw = dict(self._gam_kwargs)
+      kw.update(example_feature_num=len(example_inputs),
+                context_feature_num=len(context_inputs))
+      self.gam = layers.GAMLayer(**kw)
+    logits, _, _ = self.gam((example_inputs, context_inputs))
+    return logits

@@ -228,6 +228,41 @@ class GroupwiseRankingTrainer(RankingTrainer):
                                       t._precision, _C.stream()))
 
 
+class GAMRankingTrainer(RankingTrainer):
+  """Fused step for the neural additive model (GAMLayer, keras/layers.py:591-803), as in
+  the reference's canned-GAM recipe (examples/tf_ranking_canned_gam.py): example features
+  only.  `x` is dense [B, N, D] and `feature_dims` partitions D into the F features, in
+  order; `gam` is a `keras.layers.GAMLayer` (built here for those widths if it has not
+  been).  The towers run in csrc/gam.cu (tfr_gam_fwd / tfr_gam_bwd); circular padding,
+  the fused loss, the optimizer / all-reduce, fit, evaluate and checkpoints are the base
+  class's."""
+
+  def __init__(self, gam, loss, feature_dims, **kw):
+    feature_dims = [int(d) for d in feature_dims]
+    if not gam.built:
+      gam.build(feature_dims)
+    elif gam.example_dims != feature_dims:
+      raise ValueError('feature_dims %s, the GAM was built for %s' %
+                       (feature_dims, gam.example_dims))
+    super().__init__(gam, loss, **kw)
+    self.feature_dims = feature_dims
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, d = x.shape
+    if d != sum(self.feature_dims):
+      raise ValueError('x has %d features, feature_dims sum to %d' %
+                       (d, sum(self.feature_dims)))
+    _C.check(_C.lib.tfr_gam_fwd(_C.ptr(x), None, b * n, cfg, _C.ptr(self.tower.flat.data),
+                                _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores), None, None,
+                                _C.stream()))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    _C.check(_C.lib.tfr_gam_bwd(_C.ptr(x), None, b * n, cfg, _C.ptr(self.tower.flat.data),
+                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                _C.ptr(grads), _C.stream()))
+
+
 class HostBatchPipeline(object):
   """End-to-end step from HOST buffers: pinned-memory batches are copied to the
   device on a copy stream, double-buffered so the copy of batch k+1 overlaps the
