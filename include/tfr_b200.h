@@ -285,6 +285,11 @@ typedef struct {
   float* bpref_alt;
 } tfr_metric_ext;
 
+/* Shared memory per list: 8 P + 17 N + 144 bytes (P = next power of two >= N), plus 1 KB
+ * when any extended output is requested: 205,968 bytes at N = 8192, so every output works up
+ * to the 8192-item maximum on an H100 (232,448-byte opt-in limit).  The size is checked
+ * against the device's opt-in limit before any CUDA call; a list that does not fit returns
+ * TFR_INVALID_ARGUMENT with a message naming the largest list_size accepted for the call. */
 int tfr_rank_metrics_ext(const float* scores, const float* labels,
                          const float* item_w, int w_per_item,
                          const uint8_t* mask, int B, int N,
@@ -297,7 +302,10 @@ int tfr_rank_metrics_ext(const float* scores, const float* labels,
 /* Diversity metrics (metrics_impl.py:313-427, 746-823): labels [B, N, S] hold per-subtopic
  * relevance (-1 pads).  precision_ia / alpha_dcg: [B, n_topn] (alpha_dcg unnormalised:
  * divide by list_w for the reference's per-list value); list_w [B]: per-list weights
- * with relevance = [any subtopic >= 1]; raw [B, 5] scratch as in tfr_rank_metrics. */
+ * with relevance = [any subtopic >= 1]; raw [B, 5] scratch as in tfr_rank_metrics.
+ * Shared memory per list: 8 P + 17 N + 4 S + 1,168 bytes: at most 222,352 bytes at N = 8192,
+ * S = 4096, so every N <= 8192 and S <= 4096 fits an H100; checked and rejected like
+ * tfr_rank_metrics_ext on devices with less. */
 int tfr_div_metrics(const float* scores, const float* labels, const float* item_w,
                     int w_per_item, const uint8_t* mask, int B, int N, int S,
                     const int32_t* topns_host, int n_topn, float alpha,

@@ -1,4 +1,5 @@
 // C-ABI glue: error string, scorer-tower dispatch, fused optimizer.
+#include <atomic>
 #include <cstring>
 
 #include "common.cuh"
@@ -27,6 +28,28 @@ int num_sms() {
       return 132;   // no device to ask (e.g. planning on a CPU-only build machine)
   }
   return n;
+}
+
+size_t smem_optin_limit() {
+  // one cached value per device ordinal; racing first calls store the same value
+  constexpr int kMaxDevices = 64;
+  static std::atomic<size_t> cache[kMaxDevices];
+  int dev = 0, v = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 48 * 1024;   // no device to ask: the limit every device grants without opt-in
+  }
+  if (dev >= 0 && dev < kMaxDevices) {
+    const size_t hit = cache[dev].load(std::memory_order_relaxed);
+    if (hit != 0) return hit;
+  }
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+      v <= 0) {
+    (void)cudaGetLastError();
+    return 48 * 1024;
+  }
+  if (dev >= 0 && dev < kMaxDevices) cache[dev].store((size_t)v, std::memory_order_relaxed);
+  return (size_t)v;
 }
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

@@ -15,6 +15,9 @@ namespace tfr {
 void set_error(const char* fmt, ...);
 void count_launch();   // bumps the host-side launch counter (tfr_launch_count)
 int num_sms();         // SM count of the current device; 132 (H100 SXM) when none can be queried
+// Opt-in dynamic shared memory per block of the current device (232,448 bytes on H100), queried
+// once per device ordinal; 48 KB when no device can be queried.
+size_t smem_optin_limit();
 
 #define TFR_REQUIRE(cond, ...)              \
   do {                                      \
@@ -24,10 +27,13 @@ int num_sms();         // SM count of the current device; 132 (H100 SXM) when no
     }                                       \
   } while (0)
 
+// A failed API call also leaves its error as the runtime's last error; it is cleared here so
+// that the next launch's TFR_LAUNCH_OK does not report it again.
 #define TFR_CUDA_OK(expr)                                                  \
   do {                                                                     \
     cudaError_t _e = (expr);                                               \
     if (_e != cudaSuccess) {                                               \
+      (void)cudaGetLastError();                                            \
       ::tfr::set_error("%s failed: %s (%s:%d)", #expr,                     \
                        cudaGetErrorString(_e), __FILE__, __LINE__);        \
       return TFR_CUDA_ERROR;                                               \

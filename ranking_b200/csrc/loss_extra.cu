@@ -90,6 +90,11 @@ circle_loss_kernel(const float* __restrict__ scores, const float* __restrict__ l
 // order): u_k = c_r x_k - D_k over valid k, c_r = n_valid - 1 - 2 r, D_k = sum_j |x_k - x_j|;
 // P[r, :] = softmax(u).  MODE 0: cross entropy against the same construction on the labels;
 // MODE 1: - sum_r disc(r + 1) sum_k P[r, k] gain_k / maxDCG.
+// c_r x_k and D_k grow with N (to ~4e4 at N = 4000 for unit-scale scores) while the softmax
+// only sees u_k - max_k u_k, which is O(1) where P is not 0 or 1: in fp32 the exponent would
+// carry ~1 ulp(4e4) = 4e-3 of rounding error.  D is therefore accumulated in fp64 and every
+// exponent c_r x_k - D_k - max is formed in fp64 (exact product and difference of fp32 inputs)
+// before the fp32 expf.
 // ---------------------------------------------------------------------------
 template <int MODE>
 __global__ void __launch_bounds__(kLossThreads)
@@ -101,14 +106,13 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const ListView v = carve(smem_raw, N);
   float* ext = reinterpret_cast<float*>(smem_raw + ((list_smem_bytes(N) + 15) & ~(size_t)15));
-  float* D = ext;            // [N] sum_j |s_k - s_j|
-  float* DL = ext + N;       // [N] same on the labels (MODE 0) / gains (MODE 1)
-  float* rmx = ext + 2 * N;  // [N] row max of u
-  float* rZ = ext + 3 * N;   // [N] row sum of exp(u - max)
-  float* tmx = ext + 4 * N;  // [N] (MODE 0) the same for the label rows
-  float* tZ = ext + 5 * N;
-  float* rA = ext + 6 * N;   // [N] sum_k g[r, k] P[r, k]
-  float* rc = ext + 7 * N;   // [N] c_r of the row owned by item i (by item index)
+  double* D = reinterpret_cast<double*>(ext);   // [N] sum_j |s_k - s_j| (fp64: see above)
+  float* DL = ext + 2 * N;   // [N] same on the labels (MODE 0) / gains (MODE 1)
+  float* rmx = ext + 3 * N;  // [N] row max of u
+  float* rZ = ext + 4 * N;   // [N] row sum of exp(u - max)
+  float* tmx = ext + 5 * N;  // [N] (MODE 0) the same for the label rows
+  float* tZ = ext + 6 * N;
+  float* rA = ext + 7 * N;   // [N] sum_k g[r, k] P[r, k]
   float* H = v.g;            // [N] column sums of G
   float* C = v.disc;         // [N] column sums of c_r G
   int* cum = v.rank;         // [N] 1-based index among the valid items
@@ -158,20 +162,28 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
   float* gain = DL;   // MODE 1: safe default gains (losses_impl.py:33-49)
   for (int k = tid; k < N; k += blockDim.x) {
     const float sk = v.z[k], lk = v.l[k];
-    float d = 0.f, dl = 0.f;
+    double d = 0.0;
+    float dl = 0.f;
     if (v.mv[k]) {
       for (int j = 0; j < N; ++j)
         if (v.mv[j]) {
-          d += fabsf(sk - v.z[j]);
+          d += fabs((double)sk - (double)v.z[j]);
           dl += fabsf(lk - v.l[j]);
         }
     }
     D[k] = d;
     if (MODE == 0) DL[k] = dl;
     else gain[k] = exp2f(lk - lmax) - exp2f(-lmax);
-    rc[k] = (float)(nv + 1 - 2 * cum[k]);
   }
   __syncthreads();
+  // c_r of the row owned by item i, and the fp64 exponent of entry (row c, column k)
+  auto rc = [&](int i) { return (float)(nv + 1 - 2 * cum[i]); };
+  auto u_of = [&](float c, int k, float mx) {
+    return (float)((double)c * (double)v.z[k] - D[k] - (double)mx);
+  };
+  auto t_of = [&](float c, int k, float mt) {
+    return (float)((double)c * (double)v.l[k] - (double)DL[k] - (double)mt);
+  };
   float inv_max_dcg = 0.f;
   if (MODE == 1) {
     // ideal DCG of the safe gains (all N cleaned labels, discount 1 / log1p(rank))
@@ -184,18 +196,18 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
   // pass 1 (thread per row): softmax statistics of the score row (and the label row)
   for (int i = tid; i < N; i += blockDim.x) {
     if (!v.mv[i]) continue;
-    const float c = rc[i];
+    const float c = rc(i);
     float mx = -CUDART_INF_F, mt = -CUDART_INF_F;
     for (int k = 0; k < N; ++k)
       if (v.mv[k]) {
-        mx = fmaxf(mx, c * v.z[k] - D[k]);
-        if (MODE == 0) mt = fmaxf(mt, c * v.l[k] - DL[k]);
+        mx = fmaxf(mx, u_of(c, k, 0.f));
+        if (MODE == 0) mt = fmaxf(mt, t_of(c, k, 0.f));
       }
     float Z = 0.f, Zt = 0.f;
     for (int k = 0; k < N; ++k)
       if (v.mv[k]) {
-        Z += expf(c * v.z[k] - D[k] - mx);
-        if (MODE == 0) Zt += expf(c * v.l[k] - DL[k] - mt);
+        Z += expf(u_of(c, k, mx));
+        if (MODE == 0) Zt += expf(t_of(c, k, mt));
       }
     rmx[i] = mx;
     rZ[i] = Z;
@@ -210,14 +222,14 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
   float part = 0.f;
   for (int i = tid; i < N; i += blockDim.x) {
     if (!v.mv[i]) continue;
-    const float c = rc[i], mx = rmx[i], iz = 1.f / rZ[i];
+    const float c = rc(i), mx = rmx[i], iz = 1.f / rZ[i];
     float A = 0.f, term = 0.f;
     if (MODE == 0) {
       const float mt = tmx[i], izt = 1.f / tZ[i];
       for (int k = 0; k < N; ++k)
         if (v.mv[k]) {
-          const float P = expf(c * v.z[k] - D[k] - mx) * iz;
-          const float T = expf(c * v.l[k] - DL[k] - mt) * izt;
+          const float P = expf(u_of(c, k, mx)) * iz;
+          const float T = expf(t_of(c, k, mt)) * izt;
           term -= T * logf(1e-20f + P);
           A -= T * P / (1e-20f + P);
         }
@@ -228,7 +240,7 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
       const float disc = 1.f / log1pf((float)cum[i]);
       float gs = 0.f;
       for (int k = 0; k < N; ++k)
-        if (v.mv[k]) gs += expf(c * v.z[k] - D[k] - mx) * iz * gain[k];
+        if (v.mv[k]) gs += expf(u_of(c, k, mx)) * iz * gain[k];
       part -= disc * gs * inv_max_dcg;
       A = -disc * inv_max_dcg * gs;
     }
@@ -241,14 +253,13 @@ neural_sort_loss_kernel(const float* __restrict__ scores, const float* __restric
     for (int k = tid; k < N; k += blockDim.x) {
       float h = 0.f, cc = 0.f;
       if (v.mv[k]) {
-        const float sk = v.z[k], lk = v.l[k], dk = D[k];
         for (int i = 0; i < N; ++i) {
           if (!v.mv[i]) continue;
-          const float c = rc[i];
-          const float P = expf(c * sk - dk - rmx[i]) / rZ[i];
+          const float c = rc(i);
+          const float P = expf(u_of(c, k, rmx[i])) / rZ[i];
           float g;
           if (MODE == 0) {
-            const float T = expf(c * lk - DL[k] - tmx[i]) / tZ[i];
+            const float T = expf(t_of(c, k, tmx[i])) / tZ[i];
             g = -T * inv_nv / (1e-20f + P);
           } else {
             g = -inv_max_dcg * gain[k] / log1pf((float)cum[i]);
@@ -311,8 +322,18 @@ extern "C" int tfr_extra_loss_fwd_bwd(const float* scores, const float* labels,
     circle_loss_kernel<<<B, kLossThreads, base, st>>>(scores, labels, item_w, w_per_item, mask, N,
                                                       p0, p1, grad_scale, grad, loss, weight);
   } else {
-    const size_t smem = base + (size_t)8 * N * sizeof(float);
-    TFR_REQUIRE(smem <= 227 * 1024, "list_size %d does not fit shared memory", N);
+    auto bytes_for = [](int n) {
+      return ((list_smem_bytes(n) + 15) & ~(size_t)15) + (size_t)8 * n * sizeof(float);
+    };
+    const size_t smem = bytes_for(N), limit = smem_optin_limit();
+    if (smem > limit) {
+      int n_max = N;
+      while (n_max >= 1 && bytes_for(n_max) > limit) --n_max;
+      TFR_REQUIRE(false,
+                  "NeuralSort: list_size %d needs %zu bytes of shared memory per block but the "
+                  "device allows %zu; the largest list_size accepted is %d",
+                  N, smem, limit, n_max);
+    }
     if (kind == TFR_EXTRA_NEURAL_SORT_CE) {
       TFR_CUDA_OK(cudaFuncSetAttribute(neural_sort_loss_kernel<0>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -99,12 +99,11 @@ rank_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ 
   float* term = wg + N;                             // per-position DCG terms
   float* red = term + N;                            // [32]
   unsigned char* valid = reinterpret_cast<unsigned char*>(red + 32);
-  // extended metrics only: cleaned scores, sorted relevance / weights, scan scratch
-  float* sc = reinterpret_cast<float*>(smem_raw + (((size_t)P * 8 + (size_t)(4 * N + 32) * 4 +
-                                                    N + 15) & ~(size_t)15));
-  float* relk = sc + N;
-  float* wk = relk + N;
-  float* scratch = wk + N;                          // [blockDim.x]
+  // extended metrics only: scan scratch.  Sorted relevance and weights are read through the
+  // sort keys, and OPA's cleaned scores go to `term` once it is free, so that every output
+  // fits shared memory up to kMaxMetricListSize (rank_metrics_smem_bytes).
+  float* scratch = reinterpret_cast<float*>(
+      smem_raw + (((size_t)P * 8 + (size_t)(4 * N + 32) * 4 + N + 15) & ~(size_t)15));
   const bool want_ext = ext.any();
 
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -128,7 +127,6 @@ rank_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ 
     w[i] = wv;
     wg[i] = wv * g;
     valid[i] = ok;
-    if (want_ext) sc[i] = sc_i;
     keys[i] = ((unsigned long long)(ok ? 0 : 1) << 45) |
               ((unsigned long long)desc_bits(sc_i) << 13) | (unsigned long long)i;
     const float rel = c >= 1.f ? 1.f : 0.f;
@@ -182,9 +180,7 @@ rank_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ 
     for (int k = tid; k < N; k += blockDim.x) {
       const int idx = (int)(keys[k] & 0x1fffull);
       const float c = cl[idx];
-      relk[k] = c >= 1.f ? 1.f : 0.f;
-      wk[k] = w[idx];
-      term[k] = relk[k];                 // -> cumulative relevant count
+      term[k] = c >= 1.f ? 1.f : 0.f;    // -> cumulative relevant count
       nv += valid[k] ? 1.f : 0.f;
       a_num += (float)(k + 1) * w[idx] * c;      // ARP (:524-536)
       a_den += w[idx] * c;
@@ -205,11 +201,13 @@ rank_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ 
       const float n_irr = nv - s_r;
       const float den_trec = fminf(n_irr, s_r);
       for (int k = tid; k < cut; k += blockDim.x) {
-        rsum += relk[k];
-        msum += term[k] / (float)(k + 1) * wk[k] * relk[k];   // precision@k at relevant k
+        const int idx = (int)(keys[k] & 0x1fffull);
+        const float relk = cl[idx] >= 1.f ? 1.f : 0.f;
+        rsum += relk;
+        msum += term[k] / (float)(k + 1) * w[idx] * relk;   // precision@k at relevant k
         const float num = fminf(fminf((float)(k + 1), nv) - term[k], s_r);
-        bsum += relk[k] * (1.f - (den_trec != 0.f ? num / den_trec : 0.f));
-        bsum_alt += relk[k] * (1.f - (s_r != 0.f ? num / s_r : 0.f));
+        bsum += relk * (1.f - (den_trec != 0.f ? num / den_trec : 0.f));
+        bsum_alt += relk * (1.f - (s_r != 0.f ? num / s_r : 0.f));
       }
       rsum = block_sum(rsum, red);
       msum = block_sum(msum, red);
@@ -228,7 +226,12 @@ rank_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ 
       }
     }
     if (ext.opa) {
-      // ordered pair accuracy (:721-743): pairs (i, j) with l_i > l_j, weight w_i
+      // ordered pair accuracy (:721-743): pairs (i, j) with l_i > l_j, weight w_i.  The
+      // cleaned scores go to `term` (free again: dcg[] holds what it was needed for).
+      __syncthreads();
+      float* sc = term;
+      for (int i = tid; i < N; i += blockDim.x) sc[i] = sc_clean(valid[i], scores[off + i], pmin);
+      __syncthreads();
       float num = 0.f, den = 0.f;
       for (int i = tid; i < N; i += blockDim.x) {
         if (!valid[i]) continue;
@@ -299,8 +302,7 @@ div_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ l
   float* relcnt = w + N;                            // [N] #subtopics with l >= 1, by position
   float* term = relcnt + N;                         // [N] alphaDCG terms by position
   float* red = term + N;                            // [32]
-  int* order = reinterpret_cast<int*>(red + 32);    // [N] item index by position
-  float* topic_any = reinterpret_cast<float*>(order + N);   // [S]
+  float* topic_any = red + 32;                               // [S]
   float* cum = topic_any + S;                                // [N] scan buffer
   float* scratch = cum + N;                                  // [blockDim.x]
   unsigned char* valid = reinterpret_cast<unsigned char*>(scratch + kMetricThreads);
@@ -348,8 +350,9 @@ div_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ l
   }
   __syncthreads();
   bitonic_sort(keys, P);
+  // the item at position k is keys[k] & 0x1fff: the sorted keys stay put for the rest
+  auto order = [keys](int k) { return (int)(keys[k] & 0x1fffull); };
   for (int k = tid; k < N; k += blockDim.x) {
-    order[k] = (int)(keys[k] & 0x1fffull);
     term[k] = 0.f;
     relcnt[k] = 0.f;
   }
@@ -360,7 +363,7 @@ div_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ l
   for (int t = 0; t < S; ++t) {
     float any = 0.f;
     for (int k = tid; k < N; k += blockDim.x) {
-      const int idx = order[k];
+      const int idx = order(k);
       const float l = valid[idx] ? lab[(size_t)idx * S + t] : 0.f;
       cum[k] = l;
       any = fmaxf(any, l >= 1.f ? 1.f : 0.f);
@@ -370,7 +373,7 @@ div_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ l
     __syncthreads();
     block_inclusive_scan(cum, N, scratch);
     for (int k = tid; k < N; k += blockDim.x) {
-      const int idx = order[k];
+      const int idx = order(k);
       const float l = valid[idx] ? lab[(size_t)idx * S + t] : 0.f;
       if (l != 0.f) term[k] += l * powf(base, cum[k] - l);   // exclusive coverage
       if (l >= 1.f) relcnt[k] += 1.f;
@@ -382,7 +385,7 @@ div_metrics_kernel(const float* __restrict__ scores, const float* __restrict__ l
   nt = block_sum(nt, red);
   for (int k = tid; k < N; k += blockDim.x) {
     const float d = disc_fn == TFR_DISC_TABLE ? disc_table[k + 1] : disc_of(disc_fn, (float)(k + 1));
-    term[k] *= w[order[k]] * d;
+    term[k] *= w[order(k)] * d;
   }
   __syncthreads();
   for (int t = 0; t < topns.n; ++t) {
@@ -429,6 +432,48 @@ metric_list_weights_kernel(const float* __restrict__ raw, int B, float* __restri
   }
 }
 
+static int next_pow2(int n) {
+  int p = 1;
+  while (p < n) p <<= 1;
+  return p;
+}
+
+// Dynamic shared memory of one CTA, as carved by the kernels above.  At N = 8192 the rank
+// kernel needs 204,944 bytes (205,968 with extended outputs) and the diversity kernel
+// 205,968 + 4 S bytes: all fit the 232,448-byte opt-in limit of an H100 for every S <= 4096.
+static size_t rank_metrics_smem_bytes(int N, bool ext) {
+  const size_t P = (size_t)next_pow2(N);
+  return ((P * 8 + (size_t)(4 * N + 32) * 4 + N + 15) & ~(size_t)15) +
+         (ext ? (size_t)kMetricThreads * 4 : 0) + 16;
+}
+
+static size_t div_metrics_smem_bytes(int N, int S) {
+  return (size_t)next_pow2(N) * 8 + (size_t)(4 * N + 32 + S + kMetricThreads) * 4 + N + 16;
+}
+
+// Largest list size whose launch fits `limit` bytes (0 if none does).
+template <typename F>
+static int largest_fitting_list(F bytes_for, size_t limit) {
+  int n = kMaxMetricListSize;
+  while (n >= 1 && bytes_for(n) > limit) --n;
+  return n;
+}
+
+// Checks the launch's shared memory against the device's opt-in limit before any CUDA call,
+// then raises the kernel's limit when it needs more than the default 48 KB.
+template <typename K, typename F>
+static int prep_metric_smem(K kernel, int N, F bytes_for, const char* what) {
+  const size_t smem = bytes_for(N), limit = smem_optin_limit();
+  TFR_REQUIRE(smem <= limit,
+              "%s: list_size %d needs %zu bytes of shared memory per block but the device "
+              "allows %zu; the largest list_size accepted for this call is %d",
+              what, N, smem, limit, largest_fitting_list(bytes_for, limit));
+  if (smem > 48 * 1024)
+    TFR_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+  return TFR_OK;
+}
+
 }  // namespace tfr
 
 using namespace tfr;
@@ -453,18 +498,17 @@ extern "C" int tfr_rank_metrics_ext(const float* scores, const float* labels,
   TopnList t;
   t.n = n_topn;
   for (int i = 0; i < n_topn; ++i) t.v[i] = topns_host[i];
-  int P = 1;
-  while (P < N) P <<= 1;
+  const int P = next_pow2(N);
   MetricExt ext{};
   if (ext_host)
     ext = MetricExt{ext_host->dcg, ext_host->precision, ext_host->recall, ext_host->map,
                     ext_host->hits, ext_host->arp, ext_host->opa, ext_host->bpref,
                     ext_host->bpref_alt};
-  const size_t smem = (((size_t)P * 8 + (size_t)(4 * N + 32) * 4 + N + 15) & ~(size_t)15) +
-                      (ext.any() ? (size_t)(3 * N + kMetricThreads) * 4 : 0) + 16;
-  if (smem > 48 * 1024)
-    TFR_CUDA_OK(cudaFuncSetAttribute(rank_metrics_kernel,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const bool want_ext = ext.any();
+  auto bytes_for = [want_ext](int n) { return rank_metrics_smem_bytes(n, want_ext); };
+  int rc = prep_metric_smem(rank_metrics_kernel, N, bytes_for, "tfr_rank_metrics");
+  if (rc) return rc;
+  const size_t smem = bytes_for(N);
   cudaStream_t st = (cudaStream_t)stream;
   rank_metrics_kernel<<<B, kMetricThreads, smem, st>>>(scores, labels, item_w, w_per_item, mask,
                                                       N, P, t, gain_fn, disc_fn, gain_table,
@@ -505,12 +549,11 @@ extern "C" int tfr_div_metrics(const float* scores, const float* labels, const f
   TopnList t;
   t.n = n_topn;
   for (int i = 0; i < n_topn; ++i) t.v[i] = topns_host[i];
-  int P = 1;
-  while (P < N) P <<= 1;
-  const size_t smem = (size_t)P * 8 + (size_t)(5 * N + 32 + S + kMetricThreads) * 4 + N + 16;
-  if (smem > 48 * 1024)
-    TFR_CUDA_OK(cudaFuncSetAttribute(div_metrics_kernel,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int P = next_pow2(N);
+  auto bytes_for = [S](int n) { return div_metrics_smem_bytes(n, S); };
+  int rc = prep_metric_smem(div_metrics_kernel, N, bytes_for, "tfr_div_metrics");
+  if (rc) return rc;
+  const size_t smem = bytes_for(N);
   cudaStream_t st = (cudaStream_t)stream;
   div_metrics_kernel<<<B, kMetricThreads, smem, st>>>(scores, labels, item_w, w_per_item, mask, N,
                                                      S, P, t, alpha, disc_fn, disc_table,
