@@ -100,6 +100,15 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
 int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, const MlpPlan& p,
                      const float* params, const float* dscores, const uint8_t* mask,
                      float* ws, float* grads, int passes, cudaStream_t st);
+// Fused 3xTF32 forward of Dense first_layer .. L (mlp_tc_fused.cu): one persistent kernel,
+// bit-identical to the per-layer walk.  _ok says whether the tower fits it: no BN / dropout /
+// input BN, ReLU or no activation, Dense first_layer at most 256 wide, every later hidden
+// layer at most 128, at most 8 output units, at least one hidden layer.  Expects the
+// parameters already split.
+bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& p, int passes);
+int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
+                     const float* params, const uint8_t* mask, float* ws, float* scores,
+                     cudaStream_t st);
 
 // pieces of the CUDA-core path reused by the tensor-core path
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,

@@ -7,7 +7,8 @@
 //                                              rows split over CTAs -> partials -> reduce
 //            dZ_d-1 = (dZ_d W_d^T) * act'(H)   dZ K-major, W K-major (pre-split hi/lo)
 // The [K -> output_units] layer and the bias column sums stay on CUDA cores
-// (GEMV / reductions, HBM-bound).
+// (GEMV / reductions, HBM-bound).  The 3xTF32 forward of towers within the limits of
+// mlp_tc_fused_fwd_ok runs as one fused kernel instead (mlp_tc_fused.cu), with the same bits.
 #include "common.cuh"
 #include "mlp.h"
 #include "tc_gemm.cuh"
@@ -105,6 +106,8 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
     rc = split_params(p, params, ws, passes, st);
     if (rc) return rc;
   }
+  if (mlp_tc_fused_fwd_ok(first_layer, X, M, p, passes))
+    return mlp_tc_fused_fwd(first_layer, X, M, p, params, mask, ws, scores, st);
   const int L = p.n_dense - 1;
   const float* whi = passes == 3 ? ws + p.whi_off : params;
   const float* wlo = passes == 3 ? ws + p.wlo_off : nullptr;

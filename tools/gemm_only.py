@@ -1,7 +1,9 @@
 """Times the eight scorer GEMMs of the config-2 training step (fwd1-3, dz1-2, dw1-3) through
 the 3xTF32 engine, with the shapes, orientations and split-K counts the trainer uses, and
 prints per GEMM the time, the algorithmic TFLOP/s (2 GM GN GK) and the GB/s of the tensors it
-must move (operands read once, output and sign words written once).
+must move (operands read once, output and sign words written once).  The last line times the
+whole 3xTF32 forward of the config-2 tower (136-256-128-64-1, the fused kernel) through
+tfr_mlp_fwd: X read once; H1, H2, H3, their sign words and the scores written once.
 usage: gemm_only.py [--reps R] [--warmup W] [--out FILE.json]"""
 import argparse
 import json
@@ -95,10 +97,45 @@ def main():
           flush=True)
   total = sum(r['us'] for r in rows)
   print('total %.1f us' % total, flush=True)
+  fwd = time_tower_fwd(dev, g, args.reps, args.warmup)
+  print('tower fwd (tfr_mlp_fwd, M %d)  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s' % (
+      M, fwd['us'], fwd['tflops'], fwd['gbps']), flush=True)
   if args.out:
     with open(args.out, 'w') as f:
       json.dump(dict(device=torch.cuda.get_device_name(dev), sms=sms, reps=args.reps,
-                     gemms=rows, total_us=round(total, 2)), f, indent=1)
+                     gemms=rows, total_us=round(total, 2), tower_fwd=fwd), f, indent=1)
+
+
+def time_tower_fwd(dev, g, reps, warmup):
+  """The config-2 tower's whole 3xTF32 forward (parameter split included) at M rows."""
+  import ctypes
+  from ranking_b200.keras import layers
+  tower = layers.create_tower(DIMS[1:], 1, activation='relu', use_batch_norm=False, dropout=0,
+                              input_dim=DIMS[0], seed=0, precision='tf32x3')
+  x = torch.randn(M, DIMS[0], device=dev, generator=g)
+  ws = tower._new_workspace(M)
+  out = torch.empty(M, 1, device=dev)
+  cfg = tower._run_cfg()
+
+  def call():
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(x), M, ctypes.byref(cfg), _C.ptr(tower.flat.data),
+                                None, _C.ptr(ws), _C.ptr(out), _C.PREC_TF32X3, _C.stream()))
+  for _ in range(warmup):
+    call()
+  torch.cuda.synchronize()
+  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+  e0.record()
+  for _ in range(reps):
+    call()
+  e1.record()
+  torch.cuda.synchronize()
+  us = e0.elapsed_time(e1) * 1e3 / reps
+  dims = DIMS + [1]
+  flop = sum(2.0 * M * dims[i] * dims[i + 1] for i in range(len(dims) - 1))
+  words = sum((n + 31) // 32 for n in DIMS[1:])          # sign words per row
+  nbytes = 4 * M * (DIMS[0] + sum(DIMS[1:]) + words + 1)
+  return dict(m=M, us=round(us, 2), tflops=round(flop / us * 1e-6, 2),
+              gbps=round(nbytes / us * 1e-3, 1), bytes=nbytes, flop=flop)
 
 
 if __name__ == '__main__':
