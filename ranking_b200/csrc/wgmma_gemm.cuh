@@ -12,6 +12,7 @@
 //     B is read by the wgmma through the descriptor's transpose bit.  Only the MN-major TF32 B
 //     of the dW GEMMs (TF32 wgmma reads K-major B only) is staged through registers, where it
 //     is transposed and, for 3xTF32, split;
+//   * one wgmma group stays in flight across k blocks (two A fragment register sets);
 //   * the copies for the next tile start before the epilogue of the current one;
 //   * the epilogue runs on the accumulator registers: bias / activation, ReLU masks (from an
 //     fp32 array or from 1-bit sign words), ReLU sign words out, per-warp column sums,
@@ -332,9 +333,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
     }
   };
 
-  // cp.async groups: a tile's prologue commits stages - 1 groups (blocks 0 .. stages - 2),
-  // every k block one more (block kb + stages - 1), empty ones included, so that block kb's
-  // group is complete once at most stages - 2 younger groups are pending.
+  // cp.async groups: a tile's prologue commits stages - 2 groups (blocks 0 .. stages - 3),
+  // every k block one more (block kb + stages - 2), empty ones included, so that block kb's
+  // group is complete once at most stages - 3 younger groups are pending.
   BTileMN tb, tbl;
   auto load_b = [&](int n0, int kb) {
     tb.load(reinterpret_cast<const float*>(B), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
@@ -346,7 +347,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
     const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
     const int kb0 = z * args.kb_per_split;
     const int nkb = max(min(nkb_total, kb0 + args.kb_per_split) - kb0, 0);
-    for (int p = 0; p < stages - 1; ++p) {
+    for (int p = 0; p < stages - 2; ++p) {
       if (p < nkb) copy_block(m0, n0, kb0, p, p);
       cp_async_commit();
     }
@@ -368,11 +369,18 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
 
-    int s = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
+    // The k loop is software-pipelined one wgmma group deep: group kb is issued while group
+    // kb - 1 may still run, from its own A fragment set (kb & 1), and `wait_group 1` then
+    // retires group kb - 1.  Invariant: at the barrier of block kb every warpgroup has retired
+    // every group up to kb - 2, and group kb - 1 may still read its stage.  So the refill after
+    // that barrier goes to the stage of block kb - 2 and loads block kb + stages - 2 (copies
+    // run stages - 2 blocks ahead), and the stage of block kb, last read by group
+    // kb - stages <= kb - 3, may be written before the barrier.
+    uint32_t frag_hi[2][NKS][4], frag_lo[2][NKS][4];
+    int s = 0;   // stage of block kb
+    auto kblock = [&](int kb, auto set) {
+      constexpr int F = decltype(set)::value;   // fragment set: compile-time, stays in registers
       const uint32_t st = smem_base + s * kStage;
-      // stage s was last read by the MMAs of block kb - stages, retired before the barrier
-      // of block kb - stages + 1
       if (REG_B) {
         unsigned char* sb = smem + s * kStage;
         if (PRE_B) {
@@ -382,7 +390,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
           tb.template store<P3>(sb, sb + kTileBytes);
         }
       }
-      if (stages == 4) cp_async_wait<2>(); else cp_async_wait<1>();
+      if (stages == 4) cp_async_wait<1>(); else cp_async_wait<0>();
       if (P3 && !B_MN && !PRE_B) {   // K-major B split on the fly: each thread its own chunks
         unsigned char* sb = smem + s * kStage;
 #pragma unroll
@@ -398,10 +406,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
       }
       fence_proxy_async();   // cp.async and st.shared writes -> visible to the tensor cores
       __syncthreads();
-      // refill the stage of block kb - 1, whose MMAs every warpgroup retired before the barrier
       {
-        const int nb = kb + stages - 1;
-        if (nb < nkb) copy_block(m0, n0, kb0, nb, nb % stages);
+        const int nb = kb + stages - 2;
+        if (nb < nkb) copy_block(m0, n0, kb0, nb, s >= 2 ? s - 2 : s + stages - 2);
         cp_async_commit();
       }
       if (REG_B && kb + 1 < nkb) load_b(n0, kb0 + kb + 1);   // in flight while the tensor cores run
@@ -414,7 +421,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
         const int g = lane >> 2, t = lane & 3;
         const int row = wg * 64 + wq * 16 + g;
         const unsigned char* sa = smem + s * kStage + kAOff;
-        uint32_t ahi[NKS][4], alo[NKS][4];
+        uint32_t (&ahi)[NKS][4] = frag_hi[F];
+        uint32_t (&alo)[NKS][4] = frag_lo[F];
 #pragma unroll
         for (int ks = 0; ks < NKS; ++ks) {
 #pragma unroll
@@ -497,10 +505,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
         else if (ksteps == 3) by_width(std::integral_constant<int, 3>{});
         else if (ksteps == 2) by_width(std::integral_constant<int, 2>{});
         else by_width(std::integral_constant<int, 1>{});
-        wgmma_wait<0>();
+        wgmma_wait<1>();   // retires group kb - 1; group kb stays in flight
       }
       s = s + 1 == stages ? 0 : s + 1;
+    };
+    for (int kb = 0; kb < nkb; kb += 2) {   // unrolled by two: the fragment set is a constant
+      kblock(kb, std::integral_constant<int, 0>{});
+      if (kb + 1 < nkb) kblock(kb + 1, std::integral_constant<int, 1>{});
     }
+    wgmma_wait<0>();
     // every warpgroup is done with the stages: start the next tile's copies, then the epilogue
     __syncthreads();
     if (tile + gridDim.x < total) prologue(tile + gridDim.x);
