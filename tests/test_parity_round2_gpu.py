@@ -12,6 +12,8 @@ import math
 import pytest
 import torch
 
+from _tower_refs import _emulated_bf16_tower
+
 pytestmark = pytest.mark.gpu
 
 RTOL = 1e-5
@@ -165,40 +167,6 @@ def test_k1_sort_order_equals_counting_ranks(cuda_api, oracle_api):
 # ----------------------------------------------------------------------------
 # bf16 scorer tower (TFR_PREC_BF16, BASELINE config 3)
 # ----------------------------------------------------------------------------
-def _bf(t):
-  return t.bfloat16().double()
-
-
-def _emulated_bf16_tower(x, ws, bs, dscores, relu=True):
-  """fp64 restatement of the bf16 tower's arithmetic: bf16 inputs / weights / stored
-  activations and backward signals, exact accumulation.  Returns scores, flat grads."""
-  L = len(ws) - 1
-  h = [_bf(x)]
-  for d in range(L):
-    z = h[-1] @ _bf(ws[d]) + bs[d].double()
-    a = torch.relu(z) if relu else z
-    h.append(_bf(a))
-  scores = h[-1] @ ws[L].double() + bs[L].double()
-  grads_w, grads_b = [None] * (L + 1), [None] * (L + 1)
-  ds = dscores.double()
-  grads_w[L] = h[-1].t() @ ds
-  grads_b[L] = ds.sum(0)
-  dz_full = ds @ ws[L].double().t()
-  if relu:
-    dz_full = dz_full * (h[-1] > 0)
-  for d in range(L - 1, -1, -1):
-    grads_b[d] = dz_full.sum(0)            # column sums are taken before the bf16 rounding
-    dz = _bf(dz_full)
-    grads_w[d] = h[d].t() @ dz
-    if d > 0:
-      dz_full = dz @ _bf(ws[d]).t()
-      if relu:
-        dz_full = dz_full * (h[d] > 0)
-  flat = torch.cat([torch.cat([w.reshape(-1), b.reshape(-1)])
-                    for w, b in zip(grads_w, grads_b)])
-  return scores, flat
-
-
 @pytest.mark.parametrize('shape', [
     (300, 16, [32, 16], 1),            # small, partial tiles
     (1000, 136, [256, 128, 64], 1),    # config-2 widths
