@@ -458,6 +458,42 @@ int tfr_din_bwd(const float* X, const uint8_t* list_mask, int B, int N, const tf
                 float* grads, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K12  pooled embedding bags (tf.feature_column.embedding_column over a categorical column;
+ * Keras Embedding + a reduction over the token axis).  ids [R, T] int32, table [V, E] fp32.
+ * Bag r holds the ids ids[r, 0..T) in [0, V); -1 marks an empty slot.  Any other id (< -1 or
+ * >= V) is never read: it is skipped like -1 and counted into *bad_ids (an int device counter,
+ * optional).  With c_r the number of ids in [0, V) of bag r:
+ *   pooled_r = scale_r * sum_t table[ids[r, t]],  scale_r = 1 (SUM), 1 / c_r (MEAN),
+ *              1 / sqrt(c_r) (SQRTN); a bag with c_r = 0 pools to zeros
+ * A repeated id counts once per occurrence.
+ *   tfr_embedding_fwd  writes pooled_r into rows r * rows_per_bag .. + rows_per_bag - 1 of
+ *                      out (row pitch ldo >= E): a context bag repeated over its list
+ *                      (rows_per_bag = list_size), or one bag per row (rows_per_bag = 1); a
+ *                      column block of a wider buffer such as the tower's input.
+ *   tfr_embedding_bwd  dout rows with the same layout (pitch lddo) ->
+ *                      dtable[v] (=, or += when accumulate) sum over occurrences (r, t) of v
+ *                      of scale_r * sum_k dout[r * rows_per_bag + k].  Rows no id hit are
+ *                      written 0 (or left as they are with accumulate).  Deterministic: a
+ *                      stable radix sort of the occurrences by id, then fixed-order segment
+ *                      sums split into chunks of 128 occurrences; no float atomics, so two
+ *                      identical calls give identical bits.
+ * Limits: R * T < 2^31, V < 2^30, 1 <= E <= 1024.  workspace: tfr_embedding_workspace_bytes.
+ * ------------------------------------------------------------------------- */
+typedef enum {
+  TFR_COMBINER_SUM = 0,
+  TFR_COMBINER_MEAN = 1,
+  TFR_COMBINER_SQRTN = 2
+} tfr_combiner;
+
+size_t tfr_embedding_workspace_bytes(int R, int T, int V, int E);
+int tfr_embedding_fwd(const int32_t* ids, int R, int T, const float* table, int V, int E,
+                      int combiner, int rows_per_bag, float* out, int ldo, int* bad_ids,
+                      void* stream);
+int tfr_embedding_bwd(const int32_t* ids, int R, int T, const float* dout, int lddo,
+                      int rows_per_bag, int V, int E, int combiner, int accumulate,
+                      void* workspace, float* dtable, int* bad_ids, void* stream);
+
+/* ---------------------------------------------------------------------------
  * K10  neural additive ranking model: GAMLayer (keras/layers.py:591-803) over the
  * flattened [M = B*N] rows.  Example feature f owns columns [feature_offsets[f],
  * feature_offsets[f + 1]) of X [M, D] (D = feature_offsets[F], feature_offsets[0] = 0,
@@ -642,6 +678,47 @@ int tfr_ranking_parse(int format, const uint8_t* const* records,
                       float* context_out, float* example_out, int32_t* sizes_out,
                       uint8_t* mask_out, int n_threads);
 uint32_t tfr_masked_crc32c(const uint8_t* data, size_t n);
+
+/* Token features: bytes_list features mapped to ids through a vocabulary, as
+ * tf.feature_column.categorical_column_with_vocabulary_file / _list do.
+ *   tfr_vocab_create   tokens[i] (token_sizes[i] bytes) gets id i; a duplicate token is
+ *                      TFR_INVALID_ARGUMENT.  num_oov_buckets 0: an unknown token is id -1
+ *                      (ignored downstream); 1: it is id n (the table has n + 1 rows).  More
+ *                      buckets (Fingerprint64 hashing) are TFR_INVALID_ARGUMENT.  The object
+ *                      is a host object, read-only after creation (safe to share between
+ *                      threads); free it with tfr_vocab_destroy.
+ *   tfr_vocab_lookup   ids_out[i] = id of tokens[i]
+ *   tfr_ranking_parse_tokens
+ *                      tfr_ranking_parse plus token features: context token feature k writes
+ *                      context_ids_out[k] [B, T_k], example token feature k writes
+ *                      example_ids_out[k] [B, list_size, T_k] (HOST arrays of HOST pointers,
+ *                      T_k = max_tokens).  A bag keeps its first T_k tokens, in record order;
+ *                      the other slots hold -1, as do missing features and padded items.
+ *                      dropped_out (optional, HOST int64 [n_context_tokens +
+ *                      n_example_tokens], context features first) receives the number of
+ *                      tokens cut by the T_k limit.  A token feature with float / int64 values
+ *                      is TFR_UNSUPPORTED. */
+typedef struct {
+  const char* name;
+  int32_t max_tokens;   /* T >= 1 */
+  const void* vocab;    /* from tfr_vocab_create */
+} tfr_token_spec;
+
+int tfr_vocab_create(const char* const* tokens, const int64_t* token_sizes, int n,
+                     int num_oov_buckets, void** vocab_out);
+int tfr_vocab_destroy(void* vocab);
+int tfr_vocab_lookup(const void* vocab, const char* const* tokens, const int64_t* token_sizes,
+                     int n, int32_t* ids_out);
+int tfr_ranking_parse_tokens(int format, const uint8_t* const* records,
+                             const int64_t* record_sizes, int B, int list_size,
+                             const tfr_feature_spec* context_spec, int n_context,
+                             const tfr_feature_spec* example_spec, int n_example,
+                             const tfr_token_spec* context_tokens, int n_context_tokens,
+                             const tfr_token_spec* example_tokens, int n_example_tokens,
+                             float* context_out, float* example_out,
+                             int32_t* const* context_ids_out, int32_t* const* example_ids_out,
+                             int64_t* dropped_out, int32_t* sizes_out, uint8_t* mask_out,
+                             int n_threads);
 
 /* ---------------------------------------------------------------------------
  * Fused optimizer over the flat parameter buffer (the reference delegates to

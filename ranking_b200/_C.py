@@ -42,6 +42,13 @@ class FeatureSpec(C.Structure):
   _fields_ = [('name', C.c_char_p), ('dim', C.c_int32), ('default_value', C.c_float)]
 
 
+class TokenSpec(C.Structure):
+  _fields_ = [('name', C.c_char_p), ('max_tokens', C.c_int32), ('vocab', C.c_void_p)]
+
+
+COMBINER_SUM, COMBINER_MEAN, COMBINER_SQRTN = 0, 1, 2
+
+
 class MetricExt(C.Structure):
   _fields_ = [(k, C.c_void_p) for k in ('dcg', 'precision', 'recall', 'map', 'hits',
                                         'arp', 'opa', 'bpref', 'bpref_alt')]
@@ -119,6 +126,18 @@ _SIGNATURES = {
                                C.POINTER(FeatureSpec), _I, C.POINTER(FeatureSpec), _I, _P, _P,
                                _P, _P, _I]),
     'tfr_masked_crc32c': (C.c_uint32, [C.c_char_p, C.c_size_t]),
+    'tfr_vocab_create': (_I, [C.POINTER(C.c_char_p), C.POINTER(C.c_int64), _I, _I,
+                              C.POINTER(C.c_void_p)]),
+    'tfr_vocab_destroy': (_I, [_P]),
+    'tfr_vocab_lookup': (_I, [_P, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), _I, _P]),
+    'tfr_ranking_parse_tokens': (_I, [_I, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), _I, _I,
+                                      C.POINTER(FeatureSpec), _I, C.POINTER(FeatureSpec), _I,
+                                      C.POINTER(TokenSpec), _I, C.POINTER(TokenSpec), _I,
+                                      _P, _P, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                      _P, _P, _P, _I]),
+    'tfr_embedding_workspace_bytes': (C.c_size_t, [_I, _I, _I, _I]),
+    'tfr_embedding_fwd': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _P, _I, _P, _P]),
+    'tfr_embedding_bwd': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
     'tfr_weighted_sum': (_I, [_P, _P, _I, _F, _P, _P]),
     'tfr_mlp_param_count': (C.c_size_t, [C.POINTER(MlpCfg)]),
     'tfr_mlp_bn_state_count': (C.c_size_t, [C.POINTER(MlpCfg)]),

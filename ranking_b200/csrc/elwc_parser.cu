@@ -10,10 +10,16 @@
 //   Features { map<string, Feature> feature = 1; }   entry { string key = 1; Feature value = 2; }
 //   Feature  { oneof { BytesList bytes_list = 1; FloatList float_list = 2; Int64List int64_list = 3; } }
 //   FloatList { repeated float value = 1; }  Int64List { repeated int64 value = 1; }   (packed or not)
+//
+// Token features (bytes_list, e.g. `query_tokens` / `document_tokens` of the reference's ANTIQUE
+// examples) decode through a vocabulary into int32 id slots: [B, T] for context features,
+// [B, list_size, T] for example features, -1 in unused slots (tfr_ranking_parse_tokens).
+#include <algorithm>
 #include <atomic>
 #include <cstring>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
@@ -123,6 +129,46 @@ int parse_values(Span list, bool is_float, float* dst, int dim) {
   return n;
 }
 
+}  // namespace
+}  // namespace tfr
+
+// Token vocabulary (categorical_column_with_vocabulary_file / _list): token -> id in
+// [0, size); an unknown token maps to `size` with one OOV bucket, to -1 without.
+struct tfr_vocab_impl {
+  std::unordered_map<std::string, int32_t> ids;
+  int32_t size = 0;
+  int32_t num_oov_buckets = 0;
+  int32_t lookup(const uint8_t* p, size_t n) const {
+    auto it = ids.find(std::string(reinterpret_cast<const char*>(p), n));
+    if (it != ids.end()) return it->second;
+    return num_oov_buckets ? size : -1;
+  }
+};
+
+namespace tfr {
+namespace {
+
+// A bytes_list feature decoded into `max_tokens` id slots.
+struct TokSpec {
+  std::string name;
+  int max_tokens;
+  const tfr_vocab_impl* vocab;
+};
+
+// Where one Example (or one SequenceExample frame / context) lands: the dense row and, for
+// token feature k, the slots base[k] + row_index * max_tokens[k].
+struct Dest {
+  const std::vector<Spec>* specs;
+  float* row;
+  const std::vector<TokSpec>* toks;
+  int32_t* const* base;
+  int64_t row_index;
+  int64_t* dropped;   // per token feature: tokens past max_tokens
+  int32_t* ids(int k) const {
+    return base[k] + row_index * (*toks)[k].max_tokens;
+  }
+};
+
 // One Feature message (oneof bytes / float / int64 list) -> row[spec.offset ..].
 int parse_feature_value(Span value, const Spec& spec, float* row) {
   while (!value.done()) {
@@ -168,8 +214,54 @@ bool read_entry(Span entry, Span* key, Span* value) {
   return true;
 }
 
-// A Features message -> row (already filled with the defaults).
-int parse_features(Span features, const std::vector<Spec>& specs, float* row) {
+int find_tok(const std::vector<TokSpec>* toks, Span key) {
+  if (!toks) return -1;
+  const size_t klen = static_cast<size_t>(key.end - key.p);
+  for (size_t k = 0; k < toks->size(); ++k) {
+    const std::string& n = (*toks)[k].name;
+    if (n.size() == klen && std::memcmp(n.data(), key.p, klen) == 0) return static_cast<int>(k);
+  }
+  return -1;
+}
+
+// One Feature message of a token feature -> ids[0 .. max_tokens) (pre-filled with -1).  The
+// first max_tokens tokens are kept; the rest are counted in *dropped.  An empty float / int64
+// list is an empty bag; a non-empty one is an error.
+int parse_token_value(Span value, const TokSpec& spec, int32_t* ids, int64_t* dropped) {
+  int n = 0;
+  while (!value.done()) {
+    uint32_t f, w;
+    Span list{nullptr, nullptr};
+    uint64_t sc;
+    if (!read_field(value, &f, &w, &list, &sc)) return TFR_INVALID_ARGUMENT;
+    if (w != 2) continue;
+    if (f == 2 || f == 3) {
+      const int cnt = parse_values(list, f == 2, nullptr, 0);
+      if (cnt < 0) return TFR_INVALID_ARGUMENT;
+      if (cnt > 0) {
+        set_error("token feature '%s' is a %s; token features must be bytes_list",
+                  spec.name.c_str(), f == 2 ? "float_list" : "int64_list");
+        return TFR_UNSUPPORTED;
+      }
+      continue;
+    }
+    if (f != 1) continue;
+    while (!list.done()) {
+      Span v{nullptr, nullptr};
+      if (!read_field(list, &f, &w, &v, &sc)) return TFR_INVALID_ARGUMENT;
+      if (f != 1 || w != 2) continue;
+      if (n < spec.max_tokens)
+        ids[n] = spec.vocab->lookup(v.p, static_cast<size_t>(v.end - v.p));
+      else
+        ++*dropped;
+      ++n;
+    }
+  }
+  return TFR_OK;
+}
+
+// A Features message -> dest (already filled with the defaults).
+int parse_features(Span features, const Dest& d) {
   while (!features.done()) {
     uint32_t f, w;
     Span entry{nullptr, nullptr};
@@ -179,23 +271,29 @@ int parse_features(Span features, const std::vector<Spec>& specs, float* row) {
     Span key, value;
     if (!read_entry(entry, &key, &value)) return TFR_INVALID_ARGUMENT;
     if (!key.p || !value.p) continue;
-    const Spec* spec = find_spec(specs, key);
-    if (!spec) continue;            // feature not requested
-    const int rc = parse_feature_value(value, *spec, row);
+    const Spec* spec = find_spec(*d.specs, key);
+    if (spec) {
+      const int rc = parse_feature_value(value, *spec, d.row);
+      if (rc) return rc;
+      continue;
+    }
+    const int k = find_tok(d.toks, key);
+    if (k < 0) continue;            // feature not requested
+    const int rc = parse_token_value(value, (*d.toks)[k], d.ids(k), d.dropped + k);
     if (rc) return rc;
   }
   return TFR_OK;
 }
 
-// One serialized tf.Example { Features features = 1 } -> row.
-int parse_example(Span ex, const std::vector<Spec>& specs, float* row) {
+// One serialized tf.Example { Features features = 1 } -> dest.
+int parse_example(Span ex, const Dest& d) {
   while (!ex.done()) {
     uint32_t f, w;
     Span features{nullptr, nullptr};
     uint64_t sc;
     if (!read_field(ex, &f, &w, &features, &sc)) return TFR_INVALID_ARGUMENT;
     if (f != 1 || w != 2) continue;
-    const int rc = parse_features(features, specs, row);
+    const int rc = parse_features(features, d);
     if (rc) return rc;
   }
   return TFR_OK;
@@ -264,12 +362,53 @@ extern "C" uint32_t tfr_masked_crc32c(const uint8_t* data, size_t n) {
   return ((c >> 15) | (c << 17)) + 0xa282ead8u;   // TFRecord's masking
 }
 
-extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
-                                 const int64_t* record_sizes, int B, int list_size,
-                                 const tfr_feature_spec* context_spec, int n_context,
-                                 const tfr_feature_spec* example_spec, int n_example,
-                                 float* context_out, float* example_out, int32_t* sizes_out,
-                                 uint8_t* mask_out, int n_threads) {
+extern "C" int tfr_vocab_create(const char* const* tokens, const int64_t* token_sizes, int n,
+                                int num_oov_buckets, void** vocab_out) {
+  TFR_REQUIRE(vocab_out && n >= 0 && (n == 0 || (tokens && token_sizes)), "bad arguments");
+  TFR_REQUIRE(num_oov_buckets == 0 || num_oov_buckets == 1,
+              "num_oov_buckets=%d: only 0 (unknown tokens are ignored) or 1 (one OOV row) are "
+              "supported; more buckets need TF's Fingerprint64 hashing", num_oov_buckets);
+  *vocab_out = nullptr;
+  tfr_vocab_impl* v = new tfr_vocab_impl();
+  v->num_oov_buckets = num_oov_buckets;
+  v->ids.reserve(static_cast<size_t>(n));
+  for (int i = 0; i < n; ++i) {
+    std::string tok(tokens[i], static_cast<size_t>(token_sizes[i]));
+    if (!v->ids.emplace(tok, i).second) {
+      set_error("duplicate vocabulary token '%s' (lines %d and %d)", tok.c_str(),
+                v->ids[tok] + 1, i + 1);
+      delete v;
+      return TFR_INVALID_ARGUMENT;
+    }
+  }
+  v->size = n;
+  *vocab_out = v;
+  return TFR_OK;
+}
+
+extern "C" int tfr_vocab_destroy(void* vocab) {
+  delete static_cast<tfr_vocab_impl*>(vocab);
+  return TFR_OK;
+}
+
+extern "C" int tfr_vocab_lookup(const void* vocab, const char* const* tokens,
+                                const int64_t* token_sizes, int n, int32_t* ids_out) {
+  TFR_REQUIRE(vocab && n >= 0 && (n == 0 || (tokens && token_sizes && ids_out)), "bad arguments");
+  const tfr_vocab_impl* v = static_cast<const tfr_vocab_impl*>(vocab);
+  for (int i = 0; i < n; ++i)
+    ids_out[i] = v->lookup(reinterpret_cast<const uint8_t*>(tokens[i]),
+                           static_cast<size_t>(token_sizes[i]));
+  return TFR_OK;
+}
+
+static int parse_batch(int format, const uint8_t* const* records, const int64_t* record_sizes,
+                       int B, int list_size, const tfr_feature_spec* context_spec, int n_context,
+                       const tfr_feature_spec* example_spec, int n_example,
+                       const tfr_token_spec* context_tokens, int n_context_tokens,
+                       const tfr_token_spec* example_tokens, int n_example_tokens,
+                       float* context_out, float* example_out, int32_t* const* context_ids_out,
+                       int32_t* const* example_ids_out, int64_t* dropped_out,
+                       int32_t* sizes_out, uint8_t* mask_out, int n_threads) {
   TFR_REQUIRE(format >= TFR_FORMAT_ELWC && format <= TFR_FORMAT_SEQUENCE_EXAMPLE,
               "format %d is not a tfr_data_format", format);
   TFR_REQUIRE(records && record_sizes && B >= 0 && list_size >= 1, "bad arguments");
@@ -293,6 +432,29 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
   int dc = 0, de = 0;
   const std::vector<Spec> cspec = make_specs(context_spec, n_context, &dc);
   const std::vector<Spec> espec = make_specs(example_spec, n_example, &de);
+  TFR_REQUIRE(n_context_tokens >= 0 && n_example_tokens >= 0, "bad token feature counts");
+  TFR_REQUIRE(n_context_tokens == 0 || (context_tokens && context_ids_out),
+              "context token specs / outputs must not be NULL");
+  TFR_REQUIRE(n_example_tokens == 0 || (example_tokens && example_ids_out),
+              "example token specs / outputs must not be NULL");
+  auto make_toks = [](const tfr_token_spec* in, int n, int32_t* const* outs,
+                      std::vector<TokSpec>* out) -> int {
+    for (int i = 0; i < n; ++i) {
+      TFR_REQUIRE(in[i].max_tokens >= 1, "token feature %d has max_tokens %d", i,
+                  in[i].max_tokens);
+      TFR_REQUIRE(in[i].vocab && outs[i], "token feature %d: NULL vocabulary or output", i);
+      out->push_back(TokSpec{in[i].name ? in[i].name : "", in[i].max_tokens,
+                             static_cast<const tfr_vocab_impl*>(in[i].vocab)});
+    }
+    return TFR_OK;
+  };
+  std::vector<TokSpec> ctoks, etoks;
+  if (int rc = make_toks(context_tokens, n_context_tokens, context_ids_out, &ctoks)) return rc;
+  if (int rc = make_toks(example_tokens, n_example_tokens, example_ids_out, &etoks)) return rc;
+  const int nct = n_context_tokens, nk = n_context_tokens + n_example_tokens;
+  const bool has_ctx = dc || nct, has_ex = de || n_example_tokens;
+  // tokens dropped by truncation, per list and token feature (summed after the threads join)
+  std::vector<int64_t> dropped(static_cast<size_t>(B) * (nk ? nk : 1), 0);
 
   // one list = one independent unit of work
   auto parse_one = [&](int b) -> int {
@@ -300,12 +462,22 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
     float* crow = dc ? context_out + static_cast<size_t>(b) * dc : nullptr;
     if (crow) fill_defaults(cspec, crow);
     // padded slots are parsed from an empty Example in the reference: every feature takes
-    // its default (data.py:170-183)
+    // its default (data.py:170-183); token slots hold -1 (an empty bag)
     for (int i = 0; i < list_size && de; ++i)
       fill_defaults(espec, example_out + (static_cast<size_t>(b) * list_size + i) * de);
+    for (int k = 0; k < nct; ++k)
+      std::fill_n(context_ids_out[k] + static_cast<size_t>(b) * ctoks[k].max_tokens,
+                  ctoks[k].max_tokens, -1);
+    for (int k = 0; k < n_example_tokens; ++k)
+      std::fill_n(example_ids_out[k] + static_cast<size_t>(b) * list_size * etoks[k].max_tokens,
+                  static_cast<size_t>(list_size) * etoks[k].max_tokens, -1);
+    int64_t* drop = dropped.data() + static_cast<size_t>(b) * nk;
+    const Dest cdest{&cspec, crow, &ctoks, context_ids_out, b, drop};
     int count = 0;
     auto example_row = [&](int i) {
-      return example_out + (static_cast<size_t>(b) * list_size + i) * de;
+      const int64_t r = static_cast<int64_t>(b) * list_size + i;
+      return Dest{&espec, de ? example_out + r * de : nullptr, &etoks, example_ids_out, r,
+                  drop + nct};
     };
     auto bad_record = [&]() {
       set_error("record %d is not a valid %s", b,
@@ -323,13 +495,13 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
         if (!read_field(rec, &f, &w, &pl, &sc)) return bad_record();
         if (w != 2) continue;
         if (f == 1) {                 // one example of the list; extra ones are truncated
-          if (count < list_size && de) {
-            const int rc = parse_example(pl, espec, example_row(count));
+          if (count < list_size && has_ex) {
+            const int rc = parse_example(pl, example_row(count));
             if (rc) return rc;
           }
           ++count;
-        } else if (f == 2 && crow) {
-          const int rc = parse_example(pl, cspec, crow);
+        } else if (f == 2 && has_ctx) {
+          const int rc = parse_example(pl, cdest);
           if (rc) return rc;
         }
       }
@@ -354,12 +526,12 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
           int rc = TFR_OK;
           if (k == "serialized_context") {
             rc = for_each_bytes(value, [&](Span v) {
-              return crow ? parse_example(v, cspec, crow) : TFR_OK;
+              return has_ctx ? parse_example(v, cdest) : TFR_OK;
             });
           } else if (k == "serialized_examples") {
             rc = for_each_bytes(value, [&](Span v) {
               int r = TFR_OK;
-              if (count < list_size && de) r = parse_example(v, espec, example_row(count));
+              if (count < list_size && has_ex) r = parse_example(v, example_row(count));
               ++count;
               return r;
             });
@@ -377,8 +549,8 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
         uint64_t sc;
         if (!read_field(rec, &f, &w, &pl, &sc)) return bad_record();
         if (w != 2) continue;
-        if (f == 1 && crow) {
-          const int rc = parse_features(pl, cspec, crow);
+        if (f == 1 && has_ctx) {
+          const int rc = parse_features(pl, cdest);
           if (rc) return rc;
         } else if (f == 2) {
           while (!pl.done()) {
@@ -389,18 +561,23 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
             if (!read_entry(entry, &key, &value)) return bad_record();
             if (!key.p || !value.p) continue;
             const Spec* spec = find_spec(espec, key);
+            const int tk = spec ? -1 : find_tok(&etoks, key);
             int frame = 0;
             while (!value.done()) {           // FeatureList.feature
               Span feat{nullptr, nullptr};
               if (!read_field(value, &f, &w, &feat, &sc)) return bad_record();
               if (f != 1 || w != 2) continue;
               if (spec && frame < list_size) {
-                const int rc = parse_feature_value(feat, *spec, example_row(frame));
+                const int rc = parse_feature_value(feat, *spec, example_row(frame).row);
+                if (rc) return rc;
+              } else if (tk >= 0 && frame < list_size) {
+                const Dest d = example_row(frame);
+                const int rc = parse_token_value(feat, etoks[tk], d.ids(tk), d.dropped + tk);
                 if (rc) return rc;
               }
               ++frame;
             }
-            if (spec && frame > count) count = frame;
+            if ((spec || tk >= 0) && frame > count) count = frame;
           }
         }
       }
@@ -412,6 +589,14 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
     return TFR_OK;
   };
 
+  auto report_dropped = [&]() {
+    if (!dropped_out) return;
+    for (int k = 0; k < nk; ++k) {
+      int64_t s = 0;
+      for (int b = 0; b < B; ++b) s += dropped[static_cast<size_t>(b) * nk + k];
+      dropped_out[k] = s;
+    }
+  };
   int threads = n_threads > 0 ? n_threads : static_cast<int>(std::thread::hardware_concurrency());
   if (threads < 1) threads = 1;
   if (threads > B) threads = B;
@@ -420,6 +605,7 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
       const int rc = parse_one(b);
       if (rc) return rc;
     }
+    report_dropped();
     return TFR_OK;
   }
   // lists are handed out by an atomic counter; the first failure wins and its message
@@ -443,7 +629,33 @@ extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
       if (!m.empty()) set_error("%s", m.c_str());
     return status.load();
   }
+  report_dropped();
   return TFR_OK;
+}
+
+extern "C" int tfr_ranking_parse(int format, const uint8_t* const* records,
+                                 const int64_t* record_sizes, int B, int list_size,
+                                 const tfr_feature_spec* context_spec, int n_context,
+                                 const tfr_feature_spec* example_spec, int n_example,
+                                 float* context_out, float* example_out, int32_t* sizes_out,
+                                 uint8_t* mask_out, int n_threads) {
+  return parse_batch(format, records, record_sizes, B, list_size, context_spec, n_context,
+                     example_spec, n_example, nullptr, 0, nullptr, 0, context_out, example_out,
+                     nullptr, nullptr, nullptr, sizes_out, mask_out, n_threads);
+}
+
+extern "C" int tfr_ranking_parse_tokens(
+    int format, const uint8_t* const* records, const int64_t* record_sizes, int B,
+    int list_size, const tfr_feature_spec* context_spec, int n_context,
+    const tfr_feature_spec* example_spec, int n_example, const tfr_token_spec* context_tokens,
+    int n_context_tokens, const tfr_token_spec* example_tokens, int n_example_tokens,
+    float* context_out, float* example_out, int32_t* const* context_ids_out,
+    int32_t* const* example_ids_out, int64_t* dropped_out, int32_t* sizes_out,
+    uint8_t* mask_out, int n_threads) {
+  return parse_batch(format, records, record_sizes, B, list_size, context_spec, n_context,
+                     example_spec, n_example, context_tokens, n_context_tokens, example_tokens,
+                     n_example_tokens, context_out, example_out, context_ids_out,
+                     example_ids_out, dropped_out, sizes_out, mask_out, n_threads);
 }
 
 extern "C" int tfr_elwc_parse(const uint8_t* const* records, const int64_t* record_sizes, int B,

@@ -242,18 +242,130 @@ def encode_sequence_example(context, examples, feature_names=None):
   return _ld(1, ctx_features) + _ld(2, lists)
 
 
+class Vocabulary(object):
+  """Token -> id map of `tf.feature_column.categorical_column_with_vocabulary_file` /
+  `_list`: ids 0 .. V-1 in list (file line) order.  `num_oov_buckets=0`: an unknown token
+  gets id -1, which embedding lookups ignore; `num_oov_buckets=1`: it gets id V, so its
+  embedding table needs V + 1 rows (`num_ids`).  More buckets (TF hashes them with
+  Fingerprint64) and duplicate tokens raise ValueError.  The map lives in the native
+  decoder (tfr_vocab_create), which looks tokens up while it parses records."""
+
+  def __init__(self, tokens, num_oov_buckets=0):
+    from ranking_b200 import _C
+    toks = [t.encode() if isinstance(t, str) else bytes(t) for t in tokens]
+    n = len(toks)
+    arr = (ctypes.c_char_p * max(n, 1))(*toks)
+    lens = (ctypes.c_int64 * max(n, 1))(*[len(t) for t in toks])
+    handle = ctypes.c_void_p()
+    self._handle = None
+    _C.check(_C.lib.tfr_vocab_create(arr, lens, n, int(num_oov_buckets), ctypes.byref(handle)))
+    self._handle = handle
+    self.tokens = toks
+    self.vocabulary_size = n
+    self.num_oov_buckets = int(num_oov_buckets)
+
+  @classmethod
+  def from_list(cls, vocabulary_list, num_oov_buckets=0):
+    return cls(vocabulary_list, num_oov_buckets)
+
+  @classmethod
+  def from_file(cls, path, vocabulary_size=None, num_oov_buckets=0):
+    """One token per line (the line without its line break); `vocabulary_size` keeps the
+    first lines only and must not exceed the line count."""
+    with open(path, 'rb') as f:
+      lines = f.read().split(b'\n')
+    if lines and lines[-1] == b'':
+      lines.pop()
+    lines = [l[:-1] if l.endswith(b'\r') else l for l in lines]
+    if vocabulary_size is not None:
+      if vocabulary_size < 1 or vocabulary_size > len(lines):
+        raise ValueError('vocabulary_size %d: %s has %d tokens' %
+                         (vocabulary_size, path, len(lines)))
+      lines = lines[:vocabulary_size]
+    return cls(lines, num_oov_buckets)
+
+  @property
+  def num_ids(self):
+    """Rows an embedding table over this vocabulary needs."""
+    return self.vocabulary_size + self.num_oov_buckets
+
+  def lookup(self, tokens):
+    """ids (int32 tensor) of a sequence of str / bytes tokens."""
+    from ranking_b200 import _C
+    toks = [t.encode() if isinstance(t, str) else bytes(t) for t in tokens]
+    n = len(toks)
+    out = torch.empty(n, dtype=torch.int32)
+    arr = (ctypes.c_char_p * max(n, 1))(*toks)
+    lens = (ctypes.c_int64 * max(n, 1))(*[len(t) for t in toks])
+    _C.check(_C.lib.tfr_vocab_lookup(self._handle, arr, lens, n,
+                                     ctypes.c_void_p(out.data_ptr())))
+    return out
+
+  def __len__(self):
+    return self.vocabulary_size
+
+  def __del__(self):
+    if getattr(self, '_handle', None) is not None:
+      try:
+        from ranking_b200 import _C
+        _C.lib.tfr_vocab_destroy(self._handle)
+      except Exception:   # noqa: BLE001  (interpreter shutdown)
+        pass
+      self._handle = None
+
+
+def _token_specs(token_feature_spec):
+  """{'context': {name: (max_tokens, vocab)}, 'example': {...}} -> two (names, TokenSpec
+  array, keep-alive) triples, in the given order."""
+  from ranking_b200 import _C
+  spec = dict(token_feature_spec or {})
+  extra = set(spec) - {'context', 'example'}
+  if extra:
+    raise ValueError("token_feature_spec takes the keys 'context' and 'example', got %s" %
+                     sorted(extra))
+  out = []
+  for kind in ('context', 'example'):
+    items = list((spec.get(kind) or {}).items())
+    arr = (_C.TokenSpec * max(len(items), 1))()
+    keep = []
+    for i, (name, (max_tokens, vocab)) in enumerate(items):
+      if not isinstance(vocab, Vocabulary):
+        raise ValueError('token feature %r: the vocabulary must be a data.Vocabulary' % name)
+      if int(max_tokens) < 1:
+        raise ValueError('token feature %r: max_tokens must be >= 1' % name)
+      key = name.encode()
+      keep += [key, vocab]
+      arr[i].name = key
+      arr[i].max_tokens = int(max_tokens)
+      arr[i].vocab = vocab._handle
+    out.append(([n for n, _ in items], [int(t) for _, (t, _) in items], arr, keep))
+  return out
+
+
 def parse_from_example_list(serialized, list_size, context_feature_spec=None,
                             example_feature_spec=None, pin_memory=False, num_threads=0,
-                            data_format=EXAMPLE_LIST_WITH_CONTEXT, out=None):
+                            data_format=EXAMPLE_LIST_WITH_CONTEXT, out=None,
+                            token_feature_spec=None):
   """data.py:391-540 for dense float / int64 features.  `serialized`: a sequence of
   serialized ELWC protos; the specs map feature name -> (dim, default_value), in the
   column order wanted.  Returns dict(context [B, Dc], examples [B, list_size, De],
   sizes [B] int32, mask [B, list_size] bool) of CPU tensors.  Pass a previous result as
   `out` to decode into the same (e.g. pinned) buffers: fresh allocations are first touched
-  inside the decoder threads and the page faults serialise them."""
+  inside the decoder threads and the page faults serialise them.
+
+  Token (bytes_list) features: `token_feature_spec = {'context': {name: (max_tokens,
+  vocab)}, 'example': {name: (max_tokens, vocab)}}` with `vocab` a `Vocabulary`.  The
+  result then also holds `context_tokens` {name: int32 [B, max_tokens]}, `example_tokens`
+  {name: int32 [B, list_size, max_tokens]} (a bag's first max_tokens ids in record order,
+  -1 in the other slots, in missing features and in padded items) and `dropped_tokens`
+  {name: number of tokens cut by max_tokens}."""
   from ranking_b200 import _C
   if data_format not in _FORMATS:
     raise ValueError('Data format {} is not supported.'.format(data_format))
+  if token_feature_spec is not None:
+    return _parse_with_tokens(serialized, list_size, context_feature_spec,
+                              example_feature_spec, token_feature_spec, pin_memory,
+                              num_threads, data_format)
   records = [r if isinstance(r, bytes) else bytes(r) for r in serialized]
   b = len(records)
   carr, nc, dc, keep_c = _spec_array(context_feature_spec)
@@ -284,13 +396,56 @@ def parse_from_example_list(serialized, list_size, context_feature_spec=None,
   return {'context': ctx, 'examples': ex, 'sizes': sizes, 'mask': mask.view(torch.bool)}
 
 
+def _parse_with_tokens(serialized, list_size, context_feature_spec, example_feature_spec,
+                       token_feature_spec, pin_memory, num_threads, data_format):
+  from ranking_b200 import _C
+  records = [r if isinstance(r, bytes) else bytes(r) for r in serialized]
+  b = len(records)
+  carr, nc, dc, keep_c = _spec_array(context_feature_spec)
+  earr, ne, de, keep_e = _spec_array(example_feature_spec)
+  (cnames, ct, ctarr, keep_ct), (enames, et, etarr, keep_et) = _token_specs(token_feature_spec)
+  ptrs = (ctypes.c_char_p * max(b, 1))(*records)
+  lens = (ctypes.c_int64 * max(b, 1))(*[len(r) for r in records])
+  pin = pin_memory and torch.cuda.is_available()
+
+  def alloc(*shape, dtype=torch.float32):
+    t = torch.empty(*shape, dtype=dtype)
+    return t.pin_memory() if pin else t
+
+  ctx, ex = alloc(b, dc), alloc(b, list_size, de)
+  sizes = torch.empty(b, dtype=torch.int32)
+  mask = torch.empty(b, list_size, dtype=torch.uint8)
+  ctok = [alloc(b, t, dtype=torch.int32) for t in ct]
+  etok = [alloc(b, list_size, t, dtype=torch.int32) for t in et]
+  cptr = (ctypes.c_void_p * max(len(ctok), 1))(*[t.data_ptr() for t in ctok])
+  eptr = (ctypes.c_void_p * max(len(etok), 1))(*[t.data_ptr() for t in etok])
+  dropped = torch.zeros(max(len(ctok) + len(etok), 1), dtype=torch.int64)
+  _C.check(_C.lib.tfr_ranking_parse_tokens(
+      _FORMATS[data_format], ptrs, lens, b, int(list_size), carr, nc, earr, ne,
+      ctarr, len(ctok), etarr, len(etok),
+      ctypes.c_void_p(ctx.data_ptr()) if dc else None,
+      ctypes.c_void_p(ex.data_ptr()) if de else None, cptr, eptr,
+      ctypes.c_void_p(dropped.data_ptr()), ctypes.c_void_p(sizes.data_ptr()),
+      ctypes.c_void_p(mask.data_ptr()), int(num_threads)))
+  del keep_c, keep_e, keep_ct, keep_et
+  drops = dropped.tolist()
+  return {'context': ctx, 'examples': ex, 'sizes': sizes, 'mask': mask.view(torch.bool),
+          'context_tokens': dict(zip(cnames, ctok)),
+          'example_tokens': dict(zip(enames, etok)),
+          'dropped_tokens': dict(zip(cnames + enames, drops))}
+
+
 def elwc_batches(paths, batch_size, list_size, context_feature_spec, example_feature_spec,
-                 label_feature, drop_remainder=True, pin_memory=True):
+                 label_feature, drop_remainder=True, pin_memory=True, token_feature_spec=None):
   """Yields (x [B, list_size, Dc + De], y [B, list_size]) from TFRecord files of ELWC
   protos: context features first (repeated over the list), then the example features —
   the layout `DNNScorer` builds (keras/model.py:800-817).  `label_feature` names the
   example feature that holds the relevance label (give it the default -1 so that padded
-  slots are invalid); it is removed from x."""
+  slots are invalid); it is removed from x.
+
+  With `token_feature_spec` (see `parse_from_example_list`) it yields (x, y, tokens)
+  instead, tokens = {'context': {name: int32 [B, T]}, 'example': {name: int32
+  [B, list_size, T]}}: the batches `EmbeddingRankingTrainer` and `pipeline.fit` take."""
   ex_spec = dict(example_feature_spec)
   if label_feature not in ex_spec:
     raise ValueError('label feature %r is not in example_feature_spec' % label_feature)
@@ -309,7 +464,9 @@ def elwc_batches(paths, batch_size, list_size, context_feature_spec, example_fea
   buf = []
 
   def flush():
-    out = parse_from_example_list(buf, list_size, context_feature_spec, ex_spec)
+    out = parse_from_example_list(buf, list_size, context_feature_spec, ex_spec,
+                                  token_feature_spec=token_feature_spec,
+                                  pin_memory=pin_memory and token_feature_spec is not None)
     ex = out['examples']
     y = ex[:, :, label_col].clone()
     y = torch.where(out['mask'], y, torch.full_like(y, -1.))
@@ -320,7 +477,9 @@ def elwc_batches(paths, batch_size, list_size, context_feature_spec, example_fea
     x = feats.contiguous()
     if pin_memory and torch.cuda.is_available():
       x, y = x.pin_memory(), y.pin_memory()
-    return x, y
+    if token_feature_spec is None:
+      return x, y
+    return x, y, {'context': out['context_tokens'], 'example': out['example_tokens']}
 
   for path in ([paths] if isinstance(paths, str) else paths):
     for rec in read_tfrecords(path):

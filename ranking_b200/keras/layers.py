@@ -775,3 +775,95 @@ class DocumentInteractionAttention(torch.nn.Module):
     return {'num_heads': self.num_heads, 'head_size': self.head_size,
             'num_layers': self.num_layers, 'dropout': self.dropout,
             'input_noise_stddev': self.input_noise_stddev}
+
+
+_COMBINERS = {'sum': _C.COMBINER_SUM, 'mean': _C.COMBINER_MEAN, 'sqrtn': _C.COMBINER_SQRTN}
+
+
+class _TokenEmbeddingFn(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, ids, flat, layer):
+    r, t = ids.shape
+    out = torch.empty(r, layer.embedding_dim, dtype=torch.float32, device=ids.device)
+    bad = torch.zeros(1, dtype=torch.int32, device=ids.device)
+    _C.check(_C.lib.tfr_embedding_fwd(_C.ptr(ids), r, t, _C.ptr(flat), layer.vocab_size,
+                                      layer.embedding_dim, layer._combiner, 1, _C.ptr(out),
+                                      layer.embedding_dim, _C.ptr(bad), _C.stream()))
+    n_bad = int(bad.item())
+    if n_bad:
+      raise ValueError('%d token ids lie outside [-1, %d)' % (n_bad, layer.vocab_size))
+    ctx.layer = layer
+    ctx.save_for_backward(ids)
+    return out
+
+  @staticmethod
+  def backward(ctx, g_out):
+    ids, = ctx.saved_tensors
+    layer = ctx.layer
+    r, t = ids.shape
+    g = g_out.contiguous()
+    grads = torch.empty(layer.vocab_size * layer.embedding_dim, dtype=torch.float32,
+                        device=ids.device)
+    ws = layer._new_workspace(r, t)
+    _C.check(_C.lib.tfr_embedding_bwd(_C.ptr(ids), r, t, _C.ptr(g), layer.embedding_dim, 1,
+                                      layer.vocab_size, layer.embedding_dim, layer._combiner,
+                                      0, _C.ptr(ws), _C.ptr(grads), None, _C.stream()))
+    return None, grads, None
+
+
+class TokenEmbedding(torch.nn.Module):
+  """A pooled embedding table: `tf.feature_column.embedding_column` over a categorical
+  vocabulary column, or Keras `Embedding` followed by a reduction over the token axis
+  (examples/keras/antique_kpl_din.py:256-278).
+
+  forward(ids [..., T] int) -> [..., embedding_dim]: the combiner ('mean', 'sum' or
+  'sqrtn') of the rows of the bag's ids in [0, vocab_size); -1 marks an empty slot.  A bag
+  with no id pools to zeros (a Keras ragged reduce_mean would give NaN there).  An id that
+  occurs twice counts twice.  Any other id raises ValueError (the kernel never reads it).
+  The table is ONE flat fp32 parameter (`flat`, [vocab_size * embedding_dim] row-major),
+  initialised as Keras Embedding does, uniform(-0.05, 0.05), from a generator seeded with
+  `seed`.  Gradients flow to the table (csrc/embedding.cu, K12), not to the ids."""
+
+  def __init__(self, vocab_size, embedding_dim, combiner='mean', seed=None, device='cuda',
+               name=None):
+    super().__init__()
+    if combiner not in _COMBINERS:
+      raise ValueError('combiner must be one of %s' % sorted(_COMBINERS))
+    self.vocab_size = int(vocab_size)
+    self.embedding_dim = int(embedding_dim)
+    if self.vocab_size < 1 or self.embedding_dim < 1 or self.embedding_dim > 1024:
+      raise ValueError('need vocab_size >= 1 and 1 <= embedding_dim <= 1024')
+    self.combiner = combiner
+    self._combiner = _COMBINERS[combiner]
+    self.name = name
+    gen = torch.Generator()
+    gen.manual_seed(int(seed) if seed is not None else torch.seed())
+    table = (torch.rand(self.vocab_size * self.embedding_dim, generator=gen,
+                        dtype=torch.float64) * 0.1 - 0.05).float()
+    self.flat = torch.nn.Parameter(table.to(device))
+    self.dims = ['embedding', self.vocab_size, self.embedding_dim]
+
+  @property
+  def table(self):
+    return self.flat.view(self.vocab_size, self.embedding_dim)
+
+  def _new_workspace(self, r, t):
+    nbytes = _C.lib.tfr_embedding_workspace_bytes(r, t, self.vocab_size, self.embedding_dim)
+    if nbytes == 0:
+      raise ValueError(_C.last_error())
+    return torch.empty(nbytes, dtype=torch.uint8, device=self.flat.device)
+
+  def forward(self, ids):
+    _C.require_cuda(ids, 'TokenEmbedding ids')
+    if ids.dim() < 1:
+      raise ValueError('ids must have a token axis')
+    lead = ids.shape[:-1]
+    t = ids.shape[-1]
+    flat_ids = ids.reshape(-1, t).to(torch.int32).contiguous()
+    out = _TokenEmbeddingFn.apply(flat_ids, self.flat, self)
+    return out.reshape(*lead, self.embedding_dim)
+
+  def get_config(self):
+    return {'vocab_size': self.vocab_size, 'embedding_dim': self.embedding_dim,
+            'combiner': self.combiner}

@@ -46,9 +46,12 @@ def evaluate(trainer, batches, metric_group=None):
   group = metric_group or keras_metrics.MetricGroup.default()
   group.reset_state()
   dev = trainer.device
-  for x, y in batches:
-    x, y = x.to(dev, non_blocking=True), y.to(dev, non_blocking=True)
-    scores = trainer.predict(x, mask=(y >= 0))
+  for batch in batches:
+    x, y = batch[0].to(dev, non_blocking=True), batch[1].to(dev, non_blocking=True)
+    if len(batch) > 2:     # (x, y, tokens): token features for EmbeddingRankingTrainer
+      scores = trainer.predict(x, mask=(y >= 0), tokens=batch[2])
+    else:
+      scores = trainer.predict(x, mask=(y >= 0))
     group.update_state(y, scores)
   group.all_reduce(trainer.group)
   return group.result()
@@ -57,7 +60,8 @@ def evaluate(trainer, batches, metric_group=None):
 def fit(trainer, train_batches, num_steps, checkpoint_dir=None,
         steps_per_checkpoint=1000, eval_batches_fn=None, log_fn=print):
   """Runs `num_steps` fused training steps over `train_batches` (an iterator of host
-  or device (x, y) pairs).  With `checkpoint_dir`, resumes from `ckpt.pt` if it exists
+  or device (x, y) pairs, or (x, y, tokens) triples whose token features go to an
+  `EmbeddingRankingTrainer`).  With `checkpoint_dir`, resumes from `ckpt.pt` if it exists
   and rewrites it every `steps_per_checkpoint` steps and at the end."""
   step = 0
   ckpt = None
@@ -69,11 +73,14 @@ def fit(trainer, train_batches, num_steps, checkpoint_dir=None,
       log_fn('resumed from %s at step %d' % (ckpt, step))
   dev = trainer.device
   last = None
-  for x, y in train_batches:
+  for batch in train_batches:
     if step >= num_steps:
       break
-    x, y = x.to(dev, non_blocking=True), y.to(dev, non_blocking=True)
-    last = trainer.train_step(x, y)
+    x, y = batch[0].to(dev, non_blocking=True), batch[1].to(dev, non_blocking=True)
+    if len(batch) > 2:
+      last = trainer.train_step(x, y, tokens=batch[2])
+    else:
+      last = trainer.train_step(x, y)
     step += 1
     if ckpt and step % steps_per_checkpoint == 0:
       save_checkpoint(trainer, ckpt, step)

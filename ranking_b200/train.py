@@ -420,3 +420,221 @@ class HostBatchPipeline(object):
     pending[1].synchronize()
     losses.append(float(self.loss_host[pending[0]]))
     return losses
+
+
+class _EmbeddingScorer(object):
+  """Embedding tables + tower as one scorer with ONE flat parameter buffer: the tables first
+  (in the given order), then the tower (the modules' `flat` become views of it), so the step
+  keeps one gradient all-reduce and one optimizer launch."""
+
+  def __init__(self, tables, tower):
+    self.flat = torch.nn.Parameter(torch.cat([t.flat.data for t in tables] + [tower.flat.data]))
+    self.table_offsets = []
+    off = 0
+    for t in tables:
+      n = t.flat.numel()
+      t.flat = torch.nn.Parameter(self.flat.data[off:off + n])
+      self.table_offsets.append(off)
+      off += n
+    self.n_tables = off
+    tower.flat = torch.nn.Parameter(self.flat.data[off:])
+    self.bn_state = tower.bn_state
+    self.dims = [list(t.dims) for t in tables] + [list(tower.dims)]
+    self.use_batch_norm = tower.use_batch_norm
+    self.input_batch_norm = tower.input_batch_norm
+    self.input_dtype = torch.float32
+    self._run_cfg = tower._run_cfg
+
+
+class EmbeddingRankingTrainer(RankingTrainer):
+  """Fused step for scorers over token (text) features, the model of the reference's ANTIQUE
+  examples (examples/keras/antique_kpl_din.py:256-288, without the DIN): every token feature
+  is a bag of ids pooled through an embedding table (keras.layers.TokenEmbedding), and the
+  pooled vectors become input columns of a create_tower tower:
+
+      xe = [x | context features by sorted name | example features by sorted name]
+           x: the dense columns ([B, N, D], D >= 0); every token feature takes E columns of
+           its table; a context bag is repeated over its list, as FlattenList does
+      scores = tower(xe)                              tfr_embedding_fwd, tfr_mlp_fwd
+      loss, d loss / d scores                         fused loss kernel
+      tower gradients, d loss / d pooled columns      tfr_mlp_bwd, tfr_mlp_input_grad
+      table gradients                                 tfr_embedding_bwd (several features on
+                                                      one table accumulate)
+      optimizer                                       one launch over the shared flat buffer
+
+  `embeddings`: {table name: TokenEmbedding}; `token_features`: {'context': {feature: table
+  name}, 'example': {feature: table name}}.  Batches carry `tokens = {'context': {feature:
+  int [B, T]}, 'example': {feature: int [B, N, T]}}` (data.elwc_batches with
+  token_feature_spec).  The tower needs input_dim = D + E * (number of token features),
+  precision tf32x3 or tf32, a hidden layer and no input BN.  With BN in the tower, example id
+  rows are circularly padded like the dense rows (K9; needs T % 4 == 0), so a padded slot
+  holds a copy of a valid item's bag.  Table rows no id hit get a zero gradient: with SGD and
+  the Keras-form Adagrad that leaves them unchanged, as TF's sparse update does.  Ids outside
+  [-1, V) are skipped and counted; `check_ids()` raises if any were seen.  fit / evaluate /
+  checkpoints / data parallelism are the base class's."""
+
+  def __init__(self, embeddings, token_features, tower, loss, **kw):
+    tf = dict(token_features)
+    extra = set(tf) - {'context', 'example'}
+    if extra:
+      raise ValueError("token_features takes the keys 'context' and 'example', got %s" %
+                       sorted(extra))
+    self.table_names = sorted(embeddings)
+    tables = [embeddings[k] for k in self.table_names]
+    feats = []                     # (kind, feature, table index), in tower column order
+    for kind in ('context', 'example'):
+      for name in sorted(tf.get(kind) or {}):
+        key = tf[kind][name]
+        if key not in embeddings:
+          raise ValueError('token feature %r uses table %r, which is not in embeddings' %
+                           (name, key))
+        feats.append((kind, name, self.table_names.index(key)))
+    if not feats:
+      raise ValueError('token_features names no feature')
+    width = sum(tables[i].embedding_dim for _, _, i in feats)
+    if tower.input_dim < width:
+      raise ValueError('the tower has input_dim %d, the token features alone take %d columns' %
+                       (tower.input_dim, width))
+    if tower.precision not in ('tf32x3', 'tf32') or tower.input_batch_norm or \
+        not tower.hidden_layer_dims:
+      raise ValueError('the tower must use precision tf32x3 or tf32, have a hidden layer and '
+                       'no input BatchNormalization (its input gradient feeds the tables)')
+    self.embeddings = tables
+    self.features = feats
+    self.dense_dim = tower.input_dim - width
+    self.emb_width = width
+    self.mlp = tower
+    super().__init__(_EmbeddingScorer(tables, tower), loss, **kw)
+    self.bad_ids = torch.zeros(1, dtype=torch.int32, device=self.device)
+    self._emb_ws = None
+    self._padded = {}
+
+  def check_ids(self):
+    """Raises ValueError if a step has seen ids outside [-1, V) (host sync)."""
+    n = int(self.bad_ids.item())
+    if n:
+      raise ValueError('%d token ids lay outside [-1, vocab_size) and were skipped' % n)
+
+  def _new_workspace(self, b, n):
+    self.xe = torch.empty(b * n, self.mlp.input_dim, dtype=torch.float32, device=self.device)
+    self.d_emb = torch.empty(b * n, self.emb_width, dtype=torch.float32, device=self.device)
+    return self.mlp._new_workspace(b * n)
+
+  def _set_tokens(self, tokens, b, n):
+    if tokens is None:
+      raise ValueError('EmbeddingRankingTrainer needs the token features of the batch')
+    ids = []
+    for kind, name, _ in self.features:
+      t = (tokens.get(kind) or {}).get(name)
+      if t is None:
+        raise ValueError('the batch has no %s token feature %r' % (kind, name))
+      want = (b,) if kind == 'context' else (b, n)
+      if tuple(t.shape[:-1]) != want or t.dim() != len(want) + 1:
+        raise ValueError('%s token feature %r has shape %s, expected %s + (T,)' %
+                         (kind, name, tuple(t.shape), want))
+      ids.append(t.to(self.device, torch.int32, non_blocking=True).contiguous())
+    self._ids = ids
+
+  def train_step(self, x, y_true, tokens=None, sample_weight=None, mask=None):
+    b, n, _ = x.shape
+    self._set_tokens(tokens, b, n)
+    return super().train_step(x, y_true, sample_weight=sample_weight, mask=mask)
+
+  @torch.no_grad()
+  def predict(self, x, mask=None, y_true=None, tokens=None):
+    b, n, _ = x.shape
+    self._set_tokens(tokens, b, n)
+    return super().predict(x, mask=mask, y_true=y_true)
+
+  def _circular_pad(self, x, valid):
+    """K9 over the dense rows and over every example feature's id rows (same indices)."""
+    t = self.tower
+    self._step_ids = list(self._ids)
+    if not (t.use_batch_norm or t.input_batch_norm) or valid is None:
+      return x
+    b, n, d = x.shape
+    if d:
+      x = super()._circular_pad(x, valid)
+    v8 = valid.reshape(b, n).to(torch.uint8).contiguous()
+    if getattr(self, '_pad_idx', None) is None or self._pad_idx.shape != (b, n):
+      self._pad_idx = torch.empty(b, n, dtype=torch.int32, device=x.device)
+    for k, (kind, name, _) in enumerate(self.features):
+      if kind != 'example':
+        continue
+      ids = self._ids[k]
+      if ids.shape[-1] % 4:
+        raise ValueError('circular padding of token feature %r needs max_tokens to be a '
+                         'multiple of 4, got %d' % (name, ids.shape[-1]))
+      out = self._padded.get(name)
+      if out is None or out.shape != ids.shape:
+        out = self._padded[name] = torch.empty_like(ids)
+      _C.check(_C.lib.tfr_circular_pad_gather(_C.ptr(ids), _C.ptr(v8), b, n,
+                                              ids.shape[-1] * 4, _C.ptr(self._pad_idx),
+                                              _C.ptr(out), _C.stream()))
+      self._step_ids[k] = out
+    return x
+
+  def _bags(self, k, b, n):
+    """(ids, R, T, rows_per_bag) of feature k."""
+    ids = self._step_ids[k]
+    t = ids.shape[-1]
+    if self.features[k][0] == 'context':
+      return ids, b, t, n
+    return ids, b * n, t, 1
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, d = x.shape
+    if d != self.dense_dim:
+      raise ValueError('x has %d dense features, the tower expects %d' % (d, self.dense_dim))
+    width = self.mlp.input_dim
+    st = _C.stream()
+    if d:
+      self.xe.view(b, n, width)[..., :d].copy_(x)
+    col = d
+    for k, (_, _, ti) in enumerate(self.features):
+      emb = self.embeddings[ti]
+      ids, r, t, rpb = self._bags(k, b, n)
+      _C.check(_C.lib.tfr_embedding_fwd(_C.ptr(ids), r, t, _C.ptr(emb.flat.data),
+                                        emb.vocab_size, emb.embedding_dim, emb._combiner, rpb,
+                                        ctypes.c_void_p(self.xe.data_ptr() + 4 * col), width,
+                                        _C.ptr(self.bad_ids), st))
+      col += emb.embedding_dim
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(self.mlp.flat.data),
+                                _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores),
+                                self.mlp._precision, st))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, d = x.shape
+    mlp, sc = self.mlp, self.tower
+    st = _C.stream()
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(mlp.flat.data),
+                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.n_tables),
+                                mlp._precision, st))
+    _C.check(_C.lib.tfr_mlp_input_grad(cfg, b * n, _C.ptr(mlp.flat.data), _C.ptr(self.ws), d,
+                                       self.emb_width, _C.ptr(self.d_emb), self.emb_width,
+                                       mlp._precision, st))
+    need = 0
+    for k, (_, _, ti) in enumerate(self.features):
+      emb = self.embeddings[ti]
+      _, r, t, _ = self._bags(k, b, n)
+      need = max(need, _C.lib.tfr_embedding_workspace_bytes(r, t, emb.vocab_size,
+                                                            emb.embedding_dim))
+    if self._emb_ws is None or self._emb_ws.numel() < need:
+      self._emb_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+    written = set()
+    col = 0
+    for k, (_, _, ti) in enumerate(self.features):
+      emb = self.embeddings[ti]
+      ids, r, t, rpb = self._bags(k, b, n)
+      _C.check(_C.lib.tfr_embedding_bwd(
+          _C.ptr(ids), r, t, ctypes.c_void_p(self.d_emb.data_ptr() + 4 * col), self.emb_width,
+          rpb, emb.vocab_size, emb.embedding_dim, emb._combiner, int(ti in written),
+          _C.ptr(self._emb_ws), ctypes.c_void_p(grads.data_ptr() + 4 * sc.table_offsets[ti]),
+          None, st))
+      written.add(ti)
+      col += emb.embedding_dim
+    for ti, emb in enumerate(self.embeddings):
+      if ti not in written:     # a table no feature reads: zero gradient
+        off = sc.table_offsets[ti]
+        grads[off:off + emb.flat.numel()].zero_()
