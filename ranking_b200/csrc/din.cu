@@ -562,19 +562,13 @@ int gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, f
 
 // grads[w .. w + Kin * Nout + Nout) = {A^T dZ, column sums of dZ}: A [M, Kin] (ld lda),
 // dZ [M, Nout] (ld ldz), split over M into the plan's row splits, reduced in fixed order.
+// Always in the direct orientation: the tower's fewer-tile-units rule would swap the q / k / v
+// slices at h = 64 with two heads, which changes their rounding.
 int weight_grad(const DinPlan& p, float* ws, const float* A, int lda, int Kin, const float* dZ,
                 int ldz, int Nout, const float* colsum_src, float* grads_w, cudaStream_t st) {
-  tc::GemmDesc g{};
-  g.A = A; g.lda = lda; g.B = dZ; g.ldb = ldz; g.B_lo = nullptr;
-  g.C = ws + p.part_off; g.ldc = Nout;
-  g.GM = Kin; g.GN = Nout; g.GK = p.M;
-  g.a_mn = 1; g.b_mn = 1; g.passes = 3; g.split_b = 1;
-  g.epi = tc::EPI_STORE;
-  g.splits = p.splits; g.split_stride = p.part_stride;
-  int rc = tc::gemm(g, st);
-  if (rc) return rc;
-  return mlp_reduce2(ws + p.part_off, p.splits, p.part_stride, (size_t)Kin * Nout, colsum_src,
-                     p.splits, p.cs_stride, (size_t)Nout, grads_w, st);
+  return mlp_tc_weight_grad(A, lda, Kin, dZ, ldz, Nout, p.M, p.splits, ws + p.part_off,
+                            p.part_stride, colsum_src, p.splits, p.cs_stride, true, grads_w, 3,
+                            st);
 }
 
 template <int KD>

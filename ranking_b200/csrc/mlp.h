@@ -104,6 +104,30 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
 // at least one hidden layer): tfr_mlp_input_grad.
 int mlp_tc_input_grad(int M, const MlpPlan& p, const float* params, float* ws, int col0,
                       int ncols, float* dX, int ldx, int passes, cudaStream_t st);
+// The three roles of Dense d's GEMMs on the TF32 engine.  Apart from the split kernel and
+// the fused forward, only these know where the weight operand lives for `passes` (the
+// forward and dgrad read the split parameters mlp_tc_split_params wrote for passes = 3).
+// Forward: C[M, dims[d+1]] = A[M, kc] W_d[k0 : k0 + kc, :].  With a bias: bias, then `act`,
+// and ReLU sign words into `bits` when it is given; without: a plain store.
+int mlp_tc_dense_fwd(const MlpPlan& p, int d, int k0, int kc, const float* A, int M,
+                     const float* params, const float* ws, const float* bias, int act,
+                     uint32_t* bits, float* C, int passes, cudaStream_t st);
+// Input side: C[M, nc] (ldc) = dZ_d[M, dims[d+1]] W_d[n0 : n0 + nc, :]^T, zeroed where the
+// sign word bit is clear when `mask_bits` is given; per-CTA column sums into `colsum` when
+// given (row pitch colsum_stride, slot count into *colsum_slots).
+int mlp_tc_dense_dgrad(const MlpPlan& p, int d, int n0, int nc, const float* dZ, int M,
+                       const float* params, const float* ws, const uint32_t* mask_bits,
+                       float* colsum, size_t colsum_stride, int* colsum_slots, float* C, int ldc,
+                       int passes, cudaStream_t st);
+// Weight gradient: out[0 : Kin Nout) = A^T dZ for A [M, Kin] (lda), dZ [M, Nout] (ldz), then
+// out[Kin Nout : + Nout) = the sums of bias_slots rows of bias_src (pitch bias_stride); no
+// bias part when bias_src is null.  Split-K over `splits` row ranges into `partial` (pitch
+// pstride), reduced in fixed order.  Takes the orientation with fewer tile units unless
+// `direct`.
+int mlp_tc_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ldz, int Nout,
+                       int M, int splits, float* partial, size_t pstride, const float* bias_src,
+                       int bias_slots, size_t bias_stride, bool direct, float* out, int passes,
+                       cudaStream_t st);
 // Fused 3xTF32 forward of Dense first_layer .. L (mlp_tc_fused.cu): one persistent kernel,
 // bit-identical to the per-layer walk.  _ok says whether the tower fits it: no BN / dropout /
 // input BN, ReLU or no activation, Dense first_layer at most 256 wide, every later hidden
@@ -117,15 +141,9 @@ int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
 // pieces of the CUDA-core path reused by the tensor-core path
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,
                       const uint8_t* mask, float* scores, cudaStream_t st);
-int mlp_out_layer_bwd(const float* H, int M, int K, int O, const float* W, const float* dS,
-                      const uint8_t* mask, int act, int rows_per, int splits, float* dH,
-                      float* partial, size_t pstride, cudaStream_t st);
 int mlp_out_layer_bwd2(const float* H, int M, int K, int O, const float* W, const float* dS,
                        const uint8_t* mask, int act, int rows_per, float* dH, float* slots,
                        size_t slot_stride, cudaStream_t st);
-int mlp_regroup_sum(const float* src, int slots_in, size_t src_stride, size_t src_off, int n,
-                    int group, float* dst, int slots_out, size_t dst_stride, size_t dst_off,
-                    cudaStream_t st);
 int mlp_reduce2(const float* srcA, int slotsA, size_t strideA, size_t nA, const float* srcB,
                 int slotsB, size_t strideB, size_t nB, float* out, cudaStream_t st);
 int mlp_colsum(const float* dZ, int M, int N, int rows_per, int splits, float* partial,

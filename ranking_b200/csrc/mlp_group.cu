@@ -21,7 +21,6 @@
 // tfr_group_mlp_fwd checks it (a duplicate is reported, not silently dropped).
 #include "common.cuh"
 #include "mlp.h"
-#include "tc_gemm.cuh"
 
 namespace tfr {
 
@@ -381,27 +380,11 @@ extern "C" int tfr_group_mlp_fwd(const float* X, int B, int N, int G, int gs, co
   }
   rc = mlp_tc_split_params(p, params, ws, passes, st);
   if (rc) return rc;
-  const float* whi = passes == 3 ? ws + p.whi_off : params;
-  const float* wlo = passes == 3 ? ws + p.wlo_off : nullptr;
-  // P_j = X W_1^(j): the first Dense layer on the ungathered [B * N, D] matrix
+  // P_j = X W_1^(j): the first Dense layer on the ungathered [B * N, D] matrix, with slot j's
+  // rows j D .. (j + 1) D of W_1
   for (int j = 0; j < gs; ++j) {
-    tc::GemmDesc g{};
-    g.A = X; g.lda = D;
-    if (passes == 3) {
-      // slot j of W_1^T [H, gs * D] (pre-split transposes, K-major): columns j D .. (j + 1) D
-      g.B = ws + p.wthi_off + p.w_off[0] + (size_t)j * D; g.ldb = gs * D;
-      g.B_lo = ws + p.wtlo_off + p.w_off[0] + (size_t)j * D;
-      g.b_mn = 0;
-    } else {
-      g.B = whi + p.w_off[0] + (size_t)j * D * H; g.ldb = H;
-      g.B_lo = nullptr;
-      g.b_mn = 1;
-    }
-    g.C = gw.P + (size_t)j * gw.p_stride; g.ldc = H;
-    g.GM = (int)bn; g.GN = H; g.GK = D;
-    g.a_mn = 0; g.passes = passes; g.split_b = 0;
-    g.epi = tc::EPI_STORE; g.act = TFR_ACT_NONE; g.splits = 1;
-    rc = tc::gemm(g, st);
+    rc = mlp_tc_dense_fwd(p, 0, j * D, D, X, (int)bn, params, ws, nullptr, TFR_ACT_NONE, nullptr,
+                          gw.P + (size_t)j * gw.p_stride, passes, st);
     if (rc) return rc;
   }
   {
@@ -476,29 +459,11 @@ extern "C" int tfr_group_mlp_bwd(const float* X, int B, int N, int G, int gs, co
     group_gather_bwd_kernel<<<(unsigned)((t + 255) / 256), 256, 0, st>>>(tail.dz, gw.inv, S, B, N,
                                                                          G, gs, j, H, dP);
     TFR_LAUNCH_OK();
-    // dW^(j) [D, H] = X^T dP_j, or its transpose when that orientation has fewer tile units
-    // (decided as in mlp_tc_bwd)
-    const bool swapped = tc::tile_units(H, D) < tc::tile_units(D, H);
-    tc::GemmDesc g{};
-    if (!swapped) {
-      g.A = X; g.lda = D; g.B = dP; g.ldb = H;
-      g.GM = D; g.GN = H; g.store_transposed = 0;
-    } else {
-      g.A = dP; g.lda = H; g.B = X; g.ldb = D;
-      g.GM = H; g.GN = D; g.store_transposed = 1;
-    }
-    g.C = ws + p.partial_off; g.ldc = H;
-    g.GK = (int)bn;
-    g.a_mn = 1; g.b_mn = 1; g.passes = passes; g.split_b = 1;
-    g.epi = tc::EPI_STORE;
-    g.splits = splits; g.split_stride = p.partial_stride;
-    rc = tc::gemm(g, st);
-    if (rc) return rc;
     const bool last = j == gs - 1;   // the bias gradient follows the last slot's block
-    rc = mlp_reduce2(ws + p.partial_off, splits, p.partial_stride, (size_t)D * H,
-                     last ? tail.bias_src : nullptr, last ? tail.bias_slots : 0,
-                     last ? tail.bias_stride : 0, last ? (size_t)H : 0,
-                     grads + p.w_off[0] + (size_t)j * D * H, st);
+    rc = mlp_tc_weight_grad(X, D, D, dP, H, H, (int)bn, splits, ws + p.partial_off,
+                            p.partial_stride, last ? tail.bias_src : nullptr, tail.bias_slots,
+                            tail.bias_stride, false, grads + p.w_off[0] + (size_t)j * D * H,
+                            passes, st);
     if (rc) return rc;
   }
   return TFR_OK;

@@ -419,23 +419,6 @@ out_layer_bwd2_vec_kernel(const float4* __restrict__ H4, int M, int K4, const fl
   }
 }
 
-// dst[z][dst_off + i] = sum_{g < group} src[z * group + g][src_off + i], i < n.
-__global__ void __launch_bounds__(256)
-regroup_sum_kernel(const float* __restrict__ src, int slots_in, size_t src_stride,
-                   size_t src_off, int n, int group, float* __restrict__ dst,
-                   size_t dst_stride, size_t dst_off) {
-  const int z = blockIdx.y;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float acc = 0.f;
-#pragma unroll 8
-  for (int g = 0; g < group; ++g) {
-    const int s = z * group + g;
-    if (s < slots_in) acc += src[(size_t)s * src_stride + src_off + i];
-  }
-  dst[(size_t)z * dst_stride + dst_off + i] = acc;
-}
-
 // out[i] = sum over slots of srcA (i < nA) or srcB (nA <= i < nA + nB): the weight
 // part of a layer gradient comes from the dW split partials, the bias part straight
 // from the per-CTA column sums.  16 outputs x 16 slot lanes per block, fixed order.
@@ -615,31 +598,11 @@ int mlp_out_layer_bwd2(const float* H, int M, int K, int O, const float* W, cons
   return TFR_OK;
 }
 
-int mlp_regroup_sum(const float* src, int slots_in, size_t src_stride, size_t src_off, int n,
-                    int group, float* dst, int slots_out, size_t dst_stride, size_t dst_off,
-                    cudaStream_t st) {
-  dim3 grid((n + 255) / 256, slots_out);
-  regroup_sum_kernel<<<grid, 256, 0, st>>>(src, slots_in, src_stride, src_off, n, group, dst,
-                                          dst_stride, dst_off);
-  TFR_LAUNCH_OK();
-  return TFR_OK;
-}
-
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,
                       const uint8_t* mask, float* scores, cudaStream_t st) {
   const int rows_per_block = 32;
   out_layer_fwd_kernel<<<(M + rows_per_block - 1) / rows_per_block, 256, 0, st>>>(
       H, M, K, O, W, bias, mask, scores);
-  TFR_LAUNCH_OK();
-  return TFR_OK;
-}
-
-int mlp_out_layer_bwd(const float* H, int M, int K, int O, const float* W, const float* dS,
-                      const uint8_t* mask, int act, int rows_per, int splits, float* dH,
-                      float* partial, size_t pstride, cudaStream_t st) {
-  const int threads = ((K + 31) / 32) * 32;
-  out_layer_bwd_kernel<<<splits, threads, 0, st>>>(H, M, K, O, W, dS, mask, act, rows_per, dH,
-                                                  partial, pstride);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

@@ -90,6 +90,78 @@ int mlp_tc_split_params(const MlpPlan& p, const float* params, float* ws, int pa
   return split_params(p, params, ws, passes, st);
 }
 
+int mlp_tc_dense_fwd(const MlpPlan& p, int d, int k0, int kc, const float* A, int M,
+                     const float* params, const float* ws, const float* bias, int act,
+                     uint32_t* bits, float* C, int passes, cudaStream_t st) {
+  const int nout = p.dims[d + 1];
+  tc::GemmDesc g{};
+  g.A = A; g.lda = kc;
+  if (passes == 3) {   // W^T [out, in], pre-split: K-major
+    g.B = ws + p.wthi_off + p.w_off[d] + k0; g.ldb = p.dims[d];
+    g.B_lo = ws + p.wtlo_off + p.w_off[d] + k0;
+    g.b_mn = 0;
+  } else {             // single-pass TF32 reads the fp32 kernel [in, out] as is: MN-major
+    g.B = params + p.w_off[d] + (size_t)k0 * nout; g.ldb = nout;
+    g.b_mn = 1;
+  }
+  g.C = C; g.ldc = nout;
+  g.GM = M; g.GN = nout; g.GK = kc;
+  g.passes = passes;
+  g.epi = bias ? tc::EPI_BIAS_ACT : tc::EPI_STORE;
+  g.bias = bias; g.act = act;
+  g.mask_bits_out = bits;
+  g.splits = 1;
+  return tc::gemm(g, st);
+}
+
+int mlp_tc_dense_dgrad(const MlpPlan& p, int d, int n0, int nc, const float* dZ, int M,
+                       const float* params, const float* ws, const uint32_t* mask_bits,
+                       float* colsum, size_t colsum_stride, int* colsum_slots, float* C, int ldc,
+                       int passes, cudaStream_t st) {
+  const int nout = p.dims[d + 1];
+  const size_t w = p.w_off[d] + (size_t)n0 * nout;   // W rows n0 .. n0 + nc: K-major B rows
+  tc::GemmDesc g{};
+  g.A = dZ; g.lda = nout;
+  g.B = (passes == 3 ? ws + p.whi_off : params) + w; g.ldb = nout;
+  g.B_lo = passes == 3 ? ws + p.wlo_off + w : nullptr;
+  g.C = C; g.ldc = ldc;
+  g.GM = M; g.GN = nc; g.GK = nout;
+  g.passes = passes;
+  g.epi = mask_bits ? tc::EPI_MASK_BITS : tc::EPI_STORE;
+  g.mask_bits_in = mask_bits;
+  g.splits = 1;
+  g.colsum = colsum; g.colsum_stride = (int)colsum_stride; g.colsum_slots_out = colsum_slots;
+  return tc::gemm(g, st);
+}
+
+int mlp_tc_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ldz, int Nout,
+                       int M, int splits, float* partial, size_t pstride, const float* bias_src,
+                       int bias_slots, size_t bias_stride, bool direct, float* out, int passes,
+                       cudaStream_t st) {
+  // dW[Kin, Nout] = A^T dZ in one of two orientations:
+  //   direct : GM = Kin (tiles of 128), GN = Nout
+  //   swapped: GM = Nout,               GN = Kin, stored transposed
+  const bool swapped = !direct && tc::tile_units(Nout, Kin) < tc::tile_units(Kin, Nout);
+  tc::GemmDesc g{};
+  if (!swapped) {
+    g.A = A; g.lda = lda; g.B = dZ; g.ldb = ldz;
+    g.GM = Kin; g.GN = Nout;
+  } else {
+    g.A = dZ; g.lda = ldz; g.B = A; g.ldb = lda;
+    g.GM = Nout; g.GN = Kin; g.store_transposed = 1;
+  }
+  g.C = partial; g.ldc = Nout;
+  g.GK = M;
+  g.a_mn = 1; g.b_mn = 1; g.passes = passes; g.split_b = 1;
+  g.epi = tc::EPI_STORE;
+  g.splits = splits; g.split_stride = pstride;
+  int rc = tc::gemm(g, st);
+  if (rc) return rc;
+  return mlp_reduce2(partial, splits, pstride, (size_t)Kin * Nout, bias_src,
+                     bias_src ? bias_slots : 0, bias_src ? bias_stride : 0,
+                     bias_src ? (size_t)Nout : 0, out, st);
+}
+
 int mlp_tc_fwd(const float* X, int M, const MlpPlan& p, const float* params,
                const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st) {
   return mlp_tc_fwd_from(0, X, M, p, params, mask, ws, scores, passes, st);
@@ -109,8 +181,6 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
   if (mlp_tc_fused_fwd_ok(first_layer, X, M, p, passes))
     return mlp_tc_fused_fwd(first_layer, X, M, p, params, mask, ws, scores, st);
   const int L = p.n_dense - 1;
-  const float* whi = passes == 3 ? ws + p.whi_off : params;
-  const float* wlo = passes == 3 ? ws + p.wlo_off : nullptr;
   const float* in = X;
   if (p.input_bn && first_layer == 0) {
     rc = mlp_input_bn_fwd(X, M, p, params, ws, st);
@@ -118,27 +188,13 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
     in = ws + p.xin_off;
   }
   for (int d = first_layer; d < L; ++d) {
-    tc::GemmDesc g{};
-    g.A = in; g.lda = p.dims[d];
-    if (passes == 3) {   // W^T [out, in], pre-split: K-major
-      g.B = ws + p.wthi_off + p.w_off[d]; g.ldb = p.dims[d];
-      g.B_lo = ws + p.wtlo_off + p.w_off[d];
-      g.b_mn = 0;
-    } else {             // single-pass TF32 reads the fp32 kernel [in, out] as is: MN-major
-      g.B = whi + p.w_off[d]; g.ldb = p.dims[d + 1];
-      g.B_lo = nullptr;
-      g.b_mn = 1;
-    }
-    g.C = ws + (p.use_bn ? p.xhat_off[d] : p.act_off[d]); g.ldc = p.dims[d + 1];
-    g.GM = M; g.GN = p.dims[d + 1]; g.GK = p.dims[d];
-    g.a_mn = 0; g.passes = passes; g.split_b = 0;
-    g.epi = tc::EPI_BIAS_ACT; g.bias = params + p.b_off[d];
-    g.act = p.use_bn ? TFR_ACT_NONE : p.activation;   // BN sits before the activation
-    g.splits = 1; g.split_stride = 0;
     // ReLU sign bits for the backward mask: 1 bit per activation instead of re-reading H
-    if (p.activation == TFR_ACT_RELU && !p.post())
-      g.mask_bits_out = reinterpret_cast<uint32_t*>(ws + p.bits_off[d]);
-    rc = tc::gemm(g, st);
+    uint32_t* bits = p.activation == TFR_ACT_RELU && !p.post()
+                         ? reinterpret_cast<uint32_t*>(ws + p.bits_off[d])
+                         : nullptr;
+    rc = mlp_tc_dense_fwd(p, d, 0, p.dims[d], in, M, params, ws, params + p.b_off[d],
+                          p.use_bn ? TFR_ACT_NONE : p.activation,   // BN sits before the activation
+                          bits, ws + (p.use_bn ? p.xhat_off[d] : p.act_off[d]), passes, st);
     if (rc) return rc;
     rc = mlp_hidden_post_fwd(d, M, p, params, ws, st);
     if (rc) return rc;
@@ -166,8 +222,6 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
   float* partial = ws + p.partial_off;
   const size_t pstride = p.partial_stride;
   const int splits = p.splits;
-  const float* whi = passes == 3 ? ws + p.whi_off : params;   // written by the forward
-  const float* wlo = passes == 3 ? ws + p.wlo_off : nullptr;
   float* dz_cur = ws + p.dz_off[0];
   float* dz_nxt = ws + p.dz_off[1];
   float* tiles = ws + p.tile_off;
@@ -208,49 +262,17 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
       bslots = splits;
       bstride = p.tile_stride;
     }
-    {
-      // dW[Kin, Nout] = A^T dZ in one of two orientations:
-      //   direct : GM = Kin (tiles of 128), GN = Nout
-      //   swapped: GM = Nout,               GN = Kin, stored transposed
-      const bool swapped = tc::tile_units(Nout, Kin) < tc::tile_units(Kin, Nout);
-      tc::GemmDesc g{};
-      if (!swapped) {
-        g.A = A; g.lda = Kin; g.B = dz_cur; g.ldb = Nout;
-        g.GM = Kin; g.GN = Nout; g.store_transposed = 0;
-      } else {
-        g.A = dz_cur; g.lda = Nout; g.B = A; g.ldb = Kin;
-        g.GM = Nout; g.GN = Kin; g.store_transposed = 1;
-      }
-      g.B_lo = nullptr;
-      g.C = partial; g.ldc = Nout;
-      g.GK = M;
-      g.a_mn = 1; g.b_mn = 1; g.passes = passes; g.split_b = 1;
-      g.epi = tc::EPI_STORE;
-      g.splits = splits; g.split_stride = pstride;
-      rc = tc::gemm(g, st);
-      if (rc) return rc;
-    }
-    rc = mlp_reduce2(partial, splits, pstride, (size_t)Kin * Nout, bsrc, bslots, bstride,
-                     (size_t)Nout, grads + p.w_off[d], st);
+    rc = mlp_tc_weight_grad(A, Kin, Kin, dz_cur, Nout, Nout, M, splits, partial, pstride, bsrc,
+                            bslots, bstride, false, grads + p.w_off[d], passes, st);
     if (rc) return rc;
     if (d > 0 || p.input_bn) {   // d == 0 with input BN: dL/dXin for its gamma / beta
-      tc::GemmDesc g{};
-      g.A = dz_cur; g.lda = Nout;
-      g.B = whi + p.w_off[d]; g.ldb = Nout;     // W [Kin rows (GN), Nout (GK)] : K-major
-      g.B_lo = wlo ? wlo + p.w_off[d] : nullptr;
-      g.C = dz_nxt; g.ldc = Kin;
-      g.GM = M; g.GN = Kin; g.GK = Nout;
-      g.a_mn = 0; g.b_mn = 0; g.passes = passes; g.split_b = 0;
       const bool masked = d > 0 && mact != TFR_ACT_NONE;
-      g.epi = masked ? tc::EPI_MASK_BITS : tc::EPI_STORE;
-      g.mask_bits_in = masked ? reinterpret_cast<const uint32_t*>(ws + p.bits_off[d - 1]) : nullptr;
-      g.act = mact;
-      g.splits = 1; g.split_stride = 0;
+      const bool sums = d > 0 && !p.post();
       int cslots = 0;
-      if (d > 0 && !p.post()) {
-        g.colsum = tiles; g.colsum_stride = (int)p.tile_stride; g.colsum_slots_out = &cslots;
-      }
-      rc = tc::gemm(g, st);
+      rc = mlp_tc_dense_dgrad(
+          p, d, 0, Kin, dz_cur, M, params, ws,
+          masked ? reinterpret_cast<const uint32_t*>(ws + p.bits_off[d - 1]) : nullptr,
+          sums ? tiles : nullptr, p.tile_stride, sums ? &cslots : nullptr, dz_nxt, Kin, passes, st);
       if (rc) return rc;
       bsrc = tiles;            // column sums of dZ_{d-1}: one slot per CTA and quarter
       bslots = cslots;
@@ -271,23 +293,14 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
 }
 
 // dX[:, 0:ncols] = dZ_0 W_0[col0:col0 + ncols, :]^T.  Without input BN, mlp_tc_bwd leaves dZ_0
-// in the ping-pong buffer it started from after L - 1 swaps; W_0's rows are K-major B rows.
+// in the ping-pong buffer it started from after L - 1 swaps.
 int mlp_tc_input_grad(int M, const MlpPlan& p, const float* params, float* ws, int col0,
                       int ncols, float* dX, int ldx, int passes, cudaStream_t st) {
   int rc = check_dims(p);
   if (rc) return rc;
-  const int L = p.n_dense - 1, n1 = p.dims[1];
-  const float* whi = passes == 3 ? ws + p.whi_off : params;
-  tc::GemmDesc g{};
-  g.A = ws + p.dz_off[(L - 1) & 1]; g.lda = n1;
-  g.B = whi + p.w_off[0] + (size_t)col0 * n1; g.ldb = n1;
-  g.B_lo = passes == 3 ? ws + p.wlo_off + p.w_off[0] + (size_t)col0 * n1 : nullptr;
-  g.C = dX; g.ldc = ldx;
-  g.GM = M; g.GN = ncols; g.GK = n1;
-  g.a_mn = 0; g.b_mn = 0; g.passes = passes; g.split_b = 0;
-  g.epi = tc::EPI_STORE;
-  g.splits = 1; g.split_stride = 0;
-  return tc::gemm(g, st);
+  const int L = p.n_dense - 1;
+  return mlp_tc_dense_dgrad(p, 0, col0, ncols, ws + p.dz_off[(L - 1) & 1], M, params, ws,
+                            nullptr, nullptr, 0, nullptr, dX, ldx, passes, st);
 }
 
 }  // namespace tfr

@@ -8,8 +8,6 @@
 namespace tfr {
 namespace tc {
 
-bool shape_supported(int lda, int ldb) { return lda % 4 == 0 && ldb % 4 == 0; }
-
 template <bool A_MN, bool B_MN>
 static int dispatch(const GemmDesc& g, const wg::Args& a, cudaStream_t st, int* ctas) {
   if (g.passes == 1) return wg::launch<float, A_MN, B_MN, 1, false, false>(a, st, ctas);

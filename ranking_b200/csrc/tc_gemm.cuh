@@ -52,8 +52,5 @@ int gemm(const GemmDesc& g, cudaStream_t stream);
 // walking the whole k range.  Picks the cheaper orientation of a dW GEMM.
 inline int tile_units(int gm, int gn) { return ((gm + 127) / 128) * ((gn + 63) / 64); }
 
-// True if a layer shape can run on this engine (alignment constraints).
-bool shape_supported(int rows_ld_a, int rows_ld_b);
-
 }  // namespace tc
 }  // namespace tfr

@@ -14,27 +14,47 @@ def kernel_launches(fn):
   launch order.  `kernel` is the bare name with its template arguments, e.g.
   'out_layer_bwd2_vec_kernel<4>'; grid and block are (x, y, z) tuples.
 
-  A profiling session now and then delivers no kernel records at all (seen on H100 with
-  torch 2.11); fn() is then run again, up to three times, so it must be repeatable: it
-  resets whatever state it changes (gradients, BN statistics, dropout counters)."""
-  from torch.profiler import ProfilerActivity, profile
+  A profiling session can lose GPU kernel records: most often those of the first kernels
+  it sees, now and then all of them (seen on H100 with torch 2.11, more often late in a
+  long test run).  So a session runs fn() three times, each run in its own annotated
+  range, and the launches of the first run whose every kernel launch call has its GPU
+  record (matched by correlation id) are returned; if no run is complete, the session is
+  repeated, up to three times.  fn() must therefore be repeatable: it resets whatever
+  state it changes (gradients, BN statistics, dropout counters)."""
+  from torch.profiler import ProfilerActivity, profile, record_function
+  runs = 3
+  launches = []
   for _ in range(3):
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-      out = fn()
-      torch.cuda.synchronize()
+      for r in range(runs):
+        with record_function('kernel_launches %d' % r):
+          out = fn()
+          torch.cuda.synchronize()
     with tempfile.TemporaryDirectory() as d:
       path = os.path.join(d, 'trace.json')
       prof.export_chrome_trace(path)
       with open(path) as f:
         events = json.load(f)['traceEvents']
-    launches = []
-    for e in sorted((e for e in events if e.get('cat') == 'kernel'), key=lambda e: e['ts']):
-      m = re.search(r'(\w+(?:<[^<>()]*>)?)\(', e['name'])
-      name = (m.group(1) if m else e['name']).replace(' ', '')
-      launches.append((name, tuple(e['args']['grid']), tuple(e['args']['block'])))
-    if launches:
-      break
+    spans = {e['name']: e for e in events if e.get('cat') == 'user_annotation'}
+    for r in range(runs):
+      span = spans.get('kernel_launches %d' % r)
+      if span is None:
+        continue
+      calls = {e['args']['correlation'] for e in events
+               if e.get('cat') in ('cuda_runtime', 'cuda_driver')
+               and re.search(r'Launch\w*Kernel', e['name'])
+               and span['ts'] <= e['ts'] <= span['ts'] + span['dur']}
+      records = sorted((e for e in events
+                        if e.get('cat') == 'kernel' and e['args'].get('correlation') in calls),
+                       key=lambda e: e['ts'])
+      launches = []
+      for e in records:
+        m = re.search(r'(\w+(?:<[^<>()]*>)?)\(', e['name'])
+        name = (m.group(1) if m else e['name']).replace(' ', '')
+        launches.append((name, tuple(e['args']['grid']), tuple(e['args']['block'])))
+      if calls and len(records) == len(calls):
+        return out, launches
   return out, launches
 
 

@@ -8,10 +8,10 @@ hidden layer and the column sums that become that layer's bias gradient, without
 flips loosening the bar.  Each case restates the dispatch rule it is named for and checks,
 from the kernels the call launched (torch.profiler), that the rule's variant ran:
 
-  fp32            out_layer_bwd_kernel, one thread per k (mlp_simt.cu:152, 704-716)
-  tf32x3 / tf32   mlp_out_layer_bwd2 (mlp_simt.cu:563-616): o1, vec<O>, generic
+  fp32            out_layer_bwd_kernel, one thread per k (mlp_simt.cu:152, 667-679)
+  tf32x3 / tf32   mlp_out_layer_bwd2 (mlp_simt.cu:546-599): o1, vec<O>, generic
   bf16            mlp_bf16.cu:394-415 (forward), 434-469 (backward): fast<C, O>, generic
-  reduction       mlp_reduce2 (mlp_simt.cu:539-561) of the per-block output-layer slots
+  reduction       mlp_reduce2 (mlp_simt.cu:522-544) of the per-block output-layer slots
                   (tf32x3 / tf32 / bf16): reduce2_vec, reduce_tall, reduce2
 
 M = 1000 keeps the output-layer backward below 128 block slots, M = 6000 above it (the slot
@@ -48,7 +48,7 @@ def _rel(a, b):
 
 # ------------------------------------------------------------ dispatch mirrors ---
 def tc_out_kernel(k, o, masked):
-  """mlp_out_layer_bwd2 (mlp_simt.cu:566, 581, 604): the tower's H, W and dH are 16-byte
+  """mlp_out_layer_bwd2 (mlp_simt.cu:549, 564, 587): the tower's H, W and dH are 16-byte
   aligned at these shapes (K % 4 == 0, one hidden layer over D = 16 inputs)."""
   if o == 1 and k % 4 == 0 and k <= 1024:
     return 'out_layer_bwd2_o1_kernel'
@@ -75,7 +75,7 @@ def out_slots(m):
 
 
 def reduce_kernel(k, o, m):
-  """mlp_reduce2 (mlp_simt.cu:543-557) over the output layer's [K * O + O] slots: the slot
+  """mlp_reduce2 (mlp_simt.cu:526-540) over the output layer's [K * O + O] slots: the slot
   stride is a multiple of 64 floats and the gradient slice starts at w_off[1] = (D + 1) K,
   16-byte aligned when K % 4 == 0."""
   n = k * o + o
