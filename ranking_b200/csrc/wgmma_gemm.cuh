@@ -203,8 +203,11 @@ __device__ __forceinline__ int swz_chunk(int row, int kc) { return row * 128 + (
 // The register-staged operand: an MN-major fp32 B tile ([k][n], n contiguous) of 128 columns
 // x 32 k, transposed into the K-major swizzled tile(s) and, for 3xTF32, split into hi / lo.
 // A warp takes 8 consecutive column chunks (one 128-byte line per k row) of 4 consecutive k
-// rows: within one k row every lane's columns share their swizzle phase, which keeps the
-// scalar K-major stores on 4 ways of bank conflict instead of 16.
+// rows, so all 32 lanes of a scalar K-major store write the same 16-byte k chunk position of
+// their rows and differ only in the row's swizzle phase (row mod 8) and in k mod 4.  Store
+// step j of a lane writes column r + ((j + s) & 3) of its chunk, s = (lane mod 8) / 2: the 8
+// lanes of a k row then write rows of 8 different phases, and the 32 lanes hit 32 different
+// banks.  (With s = 0 they would write rows of 2 phases: 4 ways of bank conflict.)
 struct BTileMN {
   float4 v[4];
   __device__ __forceinline__ static void chunk(int i, int& k, int& r) {
@@ -231,14 +234,25 @@ struct BTileMN {
   }
   template <bool SPLIT>
   __device__ __forceinline__ void store(unsigned char* hi, unsigned char* lo) const {
+    const int s = (threadIdx.x & 7) >> 1;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       int k, r;
       chunk(i, k, r);
-      const float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+      // rotate the chunk left by s with selects (a dynamic index would go to local memory)
+      float e0 = v[i].x, e1 = v[i].y, e2 = v[i].z, e3 = v[i].w;
+      if (s & 1) {
+        const float t = e0;
+        e0 = e1; e1 = e2; e2 = e3; e3 = t;
+      }
+      if (s & 2) {
+        float t = e0; e0 = e2; e2 = t;
+        t = e1; e1 = e3; e3 = t;
+      }
+      const float e[4] = {e0, e1, e2, e3};   // e[j]: column r + ((j + s) & 3)
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const int off = swz_chunk(r + j, k >> 2) + (k & 3) * 4;
+        const int off = swz_chunk(r + ((j + s) & 3), k >> 2) + (k & 3) * 4;
         if (SPLIT) {
           const float h = tf32_rn(e[j]);
           *reinterpret_cast<float*>(hi + off) = h;

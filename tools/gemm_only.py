@@ -1,7 +1,10 @@
 """Times the eight scorer GEMMs of the config-2 training step (fwd1-3, dz1-2, dw1-3) through
 the 3xTF32 engine, with the shapes, orientations and split-K counts the trainer uses, and
 prints per GEMM the time, the algorithmic TFLOP/s (2 GM GN GK) and the GB/s of the tensors it
-must move (operands read once, output and sign words written once).  The last line times the
+must move (operands read once, output and sign words written once).  dw1t-dw3t time the dW
+GEMMs as they would run on a transposed dZ (dZ^T [width][M]): direct orientation, A the
+MN-major activations, B = dZ^T K-major, copied by cp.async and split in shared memory; same
+shapes and split-K count as dw1-dw3.  The last line times the
 whole 3xTF32 forward of the config-2 tower (136-256-128-64-1, the fused kernel) through
 tfr_mlp_fwd: X read once; H1, H2, H3, their sign words and the scores written once.
 usage: gemm_only.py [--reps R] [--warmup W] [--out FILE.json]"""
@@ -41,6 +44,8 @@ def shapes(sms):
       out['dw%d' % (d + 1)] = (nout, kin, M, 1, 1, 1, 0, 1, s)
     else:
       out['dw%d' % (d + 1)] = (kin, nout, M, 1, 1, 1, 0, 0, s)
+  for d in range(L):         # dW = A^T (dZ^T)^T: A MN-major, B = dZ^T K-major through cp.async
+    out['dw%dt' % (d + 1)] = (DIMS[d], DIMS[d + 1], M, 1, 0, 1, 0, 0, s)
   return out
 
 
@@ -95,15 +100,21 @@ def main():
     print('%-5s GM %6d GN %4d GK %6d splits %4d  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s' % (
         name, shape[0], shape[1], shape[2], shape[3], us, rows[-1]['tflops'], rows[-1]['gbps']),
           flush=True)
-  total = sum(r['us'] for r in rows)
+  step = [r for r in rows if not r['gemm'].endswith('t')]   # the eight GEMMs the step runs
+  total = sum(r['us'] for r in step)
   print('total %.1f us' % total, flush=True)
+  dw = sum(r['us'] for r in step if r['gemm'].startswith('dw'))
+  dwt = sum(r['us'] for r in rows if r['gemm'].startswith('dw') and r['gemm'].endswith('t'))
+  print('dw1-dw3 %.1f us, dw1t-dw3t %.1f us (%+.1f %%)' % (dw, dwt, 100.0 * (dwt / dw - 1.0)),
+        flush=True)
   fwd = time_tower_fwd(dev, g, args.reps, args.warmup)
   print('tower fwd (tfr_mlp_fwd, M %d)  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s' % (
       M, fwd['us'], fwd['tflops'], fwd['gbps']), flush=True)
   if args.out:
     with open(args.out, 'w') as f:
       json.dump(dict(device=torch.cuda.get_device_name(dev), sms=sms, reps=args.reps,
-                     gemms=rows, total_us=round(total, 2), tower_fwd=fwd), f, indent=1)
+                     gemms=rows, total_us=round(total, 2), dw_us=round(dw, 2),
+                     dwt_us=round(dwt, 2), tower_fwd=fwd), f, indent=1)
 
 
 def time_tower_fwd(dev, g, reps, warmup):
