@@ -14,9 +14,16 @@
 //     is transposed and, for 3xTF32, split;
 //   * one wgmma group stays in flight across k blocks (two A fragment register sets);
 //   * the copies for the next tile start before the epilogue of the current one;
-//   * the epilogue runs on the accumulator registers: bias / activation, ReLU masks (from an
-//     fp32 array or from 1-bit sign words), ReLU sign words out, per-warp column sums,
-//     row-major, transposed or split-K partial stores, fp32 or bf16 output.
+//   * the epilogue: bias / activation, ReLU masks (from an fp32 array or from 1-bit sign
+//     words), ReLU sign words out, column sums, row-major, transposed or split-K partial
+//     stores, fp32 or bf16 output.  Where it runs follows from A's layout:
+//       - K-major A (forward and dZ GEMMs: GM long, a few k blocks per tile): a third
+//         warpgroup runs it.  The MMA warpgroups write a tile's raw accumulators to a staging
+//         tile in shared memory and start the next tile's k loop; the epilogue warpgroup reads
+//         the staging tile row-major (a lane takes 4 adjacent columns, a warp whole rows) and
+//         overlaps that k loop.  The staging tile takes the room of one ring stage.
+//       - MN-major A (the dW GEMMs: one epilogue per 50-100 k blocks): the two MMA warpgroups
+//         run it on their accumulator registers and keep the fourth stage.
 // The grid is persistent (at most one CTA per SM), so the column-sum slots are bounded by
 // 8 x the SM count.
 #pragma once
@@ -33,8 +40,9 @@ namespace wg {
 
 constexpr int BM = 128;          // rows of an output tile (two warpgroups of 64)
 constexpr int BN = 128;          // columns of an output tile (one m64n128 instruction)
-constexpr int kThreads = 256;
+constexpr int kThreads = 256;    // the two MMA warpgroups
 constexpr int kWarps = kThreads / 32;
+constexpr int kEpiThreads = 128; // the epilogue warpgroup of a staged kernel (threads 256..383)
 constexpr int kTileBytes = 128 * 128;   // one swizzled B tile: 128 rows x 128 bytes of k
 // A tile: 128 rows x 128 bytes of k.  K-major rows are padded to 144 B, MN-major k rows
 // (512 B of m) to 544 B (fp32, 32 rows) / 272 B (bf16, 64 rows): either way the fragment
@@ -44,6 +52,23 @@ constexpr int kAPitchMN = 4 * (128 + 8);   // bytes per k row (fp32); bf16 uses 
 constexpr int kATileBytes = 128 * kAPitchK;
 constexpr int kMaxStages = 4;
 constexpr int kSmemLimit = 227 * 1024;  // dynamic shared memory of one CTA on sm_90
+// Staging tile: 128 x 128 fp32 accumulators, rows padded to 136 floats.  The pitch is 8 banks
+// mod 32, so the float2 stores of the accumulator layout (8 rows x 4 column pairs per warp)
+// are conflict-free per half-warp; the float4 row reads and the column reads are contiguous.
+constexpr int kStagingPitch = BN + 8;
+constexpr int kStagingBytes = BM * kStagingPitch * 4;
+// Named barriers of a staged kernel (0 is __syncthreads, which it never uses).
+//   kBarMma:  bar.sync over the 256 MMA threads: the k loop's barrier.
+//   kBarFull: 256 MMA threads arrive after writing the staging tile, the 128 epilogue threads
+//             wait: 384.  Once per tile.
+//   kBarFree: 128 epilogue threads arrive after their last read of the staging tile, the 256
+//             MMA threads wait before writing the next one: 384.  Once per tile but a CTA's
+//             last, which nobody would wait for.
+//   kBarEpi:  bar.sync over the 128 epilogue threads, between the row pass and the column sums.
+constexpr int kBarMma = 1, kBarFull = 2, kBarFree = 3, kBarEpi = 4;
+// Registers after setmaxnreg: 2 x 128 x 216 + 128 x 72 = 64,512 of the SM's 65,536.  With
+// 72 the epilogue's row loop fits unrolled once, without spills.
+constexpr int kMmaRegs = 216, kEpiRegs = 72;
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 };
 
@@ -70,17 +95,23 @@ struct Args {
 __host__ __device__ constexpr int stage_bytes(int passes) {
   return (passes == 3 ? 2 : 1) * kTileBytes + kATileBytes;
 }
-// Stages that fit beside the [8][colsum_cols] column-sum accumulator and the 1 KB alignment
-// slack; at most kMaxStages.  The one place that sizes the shared memory of a launch.
-__host__ __device__ constexpr int num_stages(int passes, int colsum_cols) {
-  return (kSmemLimit - 1024 - kWarps * colsum_cols * 4) / stage_bytes(passes) < kMaxStages
-             ? (kSmemLimit - 1024 - kWarps * colsum_cols * 4) / stage_bytes(passes)
+// What follows the stages: the staging tile of a staged kernel (its column sums live in
+// global memory), else the [8][colsum_cols] column-sum accumulator.
+__host__ __device__ constexpr int tail_bytes(int colsum_cols, bool staged) {
+  return staged ? kStagingBytes : kWarps * colsum_cols * 4;
+}
+// Stages that fit beside the tail and the 1 KB alignment slack; at most kMaxStages.  The one
+// place that sizes the shared memory of a launch.
+__host__ __device__ constexpr int num_stages(int passes, int colsum_cols, bool staged) {
+  return (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes) < kMaxStages
+             ? (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes)
              : kMaxStages;
 }
-static_assert(num_stages(3, 1024) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
-inline size_t smem_bytes(int passes, int colsum_cols) {
-  return (size_t)num_stages(passes, colsum_cols) * stage_bytes(passes) +
-         (size_t)kWarps * colsum_cols * sizeof(float) + 1024;
+static_assert(num_stages(3, 1024, false) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
+static_assert(num_stages(3, 1024, true) >= 3, "3xTF32 needs three stages beside the staging tile");
+inline size_t smem_bytes(int passes, int colsum_cols, bool staged) {
+  return (size_t)num_stages(passes, colsum_cols, staged) * stage_bytes(passes) +
+         (size_t)tail_bytes(colsum_cols, staged) + 1024;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -141,6 +172,21 @@ __device__ __forceinline__ void cp_async_commit() {
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// Every warp of a warpgroup executes these.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
 }
 
 #define TFR_WG_D32                                                                           \
@@ -271,11 +317,190 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return r;
 }
 
+// The epilogue warpgroup of a staged kernel: walks the CTA's tiles as the MMA warpgroups do and
+// finishes each from the staging tile `stg`.  Warp `ew` takes rows 32 ew .. 32 ew + 31, a lane
+// 4 adjacent columns of each, so a row is stored as one 512-byte line and the eight lanes of a
+// 32-column chunk assemble its sign word with one redux.  Column tests are made once per tile,
+// row tests once per row.  Column sums: the row pass writes the stored fp32 values back to the
+// staging tile; thread t then owns tile column t, adds the 16 rows of each of the 8 row groups
+// in the order the accumulator layout gave them (rows g and g + 8, then g pairs 1, 2, 4 apart)
+// and adds that to its running sum in the group's slot in global memory.  Slot and column
+// always meet the same thread, so plain loads and stores keep the running sums.
+template <bool OUT_BF16>
+__device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg) {
+  const int lane = threadIdx.x & 31;
+  const int et = threadIdx.x - kThreads, ew = et >> 5;
+  const int tiles_mn = args.m_tiles * args.n_tiles;
+  const int total = tiles_mn * args.splits;
+  if (args.colsum_cols) {
+    for (int w = 0; w < kWarps; ++w) {
+      float* dst = args.colsum + static_cast<size_t>(blockIdx.x * kWarps + w) * args.colsum_stride;
+      for (int c = et; c < args.GN; c += kEpiThreads) dst[c] = 0.f;
+    }
+  }
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const int z = tile / tiles_mn;
+    const int r = tile - z * tiles_mn;
+    const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
+    const int col = n0 + 4 * lane;
+    const int live = min(max(args.GN - col, 0), 4);   // live columns of this lane
+    float b4[4] = {0.f, 0.f, 0.f, 0.f};
+    if (args.epi == EPI_BIAS_ACT) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (j < live) b4[j] = __ldg(args.bias + col + j);
+    }
+    float* Cf = static_cast<float*>(args.C) + static_cast<size_t>(z) * args.split_stride;
+    __nv_bfloat16* Cb = static_cast<__nv_bfloat16*>(args.C);
+    // vector stores need a row pitch of a multiple of 4 elements and a 16-byte (bf16: 8-byte)
+    // aligned base (C and every split-K slice C + z * split_stride)
+    const uintptr_t cbase = OUT_BF16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
+    const bool vec_ok = (args.ldc % 4) == 0 && (cbase & (OUT_BF16 ? 7u : 15u)) == 0;
+    const bool vec4 = live == 4 && vec_ok;
+    const uint32_t* bin = args.epi == EPI_MASK_BITS && live > 0
+                              ? args.bits_in + static_cast<size_t>(col >> 5) * args.GM : nullptr;
+    uint32_t* bout = args.bits_out && (lane & 7) == 0 && live > 0
+                         ? args.bits_out + static_cast<size_t>(col >> 5) * args.GM : nullptr;
+    bar_sync(kBarFull, kThreads + kEpiThreads);
+    // Full row blocks whose lanes hold 4 live columns or none, stored as vectors: the row loop
+    // has no bounds tests, its epilogue kind is a compile-time constant and its pointers advance
+    // by a constant per row.  Everything else takes the general loop below it.
+    auto fast_rows = [&](auto kind) {
+      constexpr int EPI = decltype(kind)::value;
+      using V = std::conditional_t<OUT_BF16, uint2, float4>;
+      const bool on = live == 4, relu = args.act == TFR_ACT_RELU;
+      const int row0 = m0 + ew * 32;
+      const float4* sp = reinterpret_cast<const float4*>(stg + ew * 32 * kStagingPitch + 4 * lane);
+      const size_t coff = static_cast<size_t>(row0) * args.ldc + col;
+      V* cp = OUT_BF16 ? reinterpret_cast<V*>(Cb + coff) : reinterpret_cast<V*>(Cf + coff);
+      const int cstep = args.ldc / 4;
+      const uint32_t* bi = bin ? bin + row0 : nullptr;
+      uint32_t* bo = bout ? bout + row0 : nullptr;
+      const int sh = (4 * lane) & 31;
+#pragma unroll 4
+      for (int i = 0; i < 32; ++i) {
+        float4 v = sp[i * (kStagingPitch / 4)];
+        if (EPI == EPI_BIAS_ACT) {
+          v.x += b4[0]; v.y += b4[1]; v.z += b4[2]; v.w += b4[3];
+          if (relu) {
+            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+          }
+        } else if (EPI == EPI_MASK_BITS) {
+          const uint32_t w = on ? __ldg(bi + i) >> sh : 0u;
+          if (!(w & 1u)) v.x = 0.f;
+          if (!(w & 2u)) v.y = 0.f;
+          if (!(w & 4u)) v.z = 0.f;
+          if (!(w & 8u)) v.w = 0.f;
+        }
+        if (!on) v = make_float4(0.f, 0.f, 0.f, 0.f);
+        const uint2 packed = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+        if (args.bits_out) {
+          auto pos = [](float y) {   // the sign bit is that of the stored value
+            return (OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(y)) : y) > 0.f ? 1u : 0u;
+          };
+          const uint32_t nib = pos(v.x) | pos(v.y) << 1 | pos(v.z) << 2 | pos(v.w) << 3;
+          const uint32_t w = __reduce_or_sync(0xffu << (lane & 24), nib << (4 * (lane & 7)));
+          if (bo) bo[i] = w;
+        }
+        if (args.colsum_cols) const_cast<float4*>(sp)[i * (kStagingPitch / 4)] = v;
+        if (on) {
+          if (OUT_BF16) *reinterpret_cast<uint2*>(cp + static_cast<size_t>(i) * cstep) = packed;
+          else *reinterpret_cast<float4*>(cp + static_cast<size_t>(i) * cstep) = v;
+        }
+      }
+    };
+    const bool fast = m0 + BM <= args.GM && (args.GN % 4) == 0 && vec_ok && !args.store_transposed;
+    bool general = false;
+    if (fast && args.epi == EPI_STORE) fast_rows(std::integral_constant<int, EPI_STORE>{});
+    else if (fast && args.epi == EPI_BIAS_ACT) fast_rows(std::integral_constant<int, EPI_BIAS_ACT>{});
+    else if (fast && args.epi == EPI_MASK_BITS) fast_rows(std::integral_constant<int, EPI_MASK_BITS>{});
+    else general = true;
+#pragma unroll 1
+    for (int i = general ? 0 : 32; i < 32; ++i) {
+      const int rl = ew * 32 + i, row = m0 + rl;
+      const bool rlive = row < args.GM;
+      float* sp = stg + rl * kStagingPitch + 4 * lane;
+      const float4 v = *reinterpret_cast<const float4*>(sp);
+      float x[4] = {v.x, v.y, v.z, v.w};
+      uint32_t wbits = 0u, nib = 0u;
+      if (bin && rlive) wbits = __ldg(bin + row);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float y = x[j];
+        if (args.epi == EPI_BIAS_ACT) {
+          y += b4[j];
+          if (args.act == TFR_ACT_RELU) y = fmaxf(y, 0.f);
+        } else if (args.epi == EPI_MASK_POS) {
+          if (args.act == TFR_ACT_RELU && rlive && j < live &&
+              !(__ldg(args.aux + static_cast<size_t>(row) * args.ldc + col + j) > 0.f))
+            y = 0.f;
+        } else if (args.epi == EPI_MASK_BITS) {
+          if (!((wbits >> ((4 * lane + j) & 31)) & 1u)) y = 0.f;
+        }
+        if (!rlive || j >= live) y = 0.f;
+        x[j] = y;   // column sums take the fp32 value, sign bits the stored one
+        const float stored = OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(y)) : y;
+        nib |= (stored > 0.f ? 1u : 0u) << j;
+      }
+      if (args.bits_out) {
+        const uint32_t w = __reduce_or_sync(0xffu << (lane & 24), nib << (4 * (lane & 7)));
+        if (bout && rlive) bout[row] = w;
+      }
+      if (args.colsum_cols) *reinterpret_cast<float4*>(sp) = make_float4(x[0], x[1], x[2], x[3]);
+      if (!rlive || live == 0) continue;
+      if (OUT_BF16) {
+        __nv_bfloat16* p = Cb + static_cast<size_t>(row) * args.ldc + col;
+        if (vec4) {
+          *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]));
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (j < live) p[j] = __float2bfloat16_rn(x[j]);
+        }
+      } else if (args.store_transposed) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (j < live) Cf[static_cast<size_t>(col + j) * args.ldc + row] = x[j];
+      } else {
+        float* p = Cf + static_cast<size_t>(row) * args.ldc + col;
+        if (vec4) {
+          *reinterpret_cast<float4*>(p) = make_float4(x[0], x[1], x[2], x[3]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (j < live) p[j] = x[j];
+        }
+      }
+    }
+    if (args.colsum_cols) {
+      bar_sync(kBarEpi, kEpiThreads);   // the write-backs of all four warps
+      if (n0 + et < args.GN) {
+#pragma unroll
+        for (int w = 0; w < kWarps; ++w) {
+          const float* p = stg + w * 16 * kStagingPitch + et;
+          float s[8];
+#pragma unroll
+          for (int g = 0; g < 8; ++g) s[g] = p[g * kStagingPitch] + p[(g + 8) * kStagingPitch];
+          const float sum = ((s[0] + s[1]) + (s[2] + s[3])) + ((s[4] + s[5]) + (s[6] + s[7]));
+          float* dst = args.colsum + static_cast<size_t>(blockIdx.x * kWarps + w) * args.colsum_stride +
+                       n0 + et;
+          *dst += sum;
+        }
+      }
+    }
+    if (tile + gridDim.x < total) bar_arrive(kBarFree, kThreads + kEpiThreads);
+  }
+}
+
 // PASSES: 1 (one product) or 3 (3xTF32: Ahi Bhi + Alo Bhi + Ahi Blo; float only).
 // PRE_B: B comes pre-split (B = hi parts, B_lo = lo parts).  OUT_BF16: C is bf16 (row-major).
-// Shared memory: num_stages x {B hi, [B lo,] A}, then [8][colsum_cols] floats.
+// Staged (K-major A): a third warpgroup runs the epilogue from a staging tile.
+// Shared memory: num_stages x {B hi, [B lo,] A}, then the staging tile (staged) or
+// [8][colsum_cols] floats.
 template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
-__global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
+__global__ void __launch_bounds__(A_MN ? kThreads : kThreads + kEpiThreads, 1)
+gemm_kernel(const Args args) {
+  constexpr bool STAGED = !A_MN;
   constexpr bool F32 = sizeof(T) == 4;
   constexpr int EPC = Elem<T>::EPC;
   constexpr int BK = Elem<T>::BK;
@@ -290,8 +515,20 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
   static_assert(!PRE_B || P3, "pre-split B is 3xTF32");
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int stages = num_stages(PASSES, args.colsum_cols);
-  float* cacc = reinterpret_cast<float*>(smem + stages * kStage);
+  const int stages = num_stages(PASSES, args.colsum_cols, STAGED);
+  float* cacc = reinterpret_cast<float*>(smem + stages * kStage);   // staged: the staging tile
+  if (STAGED) {
+    if (threadIdx.x >= kThreads) {
+      setmaxnreg_dec<kEpiRegs>();
+      epilogue_warpgroup<OUT_BF16>(args, cacc);
+      return;
+    }
+    setmaxnreg_inc<kMmaRegs>();
+  }
+  auto mma_sync = [] {   // barrier over the MMA warpgroups
+    if (STAGED) bar_sync(kBarMma, kThreads);
+    else __syncthreads();
+  };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2, wq = warp & 3;   // warpgroup, warp within it
@@ -303,7 +540,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
   const int total = tiles_mn * args.splits;
   const uint32_t smem_base = smem_u32(smem);
 
-  for (int c = threadIdx.x; c < kWarps * args.colsum_cols; c += kThreads) cacc[c] = 0.f;
+  if (!STAGED)
+    for (int c = threadIdx.x; c < kWarps * args.colsum_cols; c += kThreads) cacc[c] = 0.f;
 
   // Issues the cp.async copies of k block kb (relative to the split) of the tile at (m0, n0)
   // into stage s: 4 chunks of A and, unless register-staged, 4 chunks of B (and 4 of B lo).
@@ -419,7 +657,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
         }
       }
       fence_proxy_async();   // cp.async and st.shared writes -> visible to the tensor cores
-      __syncthreads();
+      mma_sync();
       {
         const int nb = kb + stages - 2;
         if (nb < nkb) copy_block(m0, n0, kb0, nb, s >= 2 ? s - 2 : s + stages - 2);
@@ -529,12 +767,27 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
     }
     wgmma_wait<0>();
     // every warpgroup is done with the stages: start the next tile's copies, then the epilogue
-    __syncthreads();
+    mma_sync();
     if (tile + gridDim.x < total) prologue(tile + gridDim.x);
 
-    // ---------------------------------------------------------------- epilogue ----
     // accumulator element j of half h: row = 16 wq + lane / 4 + 8 ((j / 2) % 2),
     // column = 64 h + 8 (j / 4) + 2 (lane % 4) + j % 2
+    if (STAGED) {
+      // hand the raw accumulators to the epilogue warpgroup, once it has read the last tile
+      if (tile != static_cast<int>(blockIdx.x)) bar_sync(kBarFree, kThreads + kEpiThreads);
+      float* sp = cacc + (wg * 64 + wq * 16 + (lane >> 2)) * kStagingPitch + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (h == 1 && !two_n) break;   // columns past GN: the epilogue does not use them
+#pragma unroll
+        for (int j = 0; j < 32; j += 2)
+          *reinterpret_cast<float2*>(sp + 8 * ((j >> 1) & 1) * kStagingPitch + h * 64 + 8 * (j >> 2)) =
+              make_float2(acc[h][j], acc[h][j + 1]);
+      }
+      bar_arrive(kBarFull, kThreads + kEpiThreads);
+      continue;
+    }
+    // ------------------------------------------- epilogue on the accumulator registers ----
     const int rbase = m0 + wg * 64 + wq * 16 + (lane >> 2);
     float* Cf = static_cast<float*>(args.C) + static_cast<size_t>(z) * args.split_stride;
     __nv_bfloat16* Cb = static_cast<__nv_bfloat16*>(args.C);
@@ -642,7 +895,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_kernel(const Args args) {
       }
     }
   }
-  if (args.colsum_cols) {
+  if (!STAGED && args.colsum_cols) {
     __syncwarp();
     float* dst = args.colsum + static_cast<size_t>(blockIdx.x * kWarps + warp) * args.colsum_stride;
     for (int c = lane; c < args.GN; c += 32) dst[c] = cacc[warp * args.colsum_cols + c];
@@ -661,10 +914,10 @@ int launch(Args a, cudaStream_t st, int* ctas) {
   const int sms = num_sms();
   const int grid = total < sms ? total : sms;
   if (ctas) *ctas = grid;
-  const size_t smem = smem_bytes(PASSES, a.colsum_cols);
+  const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN);
   auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16>;
   TFR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, kThreads, smem, st>>>(a);
+  kern<<<grid, A_MN ? kThreads : kThreads + kEpiThreads, smem, st>>>(a);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

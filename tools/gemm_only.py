@@ -1,7 +1,8 @@
 """Times the eight scorer GEMMs of the config-2 training step (fwd1-3, dz1-2, dw1-3) through
 the 3xTF32 engine, with the shapes, orientations and split-K counts the trainer uses, and
 prints per GEMM the time, the algorithmic TFLOP/s (2 GM GN GK) and the GB/s of the tensors it
-must move (operands read once, output and sign words written once).  dw1t-dw3t time the dW
+must move (operands read once, output and sign words written once), and from the shapes the
+time per 128 x 128 tile of a CTA (time x CTAs / tiles) and per 32-wide k block of it.  dw1t-dw3t time the dW
 GEMMs as they would run on a transposed dZ (dZ^T [width][M]): direct orientation, A the
 MN-major activations, B = dZ^T K-major, copied by cp.async and split in shared memory; same
 shapes and split-K count as dw1-dw3.  The last line times the
@@ -28,6 +29,14 @@ def splits_for(m, sms):     # rows_per_split / splits of the dW GEMMs (capi.cu)
   per = (m + sms - 1) // sms
   rows = 256 if per < 256 else (per + 127) // 128 * 128
   return (m + rows - 1) // rows
+
+
+def per_tile(gm, gn, gk, splits, sms, us):
+  """(tiles per CTA, k blocks per tile, us per tile, us per k block) on the persistent grid."""
+  tiles = ((gm + 127) // 128) * ((gn + 127) // 128) * splits
+  per_cta = tiles / min(tiles, sms)
+  kb = ((gk + 31) // 32 + splits - 1) // splits
+  return per_cta, kb, us / per_cta, us / per_cta / kb
 
 
 def shapes(sms):
@@ -94,12 +103,16 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / args.reps
+    per_cta, kb, us_tile, us_kb = per_tile(*shape, sms, us)
     rows.append(dict(gemm=name, gm=shape[0], gn=shape[1], gk=shape[2], splits=shape[3],
                      us=round(us, 2), tflops=round(flop / us * 1e-6, 2),
-                     gbps=round(nbytes / us * 1e-3, 1)))
-    print('%-5s GM %6d GN %4d GK %6d splits %4d  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s' % (
-        name, shape[0], shape[1], shape[2], shape[3], us, rows[-1]['tflops'], rows[-1]['gbps']),
-          flush=True)
+                     gbps=round(nbytes / us * 1e-3, 1), tiles_per_cta=round(per_cta, 2),
+                     k_blocks_per_tile=kb, us_per_tile=round(us_tile, 2),
+                     us_per_k_block=round(us_kb, 2)))
+    print('%-5s GM %6d GN %4d GK %6d splits %4d  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s  '
+          '%5.1f tiles/CTA x %3d k blocks: %6.2f us/tile %5.2f us/block' % (
+              name, shape[0], shape[1], shape[2], shape[3], us, rows[-1]['tflops'],
+              rows[-1]['gbps'], per_cta, kb, us_tile, us_kb), flush=True)
   step = [r for r in rows if not r['gemm'].endswith('t')]   # the eight GEMMs the step runs
   total = sum(r['us'] for r in step)
   print('total %.1f us' % total, flush=True)
