@@ -221,6 +221,48 @@ int tfr_ordinal_loss_fwd_bwd(const float* scores, const float* labels,
                              void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K3d  Click-model losses, fused forward + backward, one CTA per list, no float atomics
+ * (two identical calls give identical bits).  Limits: 1 <= N <= 8192, temperature > 0.
+ *
+ * ClickEMLoss (losses_impl.py:1324-1422): examination logits e and relevance logits r,
+ * element (b, i) at exam[(b N + i) stride] and rel[(b N + i) stride], stride 1 (two [B, N]
+ * planes) or 2 (the Keras [B, N, 2] tensor in place: exam = base, rel = base + 1).
+ *   valid_i = mask_i (if given) and label_i >= 0;  c_i = label_i >= 1 (clicked)
+ *   e, r = e_i / T, r_i / T, both 0 on invalid items
+ *   pe_i = c_i ? 1 : sigmoid(e - softplus(r)),  pr_i = c_i ? 1 : sigmoid(r - softplus(e))
+ *          (posteriors; no gradient flows through them)
+ *   loss_i = exam_weight * sce(pe_i, e) + rel_weight * sce(pr_i, r),
+ *          sce(z, x) = max(x, 0) - x z + log1p(exp(-|x|))
+ *   w_i = valid_i ? item weight : 0;  row[b, i] = loss_i w_i (optional),
+ *   loss[b] = sum_i row, weight[b] = sum_i w_i, nonzero[b] = #{w_i != 0} (optional);
+ *   d_exam = grad_scale exam_weight (sigmoid(e) - pe_i) w_i / T,
+ *   d_rel  = grad_scale rel_weight (sigmoid(r) - pr_i) w_i / T, written with the input
+ *   stride (both optional, both or neither); exactly 0 on invalid items.
+ *
+ * MixtureEMLoss (losses_impl.py:1472-1538): scores [B, N, M], 1 <= M <= 32 mixed models.
+ *   valid_i = mask_i (if given) else label_i >= 0;  l_im = valid_i ? sce(label_i, s_im / T) : 0
+ *   L_m = sum_i l_im (fp64),  q_m = exp(-alpha (L_m - min_k L_k)) (no gradient)
+ *   loss[b] = sum_m q_m L_m / sum_m q_m
+ *   weight[b] = list weight (sum_i w_i l_i / sum_i l_i over label_i >= 0, 1 without item_w;
+ *               :1004-1015) x [sum of the valid labels > 0]
+ *   grad[b, i, m] = grad_scale valid_i q_m / sum q (sigmoid(s_im / T) - label_i) / T
+ *
+ * Both return TFR_INVALID_ARGUMENT before any CUDA call for NULL inputs, N outside 1..8192,
+ * M outside 1..32 or a stride other than 1 or 2.
+ * ------------------------------------------------------------------------- */
+int tfr_click_em_loss_fwd_bwd(const float* exam, const float* rel, int stride,
+                              const float* labels, const float* item_w, int w_per_item,
+                              const uint8_t* mask, int B, int N, float temperature,
+                              float exam_weight, float rel_weight, float grad_scale,
+                              float* d_exam, float* d_rel, float* row, float* loss,
+                              float* weight, float* nonzero, void* stream);
+int tfr_mixture_em_loss_fwd_bwd(const float* scores, const float* labels,
+                                const float* item_w, int w_per_item, const uint8_t* mask,
+                                int B, int N, int M, float temperature, float alpha,
+                                float grad_scale, float* grad, float* loss, float* weight,
+                                void* stream);
+
+/* ---------------------------------------------------------------------------
  * GumbelSampler.sample (losses_impl.py:540-649): `sample_size` perturbed copies of
  * every list; row b * sample_size + s of out_logits [B * sample_size, N] is
  *   log(softmax((scores[b] + G) / temperature) + 1e-20),

@@ -111,6 +111,10 @@ _SIGNATURES = {
                                     _P]),
     'tfr_ordinal_loss_fwd_bwd': (_I, [_P, _P, _P, _I, _P, _I, _I, _I, _F, _I, _F, _P, _P, _P,
                                       _P, _P, _P]),
+    'tfr_click_em_loss_fwd_bwd': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _I, _F, _F, _F, _F,
+                                       _P, _P, _P, _P, _P, _P, _P]),
+    'tfr_mixture_em_loss_fwd_bwd': (_I, [_P, _P, _P, _I, _P, _I, _I, _I, _F, _F, _F, _P, _P,
+                                         _P, _P]),
     'tfr_gumbel_sample': (_I, [_P, _P, _I, _I, _I, _F, C.c_uint64, _I, _P, _P, _P, _P]),
     'tfr_rank_metrics': (_I, [_P, _P, _P, _I, _P, _I, _I, C.POINTER(C.c_int32),
                               _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -558,6 +558,77 @@ class OrdinalLoss(_PointwiseLoss):
     raise NotImplementedError('OrdinalLoss needs a multi-head scorer; use autograd')
 
 
+class ClickEMLoss(_PointwiseLoss):
+  """keras/losses.py:1344-1418: y_pred [B, N, 2] (examination, relevance logits), y_true
+  clicks.  A pointwise loss: AUTO / SUM_OVER_BATCH_SIZE divide the summed item losses by
+  B * N, padded slots included.  Not a RankingLossKey member (neither is it in the
+  reference), so `get` does not build it."""
+
+  def __init__(self, reduction=Reduction.AUTO, name=None, exam_loss_weight=1.0,
+               rel_loss_weight=1.0, ragged=False):
+    super().__init__(reduction, name, ragged)
+    self._exam_loss_weight = exam_loss_weight
+    self._rel_loss_weight = rel_loss_weight
+    self._loss = losses_impl.ClickEMLoss(
+        name='{}_impl'.format(name) if name else None, exam_loss_weight=exam_loss_weight,
+        rel_loss_weight=rel_loss_weight, ragged=ragged)
+
+  def fused_fwd_bwd(self, y_true, exam, rel, sample_weight, d_exam, d_rel, per_list, total2):
+    """Training fast path over two [B, N] logit planes (the examination and relevance
+    logits of a two-tower model): ONE launch writes d loss / d exam and d loss / d rel
+    (already divided by the Keras normaliser) into `d_exam` / `d_rel` and the per-list loss
+    sums into `per_list[0]`; a second tiny launch reduces the scalar loss into `total2[0]`."""
+    labels, rel = losses_impl._prep_2d(y_true, rel)
+    exam = losses_impl._as_f32(exam, what='exam logits')
+    if exam.shape != rel.shape:
+      raise ValueError('exam and rel logits must have the same shape')
+    w, wpi = losses_impl._prep_weights(sample_weight, rel)
+    b, n = rel.shape
+    scale = 1.0 if self.reduction == Reduction.SUM else 1.0 / float(b * n)
+    _C.check(_C.lib.tfr_click_em_loss_fwd_bwd(
+        _C.ptr(exam), _C.ptr(rel), 1, _C.ptr(labels), _C.ptr(w), wpi, None, b, n,
+        float(self._loss._temperature), float(self._exam_loss_weight),
+        float(self._rel_loss_weight), scale, _C.ptr(d_exam), _C.ptr(d_rel), None,
+        _C.ptr(per_list[0]), _C.ptr(per_list[1]), None, _C.stream()))
+    _C.check(_C.lib.tfr_weighted_sum(_C.ptr(per_list[0]), None, b, scale,
+                                     _C.ptr(total2), _C.stream()))
+
+  def get_config(self):
+    config = super().get_config()
+    config.update({'exam_loss_weight': self._exam_loss_weight,
+                   'rel_loss_weight': self._rel_loss_weight})
+    return config
+
+
+class MixtureEMLoss(_RankingLoss):
+  """keras/losses.py:1421-1496: y_pred [B, N, model_num], y_true clicks.  As in the
+  reference, `lambda_weight` and `temperature` are accepted and kept in the config but the
+  loss is built without them (keras/losses.py:1484-1489), so neither changes its value."""
+
+  def __init__(self, reduction=Reduction.AUTO, name=None, lambda_weight=None,
+               temperature=1.0, alpha=1.0, ragged=False):
+    super().__init__(reduction, name, ragged)
+    self._lambda_weight = lambda_weight
+    self._temperature = temperature
+    self._alpha = alpha
+    self._loss = losses_impl.MixtureEMLoss(
+        name='{}_impl'.format(name) if name else None, alpha=alpha, ragged=ragged)
+
+  def __call__(self, y_true, y_pred, sample_weight=None):
+    losses, weights = self._loss._run(y_true, y_pred, sample_weight, None,
+                                      self._loss._temperature)
+    return _keras_reduce((losses * weights).unsqueeze(1), None, self.reduction)
+
+  def fused_fwd_bwd(self, *args, **kwargs):
+    raise NotImplementedError('MixtureEMLoss needs a multi-head scorer; use autograd')
+
+  def get_config(self):
+    config = super().get_config()
+    config.update({'lambda_weight': self._lambda_weight, 'temperature': self._temperature,
+                   'alpha': self._alpha})
+    return config
+
+
 _KEY_TO_CLS = {
     RankingLossKey.COUPLED_RANKDISTIL_LOSS: CoupledRankDistilLoss,
     RankingLossKey.ORDINAL_LOSS: OrdinalLoss,

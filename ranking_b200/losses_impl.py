@@ -852,6 +852,135 @@ class OrdinalLoss(_PointwiseLoss):
 
 
 # ----------------------------------------------------------------------------
+# ClickEMLoss / MixtureEMLoss  (tfr_click_em_loss_fwd_bwd / tfr_mixture_em_loss_fwd_bwd, K3d)
+# ----------------------------------------------------------------------------
+class _ClickEMFn(torch.autograd.Function):
+  """(loss[B], weight[B], nonzero[B], row[B, N]) of ClickEM from one K3d launch over the
+  [B, N, 2] logits (stride 2); the gradient is produced by the same launch."""
+
+  @staticmethod
+  def forward(ctx, logits, labels, w, w_per_item, mask, temperature, exam_w, rel_w):
+    b, n, _ = logits.shape
+    dev = logits.device
+    grad = torch.empty_like(logits)
+    loss = torch.empty(b, dtype=torch.float32, device=dev)
+    weight = torch.empty_like(loss)
+    nonzero = torch.empty_like(loss)
+    row = torch.empty(b, n, dtype=torch.float32, device=dev)
+    base = logits.data_ptr()
+    gbase = grad.data_ptr()
+    _C.check(_C.lib.tfr_click_em_loss_fwd_bwd(
+        base, base + 4, 2, _C.ptr(labels), _C.ptr(w), w_per_item, _C.ptr(mask), b, n,
+        float(temperature), float(exam_w), float(rel_w), 1.0, gbase, gbase + 4, _C.ptr(row),
+        _C.ptr(loss), _C.ptr(weight), _C.ptr(nonzero), _C.stream()))
+    ctx.set_materialize_grads(False)
+    ctx.save_for_backward(grad)
+    ctx.mark_non_differentiable(weight, nonzero)
+    return loss, weight, nonzero, row
+
+  @staticmethod
+  def backward(ctx, g_loss, _gw, _gn, g_row):
+    # d loss[b] / d logits = grad; d row[b, i] / d logits[b, i, :] = grad[b, i, :]
+    grad, = ctx.saved_tensors
+    out = None
+    if g_loss is not None:
+      out = grad * g_loss.reshape(-1, 1, 1)
+    if g_row is not None:
+      out = grad * g_row.unsqueeze(2) if out is None else out + grad * g_row.unsqueeze(2)
+    return out, None, None, None, None, None, None, None
+
+
+def _prep_3d(labels, logits, what):
+  logits = _as_f32(logits, what='logits')
+  if logits.dim() != 3:
+    raise ValueError('Predictions for %s must have rank 3.' % what)
+  labels = _as_f32(labels, logits.device, 'labels')
+  if labels.shape != logits.shape[:2]:
+    raise ValueError('labels must have shape [batch_size, list_size]; got %s for logits %s' %
+                     (tuple(labels.shape), tuple(logits.shape)))
+  return labels, logits
+
+
+class ClickEMLoss(_PointwiseLoss):
+  """losses_impl.py:1324-1422: logits [B, N, 2], [..., 0] the examination logits and
+  [..., 1] the relevance logits; labels are clicks (>= 1 clicked, < 0 padding).
+  `compute_unreduced_loss` returns losses that are 0 on invalid items (the reference's
+  value there is finite but always multiplied by a zero weight)."""
+
+  def __init__(self, name=None, temperature=1.0, exam_loss_weight=1.0, rel_loss_weight=1.0,
+               ragged=False):
+    super().__init__(name, None, temperature, ragged)
+    self._exam_loss_weight = exam_loss_weight
+    self._rel_loss_weight = rel_loss_weight
+
+  def _run(self, labels, logits, weights, mask, temperature):
+    labels, logits, weights, mask = self._densify(labels, logits, weights, mask)
+    labels, logits = _prep_3d(labels, logits, 'click EM loss')
+    if logits.shape[-1] != 2:
+      raise ValueError('The last dimension of logits must be 2 (examination and relevance '
+                       'logits), the actual dimension is {}.'.format(logits.shape[-1]))
+    w, wpi = _prep_weights(weights, labels)
+    m = _prep_mask(mask, labels)
+    return _ClickEMFn.apply(logits, labels, w, wpi, m, temperature, self._exam_loss_weight,
+                            self._rel_loss_weight)
+
+  def compute_unreduced_loss(self, labels, logits, mask=None):
+    """losses_impl.py:709-726: (losses [B, N], loss weights = mask [B, N])."""
+    row = self._run(labels, logits, None, mask, 1.0)[3]
+    if self._ragged:
+      mask = self._densify(labels, None, None, None)[3]
+    elif mask is None:
+      mask = _as_f32(labels, row.device, 'labels') >= 0
+    return row, torch.as_tensor(mask, device=row.device).to(torch.float32)
+
+
+class _MixtureEMFn(torch.autograd.Function):
+  """(loss[B], weight[B]) of MixtureEM from one K3d launch over [B, N, M] logits."""
+
+  @staticmethod
+  def forward(ctx, logits, labels, w, w_per_item, mask, temperature, alpha):
+    b, n, m = logits.shape
+    grad = torch.empty_like(logits)
+    loss = torch.empty(b, dtype=torch.float32, device=logits.device)
+    weight = torch.empty_like(loss)
+    _C.check(_C.lib.tfr_mixture_em_loss_fwd_bwd(
+        _C.ptr(logits), _C.ptr(labels), _C.ptr(w), w_per_item, _C.ptr(mask), b, n, m,
+        float(temperature), float(alpha), 1.0, _C.ptr(grad), _C.ptr(loss), _C.ptr(weight),
+        _C.stream()))
+    ctx.set_materialize_grads(False)
+    ctx.save_for_backward(grad)
+    ctx.mark_non_differentiable(weight)
+    return loss, weight
+
+  @staticmethod
+  def backward(ctx, g_loss, _gw):
+    grad, = ctx.saved_tensors
+    out = None if g_loss is None else grad * g_loss.reshape(-1, 1, 1)
+    return out, None, None, None, None, None, None
+
+
+class MixtureEMLoss(_ListwiseLoss):
+  """losses_impl.py:1472-1538: logits [B, N, model_num] (1 <= model_num <= 32), one column
+  per mixed click model; labels are clicks."""
+
+  def __init__(self, name=None, temperature=1.0, alpha=1.0, ragged=False):
+    super().__init__(name, None, temperature, ragged)
+    self._alpha = alpha
+
+  def _run(self, labels, logits, weights, mask, temperature):
+    labels, logits, weights, mask = self._densify(labels, logits, weights, mask)
+    labels, logits = _prep_3d(labels, logits, 'mixture EM loss')
+    w, wpi = _prep_weights(weights, labels)
+    m = _prep_mask(mask, labels)
+    return _MixtureEMFn.apply(logits, labels, w, wpi, m, temperature, self._alpha)
+
+  def compute_unreduced_loss(self, labels, logits, mask=None):
+    """losses_impl.py:709-726: (losses [B, 1], loss weights [B, 1])."""
+    loss, weight = self._run(labels, logits, None, mask, 1.0)
+    return loss.unsqueeze(1), weight.unsqueeze(1)
+
+
+# ----------------------------------------------------------------------------
 # CoupledRankDistilLoss (losses_impl.py:1984-2116)
 # ----------------------------------------------------------------------------
 class CoupledRankDistilLoss(_ListwiseLoss):

@@ -638,3 +638,122 @@ class EmbeddingRankingTrainer(RankingTrainer):
       if ti not in written:     # a table no feature reads: zero gradient
         off = sc.table_offsets[ti]
         grads[off:off + emb.flat.numel()].zero_()
+
+
+class ClickEMRankingTrainer(RankingTrainer):
+  """Learns a relevance scorer from position-biased clicks, jointly with a per-position
+  examination propensity: the examination x relevance click model of Wang et al. 2018
+  (losses_impl.py:1324-1422) trained online, as the reference's ClickEMLoss does with a
+  two-tower model.
+
+      exam = table[position]                 tfr_embedding_fwd (one id per item, SUM)
+      rel  = tower(x)                        tfr_mlp_fwd
+      loss, d exam, d rel                    K3d ClickEM on the two [B, N] planes
+      tower gradients                        tfr_mlp_bwd
+      table gradient                         tfr_embedding_bwd (deterministic)
+      optimizer                              one launch over the shared flat buffer
+
+  `tower`: a create_tower tower with output_units 1 (precision fp32, tf32x3 or tf32; BN is
+  allowed, with circular padding as in the base class).  `loss`: a keras.losses.ClickEMLoss.
+  The position table is a keras.layers.TokenEmbedding(num_positions, 1, combiner='sum'); it
+  and the tower share one flat parameter buffer (_EmbeddingScorer), so checkpoints, the
+  optimizer and the data-parallel reducer cover it.  Its row count is rounded up to a
+  multiple of 64 so that the tower's parameters, which follow it, keep the 256-byte
+  alignment of a tower's own allocation; the extra rows are never read and keep their
+  initial values.  Labels are clicks (>= 1 clicked, < 0 padding).  `predict` returns the
+  relevance scores only, so pipeline.fit / evaluate work unchanged."""
+
+  _ROW_ALIGN = 64
+
+  def __init__(self, tower, loss, num_positions, seed=None, **kw):
+    from ranking_b200.keras import layers as keras_layers
+    from ranking_b200.keras import losses as keras_losses
+    if not isinstance(loss, keras_losses.ClickEMLoss):
+      raise ValueError('ClickEMRankingTrainer needs a keras.losses.ClickEMLoss')
+    if tower.precision not in ('fp32', 'tf32x3', 'tf32'):
+      raise ValueError('the click EM tower must use precision fp32, tf32x3 or tf32')
+    if tower.output_units != 1:
+      raise ValueError('the relevance tower needs output_units = 1')
+    num_positions = int(num_positions)
+    if num_positions < 1:
+      raise ValueError('num_positions must be >= 1')
+    rows = -(-num_positions // self._ROW_ALIGN) * self._ROW_ALIGN
+    self.num_positions = num_positions
+    self.positions_table = keras_layers.TokenEmbedding(rows, 1, combiner='sum', seed=seed,
+                                                       device=tower.flat.device)
+    self.mlp = tower
+    super().__init__(_EmbeddingScorer([self.positions_table], tower), loss, **kw)
+    self._pos = None
+    self._emb_ws = None
+
+  def _new_workspace(self, b, n):
+    dev = self.device
+    self.exam = torch.empty(b, n, dtype=torch.float32, device=dev)
+    self.dexam = torch.empty(b, n, dtype=torch.float32, device=dev)
+    self._default_pos = torch.arange(n, device=dev).clamp(max=self.num_positions - 1).to(
+        torch.int32).expand(b, n).contiguous()
+    self._emb_ws = torch.empty(
+        _C.lib.tfr_embedding_workspace_bytes(b * n, 1, self.positions_table.vocab_size, 1),
+        dtype=torch.uint8, device=dev)
+    return self.mlp._new_workspace(b * n)
+
+  def _set_positions(self, positions, b, n):
+    if positions is None:
+      self._pos = self._default_pos
+      return
+    if tuple(positions.shape) != (b, n):
+      raise ValueError('positions must have shape [batch_size, list_size] = %s, got %s' %
+                       ((b, n), tuple(positions.shape)))
+    pos = positions.to(self.device, torch.int32).contiguous()
+    if bool(((pos < 0) | (pos >= self.num_positions)).any()):
+      raise ValueError('positions must lie in [0, %d)' % self.num_positions)
+    self._pos = pos
+
+  def examination_propensity(self):
+    """sigmoid(table) [num_positions]: the learned P(examination | position)."""
+    return torch.sigmoid(self.positions_table.flat.detach()[:self.num_positions])
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    mlp = self.mlp
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(x), b * n, cfg, _C.ptr(mlp.flat.data), _C.ptr(m8),
+                                _C.ptr(self.ws), _C.ptr(self.scores), mlp._precision,
+                                _C.stream()))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    mlp, sc, emb = self.mlp, self.tower, self.positions_table
+    st = _C.stream()
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(x), b * n, cfg, _C.ptr(mlp.flat.data),
+                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.n_tables),
+                                mlp._precision, st))
+    _C.check(_C.lib.tfr_embedding_bwd(_C.ptr(self._pos), b * n, 1, _C.ptr(self.dexam), 1, 1,
+                                      emb.vocab_size, 1, emb._combiner, 0, _C.ptr(self._emb_ws),
+                                      _C.ptr(grads), None, st))
+
+  def train_step(self, x, clicks, positions=None, sample_weight=None, mask=None):
+    """x [B, N, D] (device, fp32), clicks [B, N] (>= 1 clicked, < 0 padding), positions
+    ([B, N] int in [0, num_positions), optional: by default an item's position is its row
+    in the list, clipped to num_positions - 1, i.e. the logged display order).  Returns the
+    scalar loss as a 0-d device tensor."""
+    b, n, _ = x.shape
+    self._ensure(b, n)
+    self._set_positions(positions, b, n)
+    x = self._prep_x(x)
+    cfg = ctypes.byref(self.tower._run_cfg(training=True))
+    m8 = None if mask is None else mask.reshape(-1).to(torch.uint8).contiguous()
+    grads = self.reducer.grads() if self.reducer is not None else self.grads
+    self.grads = grads
+    x = self._circular_pad(x, mask if mask is not None else (clicks >= 0))
+    emb = self.positions_table
+    st = _C.stream()
+    _C.check(_C.lib.tfr_embedding_fwd(_C.ptr(self._pos), b * n, 1, _C.ptr(emb.flat.data),
+                                      emb.vocab_size, 1, emb._combiner, 1, _C.ptr(self.exam), 1,
+                                      None, st))
+    self._forward(x, clicks, m8, cfg, True)
+    self.loss.fused_fwd_bwd(clicks, self.exam, self.scores, sample_weight, self.dexam,
+                            self.dscores, self.per_list, self.total2)
+    self._backward(x, m8, cfg, grads)
+    self._apply(grads)
+    return self.total2[0]
