@@ -34,6 +34,9 @@ int gemm(const GemmDesc& g, cudaStream_t st) {
   TFR_REQUIRE(g.epi != EPI_MASK_BITS || g.mask_bits_in, "tc gemm: mask_bits_in required");
   TFR_REQUIRE(!(g.mask_bits_out || g.epi == EPI_MASK_BITS) || (!g.store_transposed && splits == 1),
               "tc gemm: ReLU sign bits need a row-major, unsplit store");
+  // the folded remainder columns of this layout take plain stores only
+  TFR_REQUIRE(!(g.a_mn && g.b_mn) || (g.epi == EPI_STORE && !g.colsum),
+              "tc gemm: MN-major A and B (the dW layout) take the plain store epilogue");
 
   wg::Args a{};
   a.A = g.A; a.lda = g.lda; a.B = g.B; a.ldb = g.ldb; a.B_lo = g.B_lo;
@@ -51,6 +54,10 @@ int gemm(const GemmDesc& g, cudaStream_t st) {
   else rc = g.b_mn ? dispatch<true, true>(g, a, st, &ctas) : dispatch<true, false>(g, a, st, &ctas);
   if (rc == TFR_OK && g.colsum_slots_out) *g.colsum_slots_out = wg::kWarps * ctas;
   return rc;
+}
+
+int tile_units(int gm, int gn) {
+  return ((gm + wg::BM - 1) / wg::BM) * ((gn - wg::folded_cols(gn) + 63) / 64);
 }
 
 }  // namespace tc

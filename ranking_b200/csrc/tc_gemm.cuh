@@ -44,13 +44,15 @@ struct GemmDesc {
 };
 
 // Returns a tfr_status.  Requirements (checked): lda/ldb multiples of 4 floats,
-// 16-byte aligned base pointers, any GN (128-column output tiles).
+// 16-byte aligned base pointers, any GN (128-column output tiles), and the plain store
+// epilogue without column sums when A and B are both MN-major.
 int gemm(const GemmDesc& g, cudaStream_t stream);
 
-// Work units of a GM x GN output: 128-row tiles of one m64n128 (two units) or, when the
-// tile's live columns fit in 64, one m64n64 (one unit) per warpgroup and k step, each
-// walking the whole k range.  Picks the cheaper orientation of a dW GEMM.
-inline int tile_units(int gm, int gn) { return ((gm + 127) / 128) * ((gn + 63) / 64); }
+// Work units of a dW GEMM's GM x GN output (A and B MN-major): 128-row tiles of one m64n128
+// (two units) or, when the tile's live columns fit in 64, one m64n64 (one unit) per warpgroup
+// and k step, each walking the whole k range.  A remainder of up to 8 columns past the last
+// 128-column tile is folded into that tile and adds no unit.  Picks the cheaper orientation.
+int tile_units(int gm, int gn);
 
 }  // namespace tc
 }  // namespace tfr

@@ -2,7 +2,9 @@
 // the bf16 engine (tc_gemm_bf16.cu).
 //
 //   * a CTA owns a 128 x 128 output tile: two consumer warpgroups of 64 rows, each issuing one
-//     wgmma.mma_async m64n128 per k step (m64n64 when the tile's live columns fit in 64);
+//     wgmma.mma_async m64n128 per k step (m64n64 when the tile's live columns fit in 64).  In
+//     the TF32 dW kernels (A and B MN-major) the last column tile also owns a remainder of up
+//     to 8 columns past it (folded_cols), and their wide wgmma is m64n136;
 //   * A comes from registers: each warpgroup loads its fragments from a plain (unswizzled,
 //     padded) fp32 / bf16 tile in shared memory, at transposed addresses when A is MN-major.
 //     The 3xTF32 hi / lo split of A happens there, in registers;
@@ -91,9 +93,31 @@ struct Args {
   int colsum_cols;                   // shared-memory accumulator width (0: off)
 };
 
+// Column tiling of the kernels that can fold (TF32, A and B MN-major: the dW GEMMs).  A
+// remainder of 1..kFoldMax columns past the last full 128-column tile rides in that tile, which
+// then owns 128 + r columns.  The folding kernel gives every B tile kFoldMax more rows (zero
+// where no column lives) and issues m64n136 where the plain one issues m64n128.  As a tile of
+// its own the remainder would run the whole k loop of a 128-column tile.
+constexpr int kFoldMax = 8;
+template <typename T, bool A_MN, bool B_MN>
+__host__ __device__ constexpr bool folds() {
+  return sizeof(T) == 4 && A_MN && B_MN;
+}
+// Remainder columns folded into the last column tile (0: none).
+__host__ __device__ constexpr int folded_cols(int gn) {
+  return gn > BN && gn % BN <= kFoldMax ? gn % BN : 0;
+}
+__host__ __device__ constexpr int col_tiles(int gn, bool fold) {
+  return (gn - (fold ? folded_cols(gn) : 0) + BN - 1) / BN;
+}
+
+// Bytes of one swizzled B tile (hi or lo): 128 rows, 136 when the kernel folds.
+__host__ __device__ constexpr int b_tile_bytes(bool fold) {
+  return fold ? kTileBytes + kFoldMax * 128 : kTileBytes;
+}
 // Bytes of one pipeline stage: the B tile (plus its lo tile for 3xTF32), then the A tile.
-__host__ __device__ constexpr int stage_bytes(int passes) {
-  return (passes == 3 ? 2 : 1) * kTileBytes + kATileBytes;
+__host__ __device__ constexpr int stage_bytes(int passes, bool fold = false) {
+  return (passes == 3 ? 2 : 1) * b_tile_bytes(fold) + kATileBytes;
 }
 // What follows the stages: the staging tile of a staged kernel (its column sums live in
 // global memory), else the [8][colsum_cols] column-sum accumulator.
@@ -102,15 +126,16 @@ __host__ __device__ constexpr int tail_bytes(int colsum_cols, bool staged) {
 }
 // Stages that fit beside the tail and the 1 KB alignment slack; at most kMaxStages.  The one
 // place that sizes the shared memory of a launch.
-__host__ __device__ constexpr int num_stages(int passes, int colsum_cols, bool staged) {
-  return (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes) < kMaxStages
-             ? (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes)
+__host__ __device__ constexpr int num_stages(int passes, int colsum_cols, bool staged, bool fold = false) {
+  return (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes, fold) < kMaxStages
+             ? (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes, fold)
              : kMaxStages;
 }
-static_assert(num_stages(3, 1024, false) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
+static_assert(num_stages(3, 1024, false, true) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
+static_assert(num_stages(3, 0, false, true) == kMaxStages, "the 3xTF32 dW GEMMs keep four stages");
 static_assert(num_stages(3, 1024, true) >= 3, "3xTF32 needs three stages beside the staging tile");
-inline size_t smem_bytes(int passes, int colsum_cols, bool staged) {
-  return (size_t)num_stages(passes, colsum_cols, staged) * stage_bytes(passes) +
+inline size_t smem_bytes(int passes, int colsum_cols, bool staged, bool fold) {
+  return (size_t)num_stages(passes, colsum_cols, staged, fold) * stage_bytes(passes, fold) +
          (size_t)tail_bytes(colsum_cols, staged) + 1024;
 }
 
@@ -219,6 +244,20 @@ __device__ __forceinline__ void mma_tf32_n128(float (&d)[2][32], const uint32_t 
                : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
+// m64n136: d as m64n128, then t holds columns 128..135 (t[0..1] row g, t[2..3] row g + 8,
+// columns 128 + 2 (lane % 4) and the one after it).
+__device__ __forceinline__ void mma_tf32_n136(float (&d)[2][32], float (&t)[4], const uint32_t (&a)[4],
+                                              uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n136k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+               "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, "
+               "%34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+               "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, "
+               "%66, %67}, {%68, %69, %70, %71}, %72, 1, 1, 1;"
+               : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1]),
+                 "+f"(t[0]), "+f"(t[1]), "+f"(t[2]), "+f"(t[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
 // bf16 (k = 16): two bf16 per register.  TRANS_B: B is MN-major in shared memory.
 template <int TRANS_B>
 __device__ __forceinline__ void mma_bf16_n64(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
@@ -307,6 +346,30 @@ struct BTileMN {
           *reinterpret_cast<float*>(hi + off) = e[j];
         }
       }
+    }
+  }
+};
+
+// The folded remainder of a register-staged B tile: tile columns 128..135 x 32 k, one element
+// per thread (k = tid / 8, column tid % 8), stored at K-major rows 128..135; columns past
+// `cols` are zero.  The 32 lanes of a warp write 4 k of one 16-byte chunk position into 8 rows
+// of 8 different swizzle phases: 32 different banks.
+struct BTailMN {
+  float v;
+  __device__ __forceinline__ void load(const float* base, int ld, int c0, int cols, int k0, int ks) {
+    const int k = threadIdx.x >> 3, c = threadIdx.x & 7;
+    v = (c < cols && k0 + k < ks) ? __ldg(base + static_cast<size_t>(k0 + k) * ld + c0 + c) : 0.f;
+  }
+  template <bool SPLIT>
+  __device__ __forceinline__ void store(unsigned char* hi, unsigned char* lo) const {
+    const int k = threadIdx.x >> 3, c = threadIdx.x & 7;
+    const int off = swz_chunk(BN + c, k >> 2) + (k & 3) * 4;
+    if (SPLIT) {
+      const float h = tf32_rn(v);
+      *reinterpret_cast<float*>(hi + off) = h;
+      *reinterpret_cast<float*>(lo + off) = v - h;
+    } else {
+      *reinterpret_cast<float*>(hi + off) = v;
     }
   }
 };
@@ -496,8 +559,9 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
 // PRE_B: B comes pre-split (B = hi parts, B_lo = lo parts).  OUT_BF16: C is bf16 (row-major).
 // Staged (K-major A): a third warpgroup runs the epilogue from a staging tile.
 // Shared memory: num_stages x {B hi, [B lo,] A}, then the staging tile (staged) or
-// [8][colsum_cols] floats.
-template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
+// [8][colsum_cols] floats.  FOLD (launched when GN has a remainder to fold): the last column
+// tile owns it, B tiles have 136 rows and wide tiles issue m64n136.
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16, bool FOLD>
 __global__ void __launch_bounds__(A_MN ? kThreads : kThreads + kEpiThreads, 1)
 gemm_kernel(const Args args) {
   constexpr bool STAGED = !A_MN;
@@ -508,14 +572,16 @@ gemm_kernel(const Args args) {
   constexpr int NKS = BK / KSTEP;
   constexpr bool P3 = PASSES == 3;
   constexpr bool REG_B = F32 && B_MN;   // TF32 MN-major B: transposed through registers
-  constexpr int kStage = stage_bytes(PASSES);
-  constexpr int kAOff = (P3 ? 2 : 1) * kTileBytes;
+  constexpr int kBTile = b_tile_bytes(FOLD);   // offset of the B lo tile
+  constexpr int kStage = stage_bytes(PASSES, FOLD);
+  constexpr int kAOff = (P3 ? 2 : 1) * kBTile;
   constexpr int kAPitch = A_MN ? kAPitchMN * static_cast<int>(sizeof(T)) / 4 : kAPitchK;
   static_assert(!P3 || F32, "3xTF32 is float only");
   static_assert(!PRE_B || P3, "pre-split B is 3xTF32");
+  static_assert(!FOLD || folds<T, A_MN, B_MN>(), "only TF32 with A and B MN-major folds");
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int stages = num_stages(PASSES, args.colsum_cols, STAGED);
+  const int stages = num_stages(PASSES, args.colsum_cols, STAGED, FOLD);
   float* cacc = reinterpret_cast<float*>(smem + stages * kStage);   // staged: the staging tile
   if (STAGED) {
     if (threadIdx.x >= kThreads) {
@@ -539,6 +605,9 @@ gemm_kernel(const Args args) {
   const int tiles_mn = args.m_tiles * args.n_tiles;
   const int total = tiles_mn * args.splits;
   const uint32_t smem_base = smem_u32(smem);
+  const int fold = FOLD ? folded_cols(args.GN) : 0;
+  // the tile at column n0 owns the folded remainder: columns n0 + 128 .. GN - 1
+  auto has_tail = [&](int n0) { return FOLD && n0 + BN + fold == args.GN; };
 
   if (!STAGED)
     for (int c = threadIdx.x; c < kWarps * args.colsum_cols; c += kThreads) cacc[c] = 0.f;
@@ -571,7 +640,7 @@ gemm_kernel(const Args args) {
         const int n = (n0 + r < args.GN && k < args.GK) ? min(EPC, args.GK - k) : 0;
         const size_t off = n > 0 ? static_cast<size_t>(n0 + r) * args.ldb + k : 0;
         cp_async16(st + swz_chunk(r, kc), B + off, n * static_cast<int>(sizeof(T)));
-        if (PRE_B) cp_async16(st + kTileBytes + swz_chunk(r, kc), Blo + off, n * static_cast<int>(sizeof(T)));
+        if (PRE_B) cp_async16(st + kBTile + swz_chunk(r, kc), Blo + off, n * static_cast<int>(sizeof(T)));
       }
     } else if (!F32) {   // bf16 [2 atoms of 64 n][64 k rows][8 chunks of n], swizzled
 #pragma unroll
@@ -589,9 +658,15 @@ gemm_kernel(const Args args) {
   // every k block one more (block kb + stages - 2), empty ones included, so that block kb's
   // group is complete once at most stages - 3 younger groups are pending.
   BTileMN tb, tbl;
+  BTailMN tt, ttl;   // the folded remainder (hi / pre-split lo)
   auto load_b = [&](int n0, int kb) {
     tb.load(reinterpret_cast<const float*>(B), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
     if (PRE_B) tbl.load(reinterpret_cast<const float*>(Blo), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
+    if (FOLD) {   // zeros for a tile without the remainder: its m64n136 reads them too
+      const int cols = has_tail(n0) ? fold : 0;
+      tt.load(reinterpret_cast<const float*>(B), args.ldb, n0 + BN, cols, kb * BK, args.GK);
+      if (PRE_B) ttl.load(reinterpret_cast<const float*>(Blo), args.ldb, n0 + BN, cols, kb * BK, args.GK);
+    }
   };
   auto prologue = [&](int tile) {
     const int z = tile / tiles_mn;
@@ -614,12 +689,15 @@ gemm_kernel(const Args args) {
     const int kb0 = z * args.kb_per_split;
     const int nkb = max(min(nkb_total, kb0 + args.kb_per_split) - kb0, 0);
     const bool two_n = n0 + 64 < args.GN;           // the second 64 columns hold live columns
+    const bool tail = has_tail(n0);
 
-    float acc[2][32];
+    float acc[2][32], acc_t[4];   // acc_t: the folded remainder columns
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc_t[j] = 0.f;
 
     // The k loop is software-pipelined one wgmma group deep: group kb is issued while group
     // kb - 1 may still run, from its own A fragment set (kb & 1), and `wait_group 1` then
@@ -637,9 +715,17 @@ gemm_kernel(const Args args) {
         unsigned char* sb = smem + s * kStage;
         if (PRE_B) {
           tb.template store<false>(sb, nullptr);
-          tbl.template store<false>(sb + kTileBytes, nullptr);
+          tbl.template store<false>(sb + kBTile, nullptr);
         } else {
-          tb.template store<P3>(sb, sb + kTileBytes);
+          tb.template store<P3>(sb, sb + kBTile);
+        }
+        if (FOLD) {
+          if (PRE_B) {
+            tt.template store<false>(sb, nullptr);
+            ttl.template store<false>(sb + kBTile, nullptr);
+          } else {
+            tt.template store<P3>(sb, sb + kBTile);
+          }
         }
       }
       if (stages == 4) cp_async_wait<1>(); else cp_async_wait<0>();
@@ -652,7 +738,7 @@ gemm_kernel(const Args args) {
           const float4 x = *reinterpret_cast<const float4*>(sb + off);
           const float4 h = make_float4(tf32_rn(x.x), tf32_rn(x.y), tf32_rn(x.z), tf32_rn(x.w));
           *reinterpret_cast<float4*>(sb + off) = h;
-          *reinterpret_cast<float4*>(sb + kTileBytes + off) =
+          *reinterpret_cast<float4*>(sb + kBTile + off) =
               make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
         }
       }
@@ -722,12 +808,20 @@ gemm_kernel(const Args args) {
           for (int ks = 0; ks < NK; ++ks) {
             if (F32) {
               const uint64_t dbh = desc_sw128(st + ks * 32);   // 32 bytes of k per wgmma
-              const uint64_t dbl = desc_sw128(st + kTileBytes + ks * 32);
+              const uint64_t dbl = desc_sw128(st + kBTile + ks * 32);
               if (W) {
-                mma_tf32_n128(acc, ahi[ks], dbh);
-                if (P3) {
-                  mma_tf32_n128(acc, alo[ks], dbh);
-                  mma_tf32_n128(acc, ahi[ks], dbl);
+                if constexpr (FOLD) {   // B rows 128..135 (the folded columns) into acc_t
+                  mma_tf32_n136(acc, acc_t, ahi[ks], dbh);
+                  if (P3) {
+                    mma_tf32_n136(acc, acc_t, alo[ks], dbh);
+                    mma_tf32_n136(acc, acc_t, ahi[ks], dbl);
+                  }
+                } else {
+                  mma_tf32_n128(acc, ahi[ks], dbh);
+                  if (P3) {
+                    mma_tf32_n128(acc, alo[ks], dbh);
+                    mma_tf32_n128(acc, ahi[ks], dbl);
+                  }
                 }
               } else {
                 mma_tf32_n64(acc, ahi[ks], dbh);
@@ -894,6 +988,30 @@ gemm_kernel(const Args args) {
         }
       }
     }
+    // the folded remainder (fp32 C): plain stores only, the host admits no other epilogue
+    // for this layout.  Bounds, pairing and split-K slice as for the columns above.
+    if (tail) {
+      const int col = n0 + BN + 2 * (lane & 3);
+      const bool both = col + 1 < args.GN;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int row = rbase + 8 * rr;
+        if (row >= args.GM || col >= args.GN) continue;
+        const float x0 = acc_t[2 * rr], x1 = acc_t[2 * rr + 1];
+        if (args.store_transposed) {
+          Cf[static_cast<size_t>(col) * args.ldc + row] = x0;
+          if (both) Cf[static_cast<size_t>(col + 1) * args.ldc + row] = x1;
+        } else {
+          float* p = Cf + static_cast<size_t>(row) * args.ldc + col;
+          if (both && vec2) {
+            *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
+          } else {
+            p[0] = x0;
+            if (both) p[1] = x1;
+          }
+        }
+      }
+    }
   }
   if (!STAGED && args.colsum_cols) {
     __syncwarp();
@@ -902,11 +1020,10 @@ gemm_kernel(const Args args) {
   }
 }
 
-// Launches the persistent grid; *ctas receives its size (column-sum slots = 8 x ctas).
-template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
-int launch(Args a, cudaStream_t st, int* ctas) {
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16, bool FOLD>
+int launch_grid(Args a, cudaStream_t st, int* ctas) {
   a.m_tiles = (a.GM + BM - 1) / BM;
-  a.n_tiles = (a.GN + BN - 1) / BN;
+  a.n_tiles = col_tiles(a.GN, FOLD);
   if (a.splits < 1) a.splits = 1;
   const int nkb_total = (a.GK + Elem<T>::BK - 1) / Elem<T>::BK;
   a.kb_per_split = (nkb_total + a.splits - 1) / a.splits;
@@ -914,12 +1031,22 @@ int launch(Args a, cudaStream_t st, int* ctas) {
   const int sms = num_sms();
   const int grid = total < sms ? total : sms;
   if (ctas) *ctas = grid;
-  const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN);
-  auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16>;
+  const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN, FOLD);
+  auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, FOLD>;
   TFR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, A_MN ? kThreads : kThreads + kEpiThreads, smem, st>>>(a);
   TFR_LAUNCH_OK();
   return TFR_OK;
+}
+
+// Launches the persistent grid; *ctas receives its size (column-sum slots = 8 x ctas).  A GN
+// with a remainder to fold takes the folding kernel.  Every other GN takes the plain one, whose
+// m64n128 MMAs and 128-row B tiles cost less per k block when no column is folded.
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
+int launch(Args a, cudaStream_t st, int* ctas) {
+  if constexpr (folds<T, A_MN, B_MN>())
+    if (folded_cols(a.GN) > 0) return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, true>(a, st, ctas);
+  return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, false>(a, st, ctas);
 }
 
 }  // namespace wg

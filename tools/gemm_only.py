@@ -21,8 +21,12 @@ M = 204800                  # B * N rows of the config-2 batch
 DIMS = [136, 256, 128, 64]  # Dense widths before the 64 -> 1 output layer (CUDA cores)
 
 
-def tile_units(gm, gn):     # tc::tile_units (tc_gemm.cuh): picks the dW orientation
-  return ((gm + 127) // 128) * ((gn + 63) // 64)
+def folded_cols(gn):        # wg::folded_cols (wgmma_gemm.cuh): columns folded into the last tile
+  return gn % 128 if gn > 128 and gn % 128 <= 8 else 0
+
+
+def tile_units(gm, gn):     # tc::tile_units (tc_gemm.cu): picks the dW orientation
+  return ((gm + 127) // 128) * ((gn - folded_cols(gn) + 63) // 64)
 
 
 def splits_for(m, sms):     # rows_per_split / splits of the dW GEMMs (capi.cu)
@@ -31,9 +35,10 @@ def splits_for(m, sms):     # rows_per_split / splits of the dW GEMMs (capi.cu)
   return (m + rows - 1) // rows
 
 
-def per_tile(gm, gn, gk, splits, sms, us):
-  """(tiles per CTA, k blocks per tile, us per tile, us per k block) on the persistent grid."""
-  tiles = ((gm + 127) // 128) * ((gn + 127) // 128) * splits
+def per_tile(gm, gn, gk, splits, fold, sms, us):
+  """(tiles per CTA, k blocks per tile, us per tile, us per k block) on the persistent grid.
+  fold: the GEMM folds a remainder of up to 8 columns into its last tile (A and B MN-major)."""
+  tiles = ((gm + 127) // 128) * ((gn - (folded_cols(gn) if fold else 0) + 127) // 128) * splits
   per_cta = tiles / min(tiles, sms)
   kb = ((gk + 31) // 32 + splits - 1) // splits
   return per_cta, kb, us / per_cta, us / per_cta / kb
@@ -88,7 +93,7 @@ def main():
           _C.ptr(A), A.shape[1], _C.ptr(B), B.shape[1], _C.ptr(Blo), _C.ptr(C), ldc, gm, gn, gk,
           a_mn, b_mn, 3, split_b, epi, _C.ptr(bias), None, 1, tr, splits, stride,
           _C.ptr(bits if epi == 1 else None), _C.ptr(bits if epi == 3 else None), _C.stream()))
-    calls[name] = (call, 2.0 * gm * gn * gk, nbytes, (gm, gn, gk, splits))
+    calls[name] = (call, 2.0 * gm * gn * gk, nbytes, (gm, gn, gk, splits, a_mn and b_mn))
 
   for call, _, _, _ in calls.values():   # every shape warm before any is timed
     for _ in range(args.warmup):
