@@ -494,10 +494,26 @@ size_t tfr_din_workspace_bytes(const tfr_din_cfg* cfg, int B, int N);
 int tfr_din_fwd(const float* X, const uint8_t* list_mask, int B, int N, const tfr_din_cfg* cfg,
                 const float* params, void* workspace, float* out, int ldo, void* stream);
 /* dout [B * N, h] (row pitch lddo) -> grads (flat, parameter layout).  Must follow a
- * tfr_din_fwd with the same inputs, cfg and workspace.  No gradient with respect to X. */
+ * tfr_din_fwd with the same inputs, cfg and workspace.  The gradient with respect to X is
+ * tfr_din_input_grad's, from what this call leaves in the workspace. */
 int tfr_din_bwd(const float* X, const uint8_t* list_mask, int B, int N, const tfr_din_cfg* cfg,
                 const float* params, const float* dout, int lddo, void* workspace,
                 float* grads, void* stream);
+/* Gradient of the DIN's loss with respect to its input columns [col0, col0 + ncols):
+ *   dX[m, c] (row pitch ldx) (=, or += when accumulate) sum_o dZ_in[m, o] W_in[col0 + c, o]
+ * dZ_in is the gradient at the input projection's pre-activation, i.e. the ReLU gate of
+ * relu(X W_in + b_in) taken before the GaussianNoise.  It is what the preceding tfr_din_bwd
+ * (same X, list_mask, B, N, cfg, params, workspace) left in the workspace.  One 3xTF32 GEMM
+ * (K = h) in column chunks of at most 3 H h; with accumulate = 1 each chunk goes through the
+ * workspace's scratch and is then added, so the result is exactly fp32(dX + G) with G the
+ * accumulate = 0 result.  Never writes dZ_in: several windows can be taken, in any order, and
+ * tfr_din_bwd's gradients are the same with or without this call.  Two identical calls give
+ * identical bits.  TFR_INVALID_ARGUMENT before any CUDA call for the limits above, NULL
+ * params / workspace / dX, a window outside [0, D), ldx < ncols or accumulate not 0 / 1;
+ * B * N == 0 is a no-op. */
+int tfr_din_input_grad(const tfr_din_cfg* cfg, int B, int N, const float* params,
+                       void* workspace, int col0, int ncols, float* dX, int ldx,
+                       int accumulate, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K12  pooled embedding bags (tf.feature_column.embedding_column over a categorical column;

@@ -153,6 +153,7 @@ _SIGNATURES = {
     'tfr_din_workspace_bytes': (C.c_size_t, [C.POINTER(DinCfg), _I, _I]),
     'tfr_din_fwd': (_I, [_P, _P, _I, _I, C.POINTER(DinCfg), _P, _P, _P, _I, _P]),
     'tfr_din_bwd': (_I, [_P, _P, _I, _I, C.POINTER(DinCfg), _P, _P, _I, _P, _P, _P]),
+    'tfr_din_input_grad': (_I, [C.POINTER(DinCfg), _I, _I, _P, _P, _I, _I, _P, _I, _I, _P]),
     'tfr_gam_param_count': (C.c_size_t, [C.POINTER(GamCfg)]),
     'tfr_gam_bn_state_count': (C.c_size_t, [C.POINTER(GamCfg)]),
     'tfr_gam_workspace_bytes': (C.c_size_t, [C.POINTER(GamCfg), _I]),

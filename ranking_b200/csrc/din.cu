@@ -18,6 +18,8 @@
 // the queries (dQ, and D_i = rowsum(dO * O)), one owns the keys (dK, dV), so nothing is
 // accumulated with atomics and two identical calls give identical bits.  Parameter
 // gradients go through the 3xTF32 engine's split-K partials and fixed-order reductions.
+// The input gradient (tfr_din_input_grad) is one more 3xTF32 GEMM, dX = dZ_in W_in^T, over the
+// dZ_in the backward leaves in the workspace.
 #include <cstring>
 
 #include "common.cuh"
@@ -695,6 +697,41 @@ int din_bwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
   return weight_grad(p, ws, X, p.D, p.D, dres, h, h, cs, grads, st);
 }
 
+// dst[r, c] (row pitch ldd) += src[r, c] (row pitch nc), r < M, c < nc.
+__global__ void __launch_bounds__(256)
+add_cols_kernel(const float* __restrict__ src, size_t M, int nc, float* __restrict__ dst,
+                int ldd) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * nc) return;
+  const size_t r = i / nc;
+  const int c = (int)(i - r * nc);
+  dst[r * ldd + c] += src[i];
+}
+
+// dX[:, 0 : ncols) (pitch ldx) = or += dres W_in[col0 : col0 + ncols, :]^T, where dres is the
+// dZ_in that din_bwd left in the workspace.  The GEMM runs in column chunks of at most 3 HH
+// in both modes, so the two launch the same GEMMs and += adds exactly the = result.  When
+// accumulating, a chunk lands in the dqkv scratch (dead after din_bwd) and is then added.
+int din_input_grad(const DinPlan& p, const float* params, float* ws, int col0, int ncols,
+                   float* dX, int ldx, bool accumulate, cudaStream_t st) {
+  const int h = p.h, chunk = 3 * p.HH;
+  const float* dres = ws + p.dres_off;
+  float* scratch = ws + p.dqkv_off;
+  for (int c0 = 0; c0 < ncols; c0 += chunk) {
+    const int nc = ncols - c0 < chunk ? ncols - c0 : chunk;
+    float* out = accumulate ? scratch : dX + c0;
+    int rc = gemm(dres, h, 0, params + (size_t)(col0 + c0) * h, h, 0, out, accumulate ? nc : ldx,
+                  p.M, nc, h, nullptr, TFR_ACT_NONE, st);
+    if (rc) return rc;
+    if (accumulate) {
+      add_cols_kernel<<<blocks_for((size_t)p.M * nc, 256), 256, 0, st>>>(scratch, (size_t)p.M,
+                                                                          nc, dX + c0, ldx);
+      TFR_LAUNCH_OK();
+    }
+  }
+  return TFR_OK;
+}
+
 float* ws_align(void* w) {
   uintptr_t a = reinterpret_cast<uintptr_t>(w);
   return reinterpret_cast<float*>((a + 255) & ~(uintptr_t)255);
@@ -743,4 +780,24 @@ extern "C" int tfr_din_bwd(const float* X, const uint8_t* list_mask, int B, int 
   }
   return din_bwd(X, list_mask, p, params, dout, lddo, ws_align(workspace), grads,
                  (cudaStream_t)stream);
+}
+
+extern "C" int tfr_din_input_grad(const tfr_din_cfg* cfg, int B, int N, const float* params,
+                                  void* workspace, int col0, int ncols, float* dX, int ldx,
+                                  int accumulate, void* stream) {
+  // every argument check comes before make_din_plan, whose SM-count query is a CUDA call
+  TFR_REQUIRE(cfg != nullptr, "cfg must not be NULL");
+  TFR_REQUIRE(params && workspace && dX, "NULL argument");
+  TFR_REQUIRE(col0 >= 0 && ncols >= 1 && (long long)col0 + ncols <= cfg->input_dim,
+              "columns [%d, %lld) outside the DIN input [0, %d)", col0,
+              (long long)col0 + ncols, cfg->input_dim);
+  TFR_REQUIRE(ldx >= ncols, "ldx %d must be >= ncols %d", ldx, ncols);
+  TFR_REQUIRE(accumulate == 0 || accumulate == 1, "accumulate must be 0 or 1, got %d",
+              accumulate);
+  DinPlan p;
+  int rc = make_din_plan(cfg, B, N, &p);
+  if (rc) return rc;
+  if (p.M == 0) return TFR_OK;
+  return din_input_grad(p, params, ws_align(workspace), col0, ncols, dX, ldx, accumulate != 0,
+                        (cudaStream_t)stream);
 }

@@ -423,12 +423,14 @@ class HostBatchPipeline(object):
 
 
 class _EmbeddingScorer(object):
-  """Embedding tables + tower as one scorer with ONE flat parameter buffer: the tables first
-  (in the given order), then the tower (the modules' `flat` become views of it), so the step
-  keeps one gradient all-reduce and one optimizer launch."""
+  """Embedding tables (+ a DocumentInteractionAttention) + tower as one scorer with ONE flat
+  parameter buffer: the tables first (in the given order), then the DIN if there is one, then
+  the tower (the modules' `flat` become views of it), so the step keeps one gradient
+  all-reduce and one optimizer launch."""
 
-  def __init__(self, tables, tower):
-    self.flat = torch.nn.Parameter(torch.cat([t.flat.data for t in tables] + [tower.flat.data]))
+  def __init__(self, tables, tower, din=None):
+    mods = list(tables) + ([din] if din is not None else [])
+    self.flat = torch.nn.Parameter(torch.cat([t.flat.data for t in mods] + [tower.flat.data]))
     self.table_offsets = []
     off = 0
     for t in tables:
@@ -437,9 +439,15 @@ class _EmbeddingScorer(object):
       self.table_offsets.append(off)
       off += n
     self.n_tables = off
+    self.n_din = 0
+    if din is not None:
+      self.n_din = din.flat.numel()
+      din.flat = torch.nn.Parameter(self.flat.data[off:off + self.n_din])
+      off += self.n_din
+    self.tower_offset = off
     tower.flat = torch.nn.Parameter(self.flat.data[off:])
     self.bn_state = tower.bn_state
-    self.dims = [list(t.dims) for t in tables] + [list(tower.dims)]
+    self.dims = [list(t.dims) for t in mods] + [list(tower.dims)]
     self.use_batch_norm = tower.use_batch_norm
     self.input_batch_norm = tower.input_batch_norm
     self.input_dtype = torch.float32
@@ -448,7 +456,8 @@ class _EmbeddingScorer(object):
 
 class EmbeddingRankingTrainer(RankingTrainer):
   """Fused step for scorers over token (text) features, the model of the reference's ANTIQUE
-  examples (examples/keras/antique_kpl_din.py:256-288, without the DIN): every token feature
+  examples (examples/keras/antique_kpl_din.py:256-288, without the DIN; with it:
+  DINEmbeddingRankingTrainer): every token feature
   is a bag of ids pooled through an embedding table (keras.layers.TokenEmbedding), and the
   pooled vectors become input columns of a create_tower tower:
 
@@ -504,10 +513,13 @@ class EmbeddingRankingTrainer(RankingTrainer):
     self.dense_dim = tower.input_dim - width
     self.emb_width = width
     self.mlp = tower
-    super().__init__(_EmbeddingScorer(tables, tower), loss, **kw)
+    super().__init__(self._scorer(tables, tower), loss, **kw)
     self.bad_ids = torch.zeros(1, dtype=torch.int32, device=self.device)
     self._emb_ws = None
     self._padded = {}
+
+  def _scorer(self, tables, tower):
+    return _EmbeddingScorer(tables, tower)
 
   def check_ids(self):
     """Raises ValueError if a step has seen ids outside [-1, V) (host sync)."""
@@ -582,26 +594,30 @@ class EmbeddingRankingTrainer(RankingTrainer):
       return ids, b, t, n
     return ids, b * n, t, 1
 
-  def _forward(self, x, y_true, m8, cfg, training):
+  def _pool(self, x, buf, ld):
+    """buf [B * N, ld] = [x | every token feature's pooled bag, in feature order]."""
     b, n, d = x.shape
     if d != self.dense_dim:
       raise ValueError('x has %d dense features, the tower expects %d' % (d, self.dense_dim))
-    width = self.mlp.input_dim
     st = _C.stream()
     if d:
-      self.xe.view(b, n, width)[..., :d].copy_(x)
+      buf.view(b, n, ld)[..., :d].copy_(x)
     col = d
     for k, (_, _, ti) in enumerate(self.features):
       emb = self.embeddings[ti]
       ids, r, t, rpb = self._bags(k, b, n)
       _C.check(_C.lib.tfr_embedding_fwd(_C.ptr(ids), r, t, _C.ptr(emb.flat.data),
                                         emb.vocab_size, emb.embedding_dim, emb._combiner, rpb,
-                                        ctypes.c_void_p(self.xe.data_ptr() + 4 * col), width,
+                                        ctypes.c_void_p(buf.data_ptr() + 4 * col), ld,
                                         _C.ptr(self.bad_ids), st))
       col += emb.embedding_dim
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    self._pool(x, self.xe, self.mlp.input_dim)
     _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(self.mlp.flat.data),
                                 _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores),
-                                self.mlp._precision, st))
+                                self.mlp._precision, _C.stream()))
 
   def _backward(self, x, m8, cfg, grads):
     b, n, d = x.shape
@@ -609,11 +625,22 @@ class EmbeddingRankingTrainer(RankingTrainer):
     st = _C.stream()
     _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(mlp.flat.data),
                                 _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
-                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.n_tables),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.tower_offset),
                                 mlp._precision, st))
     _C.check(_C.lib.tfr_mlp_input_grad(cfg, b * n, _C.ptr(mlp.flat.data), _C.ptr(self.ws), d,
                                        self.emb_width, _C.ptr(self.d_emb), self.emb_width,
                                        mlp._precision, st))
+    cols, col = [], 0
+    for _, _, ti in self.features:
+      cols.append(col)
+      col += self.embeddings[ti].embedding_dim
+    self._tables_bwd(b, n, grads, self.d_emb, self.emb_width, cols)
+
+  def _tables_bwd(self, b, n, grads, d_pooled, ld, cols):
+    """Table gradients: feature k's pooled gradient is columns cols[k] .. of d_pooled (row
+    pitch ld)."""
+    sc = self.tower
+    st = _C.stream()
     need = 0
     for k, (_, _, ti) in enumerate(self.features):
       emb = self.embeddings[ti]
@@ -623,21 +650,140 @@ class EmbeddingRankingTrainer(RankingTrainer):
     if self._emb_ws is None or self._emb_ws.numel() < need:
       self._emb_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
     written = set()
-    col = 0
     for k, (_, _, ti) in enumerate(self.features):
       emb = self.embeddings[ti]
       ids, r, t, rpb = self._bags(k, b, n)
       _C.check(_C.lib.tfr_embedding_bwd(
-          _C.ptr(ids), r, t, ctypes.c_void_p(self.d_emb.data_ptr() + 4 * col), self.emb_width,
+          _C.ptr(ids), r, t, ctypes.c_void_p(d_pooled.data_ptr() + 4 * cols[k]), ld,
           rpb, emb.vocab_size, emb.embedding_dim, emb._combiner, int(ti in written),
           _C.ptr(self._emb_ws), ctypes.c_void_p(grads.data_ptr() + 4 * sc.table_offsets[ti]),
           None, st))
       written.add(ti)
-      col += emb.embedding_dim
     for ti, emb in enumerate(self.embeddings):
       if ti not in written:     # a table no feature reads: zero gradient
         off = sc.table_offsets[ti]
         grads[off:off + emb.flat.numel()].zero_()
+
+
+class DINEmbeddingRankingTrainer(EmbeddingRankingTrainer):
+  """EmbeddingRankingTrainer with a DocumentInteractionAttention between the pooled token
+  features and the tower: the reference's ANTIQUE example as it runs by default
+  (examples/keras/antique_kpl_din.py, use_document_interaction=True).
+
+      xd = [x | context features by sorted name | example features by sorted name]
+           the DIN's input, ConcatFeatures' order (D_din = D + E * F columns)
+      xe = the same blocks with the DIN's h columns inserted where `din_feature` sorts among
+           the example features (the reference's sorted-name rule), e.g. for ANTIQUE
+           [query_tokens | document_interaction_embedding | document_tokens]
+      xd, xe                                         tfr_embedding_fwd, strided copies
+      E = din((xd, list_mask)) into xe's DIN block   tfr_din_fwd
+      scores = tower(xe)                             tfr_mlp_fwd
+      loss, d loss / d scores                        fused loss kernel
+      tower gradients, d loss / d xe[:, D:]          tfr_mlp_bwd, tfr_mlp_input_grad
+      DIN gradients                                  tfr_din_bwd on the DIN block of d xe
+      d loss / d xd[:, D:] added to d xe's token     tfr_din_input_grad (accumulate), one
+      columns                                        window each side of the DIN block
+      table gradients                                tfr_embedding_bwd
+      optimizer                                      one launch over the shared flat buffer
+
+  No gradient is formed for the dense x.  The flat buffer holds the tables, then the DIN, then
+  the tower.  `tower` needs input_dim = D_din + head_size with D_din a multiple of 4, and the
+  limits of EmbeddingRankingTrainer.  The DIN is built for D_din on first use if it has not
+  been.  The list mask, the DIN's training flag and its seed follow DINRankingTrainer.  With
+  BN in the tower, the dense rows and the example id rows are circularly padded before the
+  DIN, as DINRankingTrainer does (the reference pads after it); with DIN dropout the padded
+  rows then draw their own dropout masks instead of repeating their source item's."""
+
+  def __init__(self, embeddings, token_features, din, tower, loss,
+               din_feature='document_interaction_embedding', **kw):
+    h = din.head_size
+    names = {f for kind in dict(token_features).values() for f in (kind or {})}
+    if din_feature in names:
+      raise ValueError('din_feature %r is also the name of a token feature' % din_feature)
+    d_din = tower.input_dim - h
+    if d_din <= 0 or d_din % 4:
+      raise ValueError('the DIN input (tower input_dim %d - head_size %d = %d columns) must be '
+                       'a positive multiple of 4' % (tower.input_dim, h, d_din))
+    if not din.built:
+      din.build(d_din)
+    if din.input_dim != d_din:
+      raise ValueError('the tower needs input_dim = %d (DIN input) + %d (head_size), got %d' %
+                       (din.input_dim, h, tower.input_dim))
+    self.din = din
+    self.din_feature = din_feature
+    super().__init__(embeddings, token_features, tower, loss, **kw)
+    self.dense_dim = d_din - self.emb_width
+    if self.dense_dim < 0:
+      raise ValueError('the token features take %d columns, the DIN input has %d' %
+                       (self.emb_width, d_din))
+    # DIN input column where the DIN block goes in the tower input
+    self.split = self.dense_dim
+    for kind, name, ti in self.features:
+      if kind == 'context' or name < din_feature:
+        self.split += self.embeddings[ti].embedding_dim
+
+  def _scorer(self, tables, tower):
+    return _EmbeddingScorer(tables, tower, din=self.din)
+
+  def _new_workspace(self, b, n):
+    m, dev = b * n, self.device
+    self.xd = torch.empty(m, self.din.input_dim, dtype=torch.float32, device=dev)
+    self.xe = torch.empty(m, self.mlp.input_dim, dtype=torch.float32, device=dev)
+    self.d_xe = torch.empty(m, self.mlp.input_dim - self.dense_dim, dtype=torch.float32,
+                            device=dev)
+    self.din_ws = self.din._new_workspace(b, n)
+    return self.mlp._new_workspace(m)
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    din, s, h = self.din, self.split, self.din.head_size
+    width = self.mlp.input_dim
+    self._pool(x, self.xd, din.input_dim)
+    self.xe[:, :s].copy_(self.xd[:, :s])
+    self.xe[:, s + h:].copy_(self.xd[:, s:])
+    lm = m8
+    if lm is None and y_true is not None:
+      lm = (y_true >= 0).reshape(-1).to(torch.uint8).contiguous()
+    self._lm = lm
+    self._din_cfg = din._run_cfg(training=training)
+    st = _C.stream()
+    _C.check(_C.lib.tfr_din_fwd(_C.ptr(self.xd), _C.ptr(lm), b, n, ctypes.byref(self._din_cfg),
+                                _C.ptr(din.flat.data), _C.ptr(self.din_ws),
+                                ctypes.c_void_p(self.xe.data_ptr() + 4 * s), width, st))
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(self.mlp.flat.data),
+                                _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores),
+                                self.mlp._precision, st))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, d = x.shape
+    din, mlp, sc = self.din, self.mlp, self.tower
+    s, h, d_din = self.split, din.head_size, din.input_dim
+    ld = mlp.input_dim - d          # d_xe: the tower input's columns [D, width)
+    st = _C.stream()
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(mlp.flat.data),
+                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.tower_offset),
+                                mlp._precision, st))
+    _C.check(_C.lib.tfr_mlp_input_grad(cfg, b * n, _C.ptr(mlp.flat.data), _C.ptr(self.ws), d,
+                                       ld, _C.ptr(self.d_xe), ld, mlp._precision, st))
+    cfg_din = ctypes.byref(self._din_cfg)
+    _C.check(_C.lib.tfr_din_bwd(_C.ptr(self.xd), _C.ptr(self._lm), b, n, cfg_din,
+                                _C.ptr(din.flat.data),
+                                ctypes.c_void_p(self.d_xe.data_ptr() + 4 * (s - d)), ld,
+                                _C.ptr(self.din_ws),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.n_tables), st))
+    # the DIN input's token columns before and after the DIN block, added onto d_xe's
+    for c0, c1, dst in ((d, s, 0), (s, d_din, s + h - d)):
+      if c1 > c0:
+        _C.check(_C.lib.tfr_din_input_grad(cfg_din, b, n, _C.ptr(din.flat.data),
+                                           _C.ptr(self.din_ws), c0, c1 - c0,
+                                           ctypes.c_void_p(self.d_xe.data_ptr() + 4 * dst), ld,
+                                           1, st))
+    cols, col = [], d
+    for _, _, ti in self.features:
+      cols.append(col - d if col < s else col - d + h)
+      col += self.embeddings[ti].embedding_dim
+    self._tables_bwd(b, n, grads, self.d_xe, ld, cols)
 
 
 class ClickEMRankingTrainer(RankingTrainer):
