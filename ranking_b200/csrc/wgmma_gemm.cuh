@@ -22,7 +22,8 @@
 //       - K-major A (forward and dZ GEMMs: GM long, a few k blocks per tile): a third
 //         warpgroup runs it.  The MMA warpgroups write a tile's raw accumulators to a staging
 //         tile in shared memory and start the next tile's k loop; the epilogue warpgroup reads
-//         the staging tile row-major (a lane takes 4 adjacent columns, a warp whole rows) and
+//         the staging tile row-major (a lane takes 4 adjacent columns, a warp whole rows, or
+//         two rows at a time on tiles of at most 64 columns) and
 //         overlaps that k loop.  The staging tile takes the room of one ring stage.
 //       - MN-major A (the dW GEMMs: one epilogue per 50-100 k blocks): the two MMA warpgroups
 //         run it on their accumulator registers and keep the fourth stage.
@@ -68,9 +69,10 @@ constexpr int kStagingBytes = BM * kStagingPitch * 4;
 //             last, which nobody would wait for.
 //   kBarEpi:  bar.sync over the 128 epilogue threads, between the row pass and the column sums.
 constexpr int kBarMma = 1, kBarFull = 2, kBarFree = 3, kBarEpi = 4;
-// Registers after setmaxnreg: 2 x 128 x 216 + 128 x 72 = 64,512 of the SM's 65,536.  With
-// 72 the epilogue's row loop fits unrolled once, without spills.
-constexpr int kMmaRegs = 216, kEpiRegs = 72;
+// Registers after setmaxnreg: 2 x 128 x 208 + 128 x 88 = 64,512 of the SM's 65,536.  The
+// epilogue's row loop needs 88 without spills: it holds the tile's mask words and running
+// column sums beside the unrolled rows.
+constexpr int kMmaRegs = 208, kEpiRegs = 88;
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 };
 
@@ -383,12 +385,18 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 // The epilogue warpgroup of a staged kernel: walks the CTA's tiles as the MMA warpgroups do and
 // finishes each from the staging tile `stg`.  Warp `ew` takes rows 32 ew .. 32 ew + 31, a lane
 // 4 adjacent columns of each, so a row is stored as one 512-byte line and the eight lanes of a
-// 32-column chunk assemble its sign word with one redux.  Column tests are made once per tile,
-// row tests once per row.  Column sums: the row pass writes the stored fp32 values back to the
-// staging tile; thread t then owns tile column t, adds the 16 rows of each of the 8 row groups
-// in the order the accumulator layout gave them (rows g and g + 8, then g pairs 1, 2, 4 apart)
-// and adds that to its running sum in the group's slot in global memory.  Slot and column
-// always meet the same thread, so plain loads and stores keep the running sums.
+// 32-column chunk assemble its sign word with three shuffles.  On a tile of at most 64 live columns
+// the warp takes two rows at a time instead, lanes 0-15 row i and lanes 16-31 row i + 1 (a
+// 256-byte line each), so no lane idles.  Column tests are made once per tile, row tests once
+// per row.  Nothing in the row loop waits on global memory: the tile's mask words are loaded
+// into registers while the previous tile's column sums run, and reach their rows by shuffle.
+// The fast loop stores sign words 8 rows at a time, one word per lane: 32-byte sectors whole.
+// Column sums: the row pass writes the stored fp32 values back to the staging tile; thread t
+// then owns tile column t, adds the 16 rows of each of the 8 row groups in the order the
+// accumulator layout gave them (rows g and g + 8, then g pairs 1, 2, 4 apart) and adds that to
+// its running sum in the group's slot in global memory.  Slot and column always meet the same
+// thread, so plain loads and stores keep the running sums; the loads are issued before the row
+// pass, so the tile's tail only stores.
 template <bool OUT_BF16>
 __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg) {
   const int lane = threadIdx.x & 31;
@@ -401,12 +409,45 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
       for (int c = et; c < args.GN; c += kEpiThreads) dst[c] = 0.f;
     }
   }
+  // Mask words of a tile's 32 rows of this warp: lane 8 p + q holds, in mw[k], the word of
+  // plane p (tile columns 32 p .. 32 p + 31) for row 8 k + q; a warp's load is 4 whole sectors.
+  // Zero past GM and GN.
+  uint32_t mw[4] = {0u, 0u, 0u, 0u};
+  auto load_masks = [&](int tile) {
+    const int r = tile % tiles_mn;
+    const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
+    const int c = n0 + 32 * (lane >> 3), row = m0 + ew * 32 + (lane & 7);
+    const uint32_t* p = args.bits_in + static_cast<size_t>(c >> 5) * args.GM + row;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mw[k] = c < args.GN && row + 8 * k < args.GM ? __ldg(p + 8 * k) : 0u;
+  };
+  // the word of row `rw` (0..31 within the warp) in plane `pl` of the tile.  The shuffle reads
+  // the source lane's choice of register, so rw >> 3 must agree across the warp: it does, as
+  // the two rows of a paired step are i and i + 1 with i even.
+  auto mask_word = [&](int rw, int pl) {
+    const int k = rw >> 3;
+    const uint32_t m = k == 0 ? mw[0] : k == 1 ? mw[1] : k == 2 ? mw[2] : mw[3];
+    return __shfl_sync(0xffffffffu, m, 8 * pl + (rw & 7));
+  };
+  const bool masks = args.epi == EPI_MASK_BITS;
+  if (masks && static_cast<int>(blockIdx.x) < total) load_masks(blockIdx.x);
   for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int z = tile / tiles_mn;
     const int r = tile - z * tiles_mn;
     const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
-    const int col = n0 + 4 * lane;
+    // lane mapping: a lane's columns 4 cl .. 4 cl + 3 of row i + half, rows advancing by step
+    const bool pair = args.GN - n0 <= 64;
+    const int cl = pair ? lane & 15 : lane, half = pair ? lane >> 4 : 0;
+    const int col = n0 + 4 * cl;
     const int live = min(max(args.GN - col, 0), 4);   // live columns of this lane
+    // the running column sums this tile adds to, loaded while the row pass runs
+    float run[kWarps];
+    const bool sums = args.colsum_cols && n0 + et < args.GN;
+    if (sums) {
+#pragma unroll
+      for (int w = 0; w < kWarps; ++w)
+        run[w] = args.colsum[static_cast<size_t>(blockIdx.x * kWarps + w) * args.colsum_stride + n0 + et];
+    }
     float b4[4] = {0.f, 0.f, 0.f, 0.f};
     if (args.epi == EPI_BIAS_ACT) {
 #pragma unroll
@@ -420,28 +461,44 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
     const uintptr_t cbase = OUT_BF16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
     const bool vec_ok = (args.ldc % 4) == 0 && (cbase & (OUT_BF16 ? 7u : 15u)) == 0;
     const bool vec4 = live == 4 && vec_ok;
-    const uint32_t* bin = args.epi == EPI_MASK_BITS && live > 0
-                              ? args.bits_in + static_cast<size_t>(col >> 5) * args.GM : nullptr;
-    uint32_t* bout = args.bits_out && (lane & 7) == 0 && live > 0
-                         ? args.bits_out + static_cast<size_t>(col >> 5) * args.GM : nullptr;
+    // this lane's plane of sign words (tile columns 32 mpl .. 32 mpl + 31); every lane of a
+    // live plane stores rows in the fast loop, also those whose own columns lie past GN
+    const int mpl = cl >> 3, pcol = n0 + 32 * mpl;
+    uint32_t* bplane = args.bits_out && pcol < args.GN
+                           ? args.bits_out + static_cast<size_t>(pcol >> 5) * args.GM : nullptr;
+    // a row's sign word from the nibbles of the 8 lanes of its plane.  Shuffles, not a redux:
+    // the redux's member mask differs between the warp's 4 groups, which sends it down the
+    // divergent path.
+    auto sign_word = [&](uint32_t nib) {
+      uint32_t w = nib << (4 * (lane & 7));
+      w |= __shfl_xor_sync(0xffffffffu, w, 1);
+      w |= __shfl_xor_sync(0xffffffffu, w, 2);
+      w |= __shfl_xor_sync(0xffffffffu, w, 4);
+      return w;
+    };
     bar_sync(kBarFull, kThreads + kEpiThreads);
     // Full row blocks whose lanes hold 4 live columns or none, stored as vectors: the row loop
-    // has no bounds tests, its epilogue kind is a compile-time constant and its pointers advance
-    // by a constant per row.  Everything else takes the general loop below it.
-    auto fast_rows = [&](auto kind) {
+    // has no bounds tests, its epilogue kind and lane mapping are compile-time constants and its
+    // pointers advance by a constant per row.  Everything else takes the general loop below it.
+    auto fast_rows = [&](auto kind, auto paired) {
       constexpr int EPI = decltype(kind)::value;
+      constexpr bool PAIR = decltype(paired)::value;
+      constexpr int STEP = PAIR ? 2 : 1;
       using V = std::conditional_t<OUT_BF16, uint2, float4>;
       const bool on = live == 4, relu = args.act == TFR_ACT_RELU;
       const int row0 = m0 + ew * 32;
-      const float4* sp = reinterpret_cast<const float4*>(stg + ew * 32 * kStagingPitch + 4 * lane);
-      const size_t coff = static_cast<size_t>(row0) * args.ldc + col;
+      const float4* sp =
+          reinterpret_cast<const float4*>(stg + (ew * 32 + half) * kStagingPitch + 4 * cl);
+      const size_t coff = static_cast<size_t>(row0 + half) * args.ldc + col;
       V* cp = OUT_BF16 ? reinterpret_cast<V*>(Cb + coff) : reinterpret_cast<V*>(Cf + coff);
       const int cstep = args.ldc / 4;
-      const uint32_t* bi = bin ? bin + row0 : nullptr;
-      uint32_t* bo = bout ? bout + row0 : nullptr;
-      const int sh = (4 * lane) & 31;
+      // sign words: lane q of a group keeps the word of row 8 b + q and stores it once the
+      // group's 8 rows are done (with two rows a step, half h keeps the rows of parity h)
+      uint32_t* bo = bplane && (!PAIR || (lane & 1) == half) ? bplane + row0 + (lane & 7) : nullptr;
+      uint32_t keep = 0u;
+      const int sh = (4 * cl) & 31;
 #pragma unroll 4
-      for (int i = 0; i < 32; ++i) {
+      for (int i = 0; i < 32; i += STEP) {
         float4 v = sp[i * (kStagingPitch / 4)];
         if (EPI == EPI_BIAS_ACT) {
           v.x += b4[0]; v.y += b4[1]; v.z += b4[2]; v.w += b4[3];
@@ -449,7 +506,7 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
             v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
           }
         } else if (EPI == EPI_MASK_BITS) {
-          const uint32_t w = on ? __ldg(bi + i) >> sh : 0u;
+          const uint32_t w = mask_word(i + half, mpl) >> sh;
           if (!(w & 1u)) v.x = 0.f;
           if (!(w & 2u)) v.y = 0.f;
           if (!(w & 4u)) v.z = 0.f;
@@ -462,8 +519,9 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
             return (OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(y)) : y) > 0.f ? 1u : 0u;
           };
           const uint32_t nib = pos(v.x) | pos(v.y) << 1 | pos(v.z) << 2 | pos(v.w) << 3;
-          const uint32_t w = __reduce_or_sync(0xffu << (lane & 24), nib << (4 * (lane & 7)));
-          if (bo) bo[i] = w;
+          const uint32_t w = sign_word(nib);
+          if (((i + half) & 7) == (lane & 7)) keep = w;
+          if (((i + STEP) & 7) == 0 && bo) bo[i & ~7] = keep;
         }
         if (args.colsum_cols) const_cast<float4*>(sp)[i * (kStagingPitch / 4)] = v;
         if (on) {
@@ -472,21 +530,26 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         }
       }
     };
+    auto fast_kind = [&](auto kind) {
+      if (pair) fast_rows(kind, std::true_type{});
+      else fast_rows(kind, std::false_type{});
+    };
     const bool fast = m0 + BM <= args.GM && (args.GN % 4) == 0 && vec_ok && !args.store_transposed;
     bool general = false;
-    if (fast && args.epi == EPI_STORE) fast_rows(std::integral_constant<int, EPI_STORE>{});
-    else if (fast && args.epi == EPI_BIAS_ACT) fast_rows(std::integral_constant<int, EPI_BIAS_ACT>{});
-    else if (fast && args.epi == EPI_MASK_BITS) fast_rows(std::integral_constant<int, EPI_MASK_BITS>{});
+    if (fast && args.epi == EPI_STORE) fast_kind(std::integral_constant<int, EPI_STORE>{});
+    else if (fast && args.epi == EPI_BIAS_ACT) fast_kind(std::integral_constant<int, EPI_BIAS_ACT>{});
+    else if (fast && masks) fast_kind(std::integral_constant<int, EPI_MASK_BITS>{});
     else general = true;
+    const int step = pair ? 2 : 1;
 #pragma unroll 1
-    for (int i = general ? 0 : 32; i < 32; ++i) {
-      const int rl = ew * 32 + i, row = m0 + rl;
+    for (int i = general ? 0 : 32; i < 32; i += step) {
+      const int rl = ew * 32 + i + half, row = m0 + rl;
       const bool rlive = row < args.GM;
-      float* sp = stg + rl * kStagingPitch + 4 * lane;
+      float* sp = stg + rl * kStagingPitch + 4 * cl;
       const float4 v = *reinterpret_cast<const float4*>(sp);
       float x[4] = {v.x, v.y, v.z, v.w};
       uint32_t wbits = 0u, nib = 0u;
-      if (bin && rlive) wbits = __ldg(bin + row);
+      if (masks) wbits = mask_word(i + half, mpl);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         float y = x[j];
@@ -498,7 +561,7 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
               !(__ldg(args.aux + static_cast<size_t>(row) * args.ldc + col + j) > 0.f))
             y = 0.f;
         } else if (args.epi == EPI_MASK_BITS) {
-          if (!((wbits >> ((4 * lane + j) & 31)) & 1u)) y = 0.f;
+          if (!((wbits >> ((4 * cl + j) & 31)) & 1u)) y = 0.f;
         }
         if (!rlive || j >= live) y = 0.f;
         x[j] = y;   // column sums take the fp32 value, sign bits the stored one
@@ -506,8 +569,8 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         nib |= (stored > 0.f ? 1u : 0u) << j;
       }
       if (args.bits_out) {
-        const uint32_t w = __reduce_or_sync(0xffu << (lane & 24), nib << (4 * (lane & 7)));
-        if (bout && rlive) bout[row] = w;
+        const uint32_t w = sign_word(nib);
+        if (bplane && (lane & 7) == 0 && rlive) bplane[row] = w;
       }
       if (args.colsum_cols) *reinterpret_cast<float4*>(sp) = make_float4(x[0], x[1], x[2], x[3]);
       if (!rlive || live == 0) continue;
@@ -535,9 +598,10 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         }
       }
     }
+    if (masks && tile + gridDim.x < total) load_masks(tile + gridDim.x);   // in flight over the sums
     if (args.colsum_cols) {
       bar_sync(kBarEpi, kEpiThreads);   // the write-backs of all four warps
-      if (n0 + et < args.GN) {
+      if (sums) {
 #pragma unroll
         for (int w = 0; w < kWarps; ++w) {
           const float* p = stg + w * 16 * kStagingPitch + et;
@@ -545,9 +609,8 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
 #pragma unroll
           for (int g = 0; g < 8; ++g) s[g] = p[g * kStagingPitch] + p[(g + 8) * kStagingPitch];
           const float sum = ((s[0] + s[1]) + (s[2] + s[3])) + ((s[4] + s[5]) + (s[6] + s[7]));
-          float* dst = args.colsum + static_cast<size_t>(blockIdx.x * kWarps + w) * args.colsum_stride +
-                       n0 + et;
-          *dst += sum;
+          args.colsum[static_cast<size_t>(blockIdx.x * kWarps + w) * args.colsum_stride + n0 + et] =
+              run[w] + sum;
         }
       }
     }
