@@ -516,6 +516,65 @@ int tfr_din_input_grad(const tfr_din_cfg* cfg, int B, int N, const float* params
                        int accumulate, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K13  DASALC scorer (research/dasalc.py:116-201): a latent-cross tower over the transformed
+ * features X [M, D] and the DocumentInteractionAttention embedding E [M, h] (row pitch lde),
+ * M = B * N flattened items, W = hidden_dim.  All BN layers are the non-fused tf.keras
+ * BatchNormalization: population variance, moving = moving * momentum + batch * (1 - momentum)
+ * in training, the moving statistics in inference.
+ *   a0  = BN_in(X) + sigma g                       (GaussianNoise, training only)
+ *   a_l = Dropout(BN_l(relu(a_{l-1} W_l + b_l)))   l = 1, 2 (exactly two hidden layers)
+ *   t   = a_2 W_t + b_t,   c = BN_c(E) W_c + b_c
+ *   s   = Dropout(relu(t * c + t)) w_o + b_o,      ln(1e-10) where mask (uint8 [M]) is 0
+ * Flat parameter layout: W_1 [D, W] (Keras kernel layout), b_1 [W], W_2 [W, W], b_2, W_t [W, W],
+ *   b_t, W_c [h, W], b_c, w_o [W], b_o [1], then gamma, beta of BN_in [D], BN_1 [W], BN_2 [W],
+ *   BN_c [h].  Gradients use the same layout.
+ * bn_state (device, tfr_dasalc_bn_state_count floats): moving mean then moving variance of
+ *   BN_in, BN_1, BN_2, BN_c in that order.
+ * Random draws (training only), with u(s, e) the tower's counter hash (tfr_mlp_cfg dropout
+ * mask) and site seeds s = seed * 0x100000001B3 + site:
+ *   site 1, 2   dropout after BN_1, BN_2, element e = m * W + j
+ *   site 3      input noise, element e = m * D + j: g = sqrt(-2 ln(1 - u(s, 2e)))
+ *               * cos(2 pi u(s, 2e + 1))  (the DIN's formula)
+ *   site 4      cross dropout, element e = m * W + j
+ *   an element is dropped iff u < dropout; kept values are scaled by 1 / (1 - dropout).
+ * precision: TFR_PREC_TF32X3 (fp32-faithful) or TFR_PREC_TF32 (TFR_UNSUPPORTED otherwise).
+ * Limits (TFR_INVALID_ARGUMENT before any CUDA call): D, W, h positive multiples of 4,
+ * W <= 4096, h <= 128, 0 <= dropout < 1, input_noise_stddev >= 0, bn_epsilon > 0,
+ * 0 <= bn_momentum <= 1, bn_state not NULL, M * max(D, W) < 2^31.  Two identical calls give
+ * identical bits (no float atomics; fixed-order partial sums).
+ * ------------------------------------------------------------------------- */
+typedef struct {
+  int32_t input_dim;            /* D */
+  int32_t hidden_dim;           /* W */
+  int32_t context_dim;          /* h, the DIN's head_size */
+  float dropout;                /* rate of the three Dropout sites */
+  float input_noise_stddev;     /* sigma; 0 = no GaussianNoise */
+  float bn_epsilon;             /* tf.compat.v1 default 1e-3 */
+  float bn_momentum;            /* `batch_norm_moment`, 0.9 in the reference recipe */
+  int32_t training;             /* 1: batch statistics + moving update, noise and dropout */
+  uint64_t seed;                /* vary per step; same value -> same draws */
+  float* bn_state;              /* device, moving statistics (see above) */
+} tfr_dasalc_cfg;
+
+/* 0 when the configuration is out of range (tfr_last_error says why) */
+size_t tfr_dasalc_param_count(const tfr_dasalc_cfg* cfg);
+size_t tfr_dasalc_bn_state_count(const tfr_dasalc_cfg* cfg);
+size_t tfr_dasalc_workspace_bytes(const tfr_dasalc_cfg* cfg, int M);
+/* scores [M]; updates bn_state in training.  The workspace carries what tfr_dasalc_bwd needs. */
+int tfr_dasalc_fwd(const float* X, const float* E, int lde, int M, const tfr_dasalc_cfg* cfg,
+                   const float* params, const uint8_t* mask, void* workspace, float* scores,
+                   int precision, void* stream);
+/* dscores [M] -> grads (flat, parameter layout) and dE [M, h] (row pitch ldde) = dL/dE, the
+ * input of tfr_din_bwd.  No gradient is formed for X.  Must follow a tfr_dasalc_fwd with the
+ * same X, M, cfg, params, mask and workspace. */
+int tfr_dasalc_bwd(const float* X, int M, const tfr_dasalc_cfg* cfg, const float* params,
+                   const float* dscores, const uint8_t* mask, void* workspace, float* grads,
+                   float* dE, int ldde, int precision, void* stream);
+/* DASALC's feature transform (research/dasalc.py:127-129), elementwise over n floats:
+ *   out = clip(sign(x) log1p(|x|), -cutoff, cutoff),  cutoff > 0; out may alias X. */
+int tfr_symmetric_log1p_clip(const float* X, size_t n, float cutoff, float* out, void* stream);
+
+/* ---------------------------------------------------------------------------
  * K12  pooled embedding bags (tf.feature_column.embedding_column over a categorical column;
  * Keras Embedding + a reduction over the token axis).  ids [R, T] int32, table [V, E] fp32.
  * Bag r holds the ids ids[r, 0..T) in [0, V); -1 marks an empty slot.  Any other id (< -1 or

@@ -86,6 +86,13 @@ class DinCfg(C.Structure):
               ('seed', C.c_uint64)]
 
 
+class DasalcCfg(C.Structure):
+  _fields_ = [('input_dim', C.c_int32), ('hidden_dim', C.c_int32), ('context_dim', C.c_int32),
+              ('dropout', C.c_float), ('input_noise_stddev', C.c_float),
+              ('bn_epsilon', C.c_float), ('bn_momentum', C.c_float), ('training', C.c_int32),
+              ('seed', C.c_uint64), ('bn_state', C.c_void_p)]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
@@ -154,6 +161,12 @@ _SIGNATURES = {
     'tfr_din_fwd': (_I, [_P, _P, _I, _I, C.POINTER(DinCfg), _P, _P, _P, _I, _P]),
     'tfr_din_bwd': (_I, [_P, _P, _I, _I, C.POINTER(DinCfg), _P, _P, _I, _P, _P, _P]),
     'tfr_din_input_grad': (_I, [C.POINTER(DinCfg), _I, _I, _P, _P, _I, _I, _P, _I, _I, _P]),
+    'tfr_dasalc_param_count': (C.c_size_t, [C.POINTER(DasalcCfg)]),
+    'tfr_dasalc_bn_state_count': (C.c_size_t, [C.POINTER(DasalcCfg)]),
+    'tfr_dasalc_workspace_bytes': (C.c_size_t, [C.POINTER(DasalcCfg), _I]),
+    'tfr_dasalc_fwd': (_I, [_P, _P, _I, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _I, _P]),
+    'tfr_dasalc_bwd': (_I, [_P, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _P, _P, _I, _I, _P]),
+    'tfr_symmetric_log1p_clip': (_I, [_P, C.c_size_t, _F, _P, _P]),
     'tfr_gam_param_count': (C.c_size_t, [C.POINTER(GamCfg)]),
     'tfr_gam_bn_state_count': (C.c_size_t, [C.POINTER(GamCfg)]),
     'tfr_gam_workspace_bytes': (C.c_size_t, [C.POINTER(GamCfg), _I]),

@@ -19,5 +19,6 @@ from ranking_b200 import model
 from ranking_b200 import train
 from ranking_b200 import data
 from ranking_b200 import pipeline
+from ranking_b200 import research
 
 __version__ = '0.1.0'

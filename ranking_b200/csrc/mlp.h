@@ -55,6 +55,10 @@ int mlp_hidden_post_fwd(int d, int M, const MlpPlan& p, const float* params, flo
 // BN gamma / beta gradients.
 int mlp_hidden_pre_bwd(int d, int M, const MlpPlan& p, const float* params, float* ws,
                        float* dz, float* grads, cudaStream_t st);
+// Batch statistics of src [M, N] into stat (mean[N], rstd[N]) through the plan's reduction
+// partials, updating the moving averages in training; the moving statistics in inference.
+int mlp_bn_batch_stats(const float* src, int M, int N, const MlpPlan& p, float* ws, float* stat,
+                       float* moving, cudaStream_t st);
 // Input BN: X -> ws + xin_off; and its parameter gradients from dL/dXin.
 int mlp_input_bn_fwd(const float* X, int M, const MlpPlan& p, const float* params, float* ws,
                      cudaStream_t st);

@@ -299,6 +299,11 @@ int mlp_hidden_pre_bwd(int d, int M, const MlpPlan& p, const float* params, floa
   return TFR_OK;
 }
 
+int mlp_bn_batch_stats(const float* src, int M, int N, const MlpPlan& p, float* ws, float* stat,
+                       float* moving, cudaStream_t st) {
+  return batch_stats(src, M, N, p, ws, stat, moving, st);
+}
+
 int mlp_input_bn_fwd(const float* X, int M, const MlpPlan& p, const float* params, float* ws,
                      cudaStream_t st) {
   const int N = p.dims[0];

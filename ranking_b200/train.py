@@ -357,6 +357,105 @@ class DINRankingTrainer(RankingTrainer):
                                 _C.ptr(grads), st))
 
 
+class _DASALCJoint(object):
+  """DocumentInteractionAttention + DASALCScorer with ONE flat parameter buffer, the DIN's
+  parameters first (the modules' `flat` become views of it), as _DINScorer."""
+
+  def __init__(self, din, scorer):
+    self.n_din = din.flat.numel()
+    self.flat = torch.nn.Parameter(torch.cat([din.flat.data, scorer.flat.data]))
+    din.flat = torch.nn.Parameter(self.flat.data[:self.n_din])
+    scorer.flat = torch.nn.Parameter(self.flat.data[self.n_din:])
+    self.bn_state = scorer.bn_state
+    self.dims = [list(din.dims), list(scorer.dims)]
+    self.use_batch_norm = True
+    self.input_batch_norm = True
+    self.input_dtype = torch.float32
+    self._run_cfg = scorer._run_cfg
+
+
+class DASALCRankingTrainer(RankingTrainer):
+  """Fused step for DASALC (research/dasalc.py): raw features x [B, N, D] go through
+
+      log1p_cutoff                            tfr_symmetric_log1p_clip
+      circular padding of the padded items    tfr_circular_pad_gather (K9)
+      E = din((x, list_mask))                 tfr_din_fwd
+      scores = scorer((x, E))                 tfr_dasalc_fwd (K13)
+      loss, d loss / d scores                 fused loss kernel
+      scorer gradients, d loss / d E          tfr_dasalc_bwd
+      DIN gradients                           tfr_din_bwd
+      optimizer                               one launch over the shared flat buffer
+
+  `din` is a DocumentInteractionAttention (built here for scorer.input_dim if it has not
+  been) with head_size == scorer.context_dim.  List validity is `mask`, or label >= 0.
+  predict runs the same chain in inference mode; fit / evaluate / checkpoints are the base
+  class's."""
+
+  def __init__(self, din, scorer, loss, cutoff=30.0, **kw):
+    if not din.built:
+      din.build(scorer.input_dim)
+    if din.input_dim != scorer.input_dim:
+      raise ValueError('the DIN was built for %d features, the scorer takes %d' %
+                       (din.input_dim, scorer.input_dim))
+    if din.head_size != scorer.context_dim:
+      raise ValueError('din.head_size %d must equal scorer.context_dim %d' %
+                       (din.head_size, scorer.context_dim))
+    if not float(cutoff) > 0:
+      raise ValueError('cutoff must be > 0')
+    self.din = din
+    self.scorer = scorer
+    self.cutoff = float(cutoff)
+    super().__init__(_DASALCJoint(din, scorer), loss, **kw)
+
+  def _new_workspace(self, b, n):
+    dev = self.device
+    h = self.din.head_size
+    self.emb = torch.empty(b * n, h, dtype=torch.float32, device=dev)
+    self.d_emb = torch.empty(b * n, h, dtype=torch.float32, device=dev)
+    self.din_ws = self.din._new_workspace(b, n)
+    return self.scorer._new_workspace(b * n)
+
+  def _prep_x(self, x):
+    if x.shape[-1] != self.scorer.input_dim:
+      raise ValueError('x has %d features, the scorer takes %d' %
+                       (x.shape[-1], self.scorer.input_dim))
+    x = x.float().contiguous()
+    if getattr(self, '_xt', None) is None or self._xt.shape != x.shape:
+      self._xt = torch.empty_like(x)
+    _C.check(_C.lib.tfr_symmetric_log1p_clip(_C.ptr(x), x.numel(), self.cutoff,
+                                             _C.ptr(self._xt), _C.stream()))
+    return self._xt
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    din, sc = self.din, self.scorer
+    lm = m8
+    if lm is None and y_true is not None:
+      lm = (y_true >= 0).reshape(-1).to(torch.uint8).contiguous()
+    self._lm = lm
+    self._din_cfg = din._run_cfg(training=training)
+    st = _C.stream()
+    _C.check(_C.lib.tfr_din_fwd(_C.ptr(x), _C.ptr(lm), b, n, ctypes.byref(self._din_cfg),
+                                _C.ptr(din.flat.data), _C.ptr(self.din_ws), _C.ptr(self.emb),
+                                din.head_size, st))
+    _C.check(_C.lib.tfr_dasalc_fwd(_C.ptr(x), _C.ptr(self.emb), din.head_size, b * n, cfg,
+                                   _C.ptr(sc.flat.data), _C.ptr(m8), _C.ptr(self.ws),
+                                   _C.ptr(self.scores), sc._precision, st))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    din, sc = self.din, self.scorer
+    h = din.head_size
+    st = _C.stream()
+    _C.check(_C.lib.tfr_dasalc_bwd(_C.ptr(x), b * n, cfg, _C.ptr(sc.flat.data),
+                                   _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                   ctypes.c_void_p(grads.data_ptr() + 4 * self.tower.n_din),
+                                   _C.ptr(self.d_emb), h, sc._precision, st))
+    _C.check(_C.lib.tfr_din_bwd(_C.ptr(x), _C.ptr(self._lm), b, n, ctypes.byref(self._din_cfg),
+                                _C.ptr(din.flat.data), _C.ptr(self.d_emb), h,
+                                _C.ptr(self.din_ws), _C.ptr(grads), st))
+
+
 class HostBatchPipeline(object):
   """End-to-end step from HOST buffers: pinned-memory batches are copied to the
   device on a copy stream, double-buffered so the copy of batch k+1 overlaps the
