@@ -8,7 +8,10 @@ same clicks:
 
   * ClickEMRankingTrainer + ClickEMLoss: relevance tower and per-position examination
     propensities learned jointly;
-  * RankingTrainer + SigmoidCrossEntropyLoss: the clicks taken as relevance labels.
+  * RankingTrainer + SigmoidCrossEntropyLoss: the clicks taken as relevance labels;
+  * with --bilinear_dim E, a third: BilinearClickRankingTrainer, a two-tower model whose
+    relevance tower and position embeddings interact through a Bilinear(E, 1), scored with
+    every item at position 0.
 
 Both are evaluated with NDCG@{1,5,10} on the TRUE grades of held-out lists, and the learned
 relative propensities are printed next to the planted ones.
@@ -68,6 +71,10 @@ def main():
   ap.add_argument('--learning_rate', type=float, default=1.0)
   ap.add_argument('--hidden', default='', help='hidden layer widths, e.g. 64,32')
   ap.add_argument('--seed', type=int, default=0)
+  ap.add_argument('--bilinear_dim', type=int, default=0,
+                  help='E > 0 (at most 8) also trains a two-tower model whose relevance '
+                       'tower and position embeddings of width E interact through a '
+                       'Bilinear(E, 1) (BilinearClickRankingTrainer)')
   args = ap.parse_args()
   if args.train_path:
     x, grades = data.load_libsvm_data(args.train_path, args.list_size, args.num_features)[:2]
@@ -80,23 +87,30 @@ def main():
   test = [(x[:n_test], grades[:n_test])]
   hidden = [int(h) for h in args.hidden.split(',') if h]
 
-  def tower():
-    return tfr.keras.layers.create_tower(hidden, 1, activation='relu', use_batch_norm=False,
+  def tower(units=1):
+    return tfr.keras.layers.create_tower(hidden, units, activation='relu', use_batch_norm=False,
                                          dropout=0, input_dim=x.shape[2], seed=args.seed)
   em = tfr.train.ClickEMRankingTrainer(tower(), tfr.keras.losses.ClickEMLoss(),
                                        args.list_size, seed=args.seed,
                                        learning_rate=args.learning_rate)
   naive = tfr.train.RankingTrainer(tower(), tfr.keras.losses.SigmoidCrossEntropyLoss(),
                                    learning_rate=args.learning_rate)
+  models = [('click_em', em), ('naive_sigmoid_ce', naive)]
+  if args.bilinear_dim > 0:
+    e = args.bilinear_dim
+    models.append(('bilinear_two_tower', tfr.train.BilinearClickRankingTrainer(
+        tower(e), tfr.keras.layers.Bilinear(e, 1, seed=args.seed),
+        tfr.keras.losses.SigmoidCrossEntropyLoss(), args.list_size, seed=args.seed,
+        learning_rate=args.learning_rate)))
   n_train = train[0].shape[0]
   for epoch in range(args.epochs):
     perm = torch.randperm(n_train, generator=torch.Generator().manual_seed(epoch)).cuda()
     for i in range(0, n_train - args.batch_size + 1, args.batch_size):
       idx = perm[i:i + args.batch_size]
       xb, cb = train[0][idx], train[1][idx]
-      em.train_step(xb, cb)
-      naive.train_step(xb, cb)
-  for name, tr in (('click_em', em), ('naive_sigmoid_ce', naive)):
+      for _, tr in models:
+        tr.train_step(xb, cb)
+  for name, tr in models:
     res = pipeline.evaluate(tr, test)
     ndcg = {k.split('/')[-1]: float(v) for k, v in res.items()}
     print('%-17s ' % name + '  '.join('NDCG@%d %.4f' % (k, ndcg['ndcg_%d' % k])

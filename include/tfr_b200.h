@@ -611,6 +611,33 @@ int tfr_embedding_bwd(const int32_t* ids, int R, int T, const float* dout, int l
                       void* workspace, float* dtable, int* bad_ids, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K14  Bilinear (keras/layers.py:807-890), the interaction layer of two-tower models for
+ * unbiased learning to rank.  v1, v2 [M, E] fp32 row-major; for every row m
+ *   y[m, k] = sum_ij v1[m, i] W[i, j, k] v2[m, j] + sum_i v1[m, i] W1[i, k]
+ *             + sum_j v2[m, j] W2[j, k] + b[k]                              y [M, K]
+ * Flat parameter layout (Keras get_weights() order): W `bilinear_term` [E, E, K] row-major,
+ * W1 `linear_term_1` [E, K], W2 `linear_term_2` [E, K], b `const_term` [K];
+ * tfr_bilinear_param_count(E, K) = E*E*K + 2*E*K + K floats.  Gradients use the same layout.
+ * row_mask (uint8 [M], optional): a row whose byte is 0 gets RestoreList's ln(1e-10) in every
+ * output; in the backward it contributes nothing to the parameter gradients and gets
+ * dv1 = dv2 = 0.
+ * The backward writes dv1, dv2 [M, E] and the six parameter gradients (=, not +=) in one pass
+ * over the rows: fixed-order per-CTA partials in the workspace (tfr_bilinear_workspace_bytes),
+ * then a fixed-order sum over the CTAs.  No float atomics: two identical calls give identical
+ * bits.  FP32 on CUDA cores (no TF32).
+ * Limits (TFR_INVALID_ARGUMENT before any CUDA call, and 0 from the size queries):
+ * M >= 1, 1 <= E <= 128, 1 <= K <= 32, E * E * K <= 16384 (W and one dW partial stay in
+ * shared memory); NULL v1 / v2 / params / y / dy / dv1 / dv2 / grads / workspace.
+ * ------------------------------------------------------------------------- */
+size_t tfr_bilinear_param_count(int E, int K);
+size_t tfr_bilinear_workspace_bytes(int M, int E, int K);
+int tfr_bilinear_fwd(const float* v1, const float* v2, int M, int E, int K, const float* params,
+                     const uint8_t* row_mask, float* y, void* stream);
+int tfr_bilinear_bwd(const float* v1, const float* v2, int M, int E, int K, const float* params,
+                     const uint8_t* row_mask, const float* dy, float* dv1, float* dv2,
+                     float* grads, void* workspace, void* stream);
+
+/* ---------------------------------------------------------------------------
  * K10  neural additive ranking model: GAMLayer (keras/layers.py:591-803) over the
  * flattened [M = B*N] rows.  Example feature f owns columns [feature_offsets[f],
  * feature_offsets[f + 1]) of X [M, D] (D = feature_offsets[F], feature_offsets[0] = 0,

@@ -867,3 +867,121 @@ class TokenEmbedding(torch.nn.Module):
   def get_config(self):
     return {'vocab_size': self.vocab_size, 'embedding_dim': self.embedding_dim,
             'combiner': self.combiner}
+
+
+class _BilinearFn(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, v1, v2, flat, layer):
+    m = v1.shape[0]
+    e, k = layer.embedding_dim, layer.output_dim
+    out = torch.empty(m, k, dtype=torch.float32, device=v1.device)
+    if m:
+      _C.check(_C.lib.tfr_bilinear_fwd(_C.ptr(v1), _C.ptr(v2), m, e, k, _C.ptr(flat), None,
+                                        _C.ptr(out), _C.stream()))
+    ctx.layer = layer
+    ctx.save_for_backward(v1, v2, flat)
+    return out
+
+  @staticmethod
+  def backward(ctx, g_out):
+    v1, v2, flat = ctx.saved_tensors
+    layer = ctx.layer
+    m = v1.shape[0]
+    e, k = layer.embedding_dim, layer.output_dim
+    dv1, dv2 = torch.empty_like(v1), torch.empty_like(v2)
+    grads = torch.zeros_like(flat)
+    if m:
+      g = g_out.contiguous()
+      ws = torch.empty(_C.lib.tfr_bilinear_workspace_bytes(m, e, k), dtype=torch.uint8,
+                       device=v1.device)
+      _C.check(_C.lib.tfr_bilinear_bwd(_C.ptr(v1), _C.ptr(v2), m, e, k, _C.ptr(flat), None,
+                                        _C.ptr(g), _C.ptr(dv1), _C.ptr(dv2), _C.ptr(grads),
+                                        _C.ptr(ws), _C.stream()))
+    return dv1, dv2, grads, None
+
+
+class Bilinear(torch.nn.Module):
+  """keras/layers.py:807-890: the bilinear interaction of two vectors of the same width E,
+  used by two-tower models for unbiased learning to rank (Yan et al., "Revisiting two tower
+  models for unbiased learning to rank"):
+
+      y[..., k] = v1 W[:, :, k] v2 + v1 W1[:, k] + v2 W2[:, k] + b[k]
+
+  forward((v1, v2)) takes two tensors of the same shape [..., E] and returns [..., K].  Runs
+  in the K14 kernels (csrc/bilinear.cu); gradients reach both inputs and the parameters.  The
+  parameters are ONE flat fp32 parameter (`flat`) in Keras get_weights() order: W
+  `bilinear_term` [E, E, K], W1 `linear_term_1` [E, K], W2 `linear_term_2` [E, K], b
+  `const_term` [K], initialised as the reference does (RandomNormal(stddev=1/E) for W,
+  RandomNormal(stddev=1/sqrt(E)) for W1 and W2, zeros for b) from a generator seeded with
+  `seed`.  Limits: 1 <= E <= 128, 1 <= K <= 32, E * E * K <= 16384."""
+
+  def __init__(self, embedding_dim, output_dim, seed=None, device='cuda', name=None):
+    super().__init__()
+    self.embedding_dim = int(embedding_dim)
+    self.output_dim = int(output_dim)
+    self.name = name
+    e, k = self.embedding_dim, self.output_dim
+    n = _C.lib.tfr_bilinear_param_count(e, k)
+    if n == 0:
+      raise ValueError(_C.last_error())
+    gen = torch.Generator()
+    gen.manual_seed(int(seed) if seed is not None else torch.seed())
+    normal = lambda size, std: (torch.randn(size, generator=gen, dtype=torch.float64) *  # noqa
+                                std).float()
+    flat = torch.cat([normal(e * e * k, 1.0 / e), normal(e * k, 1.0 / math.sqrt(e)),
+                      normal(e * k, 1.0 / math.sqrt(e)), torch.zeros(k)])
+    assert flat.numel() == n
+    self.flat = torch.nn.Parameter(flat.to(device))
+    self.dims = ['bilinear', e, k]
+
+  def _offsets(self):
+    e, k = self.embedding_dim, self.output_dim
+    return e * e * k, e * e * k + e * k, e * e * k + 2 * e * k
+
+  def bilinear_term(self):
+    e, k = self.embedding_dim, self.output_dim
+    return self.flat[:e * e * k].view(e, e, k)
+
+  def linear_term_1(self):
+    a, b, _ = self._offsets()
+    return self.flat[a:b].view(self.embedding_dim, self.output_dim)
+
+  def linear_term_2(self):
+    _, b, c = self._offsets()
+    return self.flat[b:c].view(self.embedding_dim, self.output_dim)
+
+  def const_term(self):
+    _, _, c = self._offsets()
+    return self.flat[c:c + self.output_dim]
+
+  def load_keras_weights(self, weights):
+    """Loads Keras `get_weights()`: [bilinear_term, linear_term_1, linear_term_2,
+    const_term]."""
+    parts = [torch.as_tensor(w, dtype=torch.float32).reshape(-1) for w in weights]
+    flat = torch.cat(parts) if parts else torch.zeros(0)
+    if len(parts) != 4 or flat.numel() != self.flat.numel():
+      raise ValueError('expected the 4 weights of a Bilinear(%d, %d) (%d values), got %d arrays '
+                       'with %d values' % (self.embedding_dim, self.output_dim,
+                                           self.flat.numel(), len(parts), flat.numel()))
+    with torch.no_grad():
+      self.flat.copy_(flat)
+
+  def forward(self, inputs):
+    v1, v2 = inputs
+    _C.require_cuda(v1, 'Bilinear inputs')
+    _C.require_cuda(v2, 'Bilinear inputs')
+    if v1.shape != v2.shape:
+      raise ValueError('the two inputs must have the same shape, got %s and %s' %
+                       (tuple(v1.shape), tuple(v2.shape)))
+    if v1.dim() < 1 or v1.shape[-1] != self.embedding_dim:
+      raise ValueError('expected last dim %d, got %s' % (self.embedding_dim, tuple(v1.shape)))
+    lead = v1.shape[:-1]
+    e = self.embedding_dim
+    a = v1.reshape(-1, e).float().contiguous()
+    c = v2.reshape(-1, e).float().contiguous()
+    out = _BilinearFn.apply(a, c, self.flat, self)
+    return out.reshape(*lead, self.output_dim)
+
+  def get_config(self):
+    return {'embedding_dim': self.embedding_dim, 'output_dim': self.output_dim}

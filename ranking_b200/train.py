@@ -522,14 +522,21 @@ class HostBatchPipeline(object):
 
 
 class _EmbeddingScorer(object):
-  """Embedding tables (+ a DocumentInteractionAttention) + tower as one scorer with ONE flat
-  parameter buffer: the tables first (in the given order), then the DIN if there is one, then
+  """Embedding tables (+ one module between them and the tower: a
+  DocumentInteractionAttention or a Bilinear) + tower as one scorer with ONE flat parameter
+  buffer: the tables first (in the given order), then the middle module if there is one, then
   the tower (the modules' `flat` become views of it), so the step keeps one gradient
-  all-reduce and one optimizer launch."""
+  all-reduce and one optimizer launch.  The middle block takes its size rounded up to a
+  multiple of `middle_align` floats; the padding stays zero and is never read."""
 
-  def __init__(self, tables, tower, din=None):
-    mods = list(tables) + ([din] if din is not None else [])
-    self.flat = torch.nn.Parameter(torch.cat([t.flat.data for t in mods] + [tower.flat.data]))
+  def __init__(self, tables, tower, middle=None, middle_align=1):
+    parts = [t.flat.data for t in tables]
+    n_mid = 0
+    if middle is not None:
+      n_mid = middle.flat.numel()
+      pad = -n_mid % middle_align
+      parts += [middle.flat.data, middle.flat.data.new_zeros(pad)]
+    self.flat = torch.nn.Parameter(torch.cat(parts + [tower.flat.data]))
     self.table_offsets = []
     off = 0
     for t in tables:
@@ -538,11 +545,11 @@ class _EmbeddingScorer(object):
       self.table_offsets.append(off)
       off += n
     self.n_tables = off
-    self.n_din = 0
-    if din is not None:
-      self.n_din = din.flat.numel()
-      din.flat = torch.nn.Parameter(self.flat.data[off:off + self.n_din])
-      off += self.n_din
+    self.n_middle = n_mid
+    if middle is not None:
+      middle.flat = torch.nn.Parameter(self.flat.data[off:off + n_mid])
+      off += n_mid + pad
+    mods = list(tables) + ([middle] if middle is not None else [])
     self.tower_offset = off
     tower.flat = torch.nn.Parameter(self.flat.data[off:])
     self.bn_state = tower.bn_state
@@ -822,7 +829,7 @@ class DINEmbeddingRankingTrainer(EmbeddingRankingTrainer):
         self.split += self.embeddings[ti].embedding_dim
 
   def _scorer(self, tables, tower):
-    return _EmbeddingScorer(tables, tower, din=self.din)
+    return _EmbeddingScorer(tables, tower, middle=self.din)
 
   def _new_workspace(self, b, n):
     m, dev = b * n, self.device
@@ -1002,3 +1009,149 @@ class ClickEMRankingTrainer(RankingTrainer):
     self._backward(x, m8, cfg, grads)
     self._apply(grads)
     return self.total2[0]
+
+
+class BilinearClickRankingTrainer(RankingTrainer):
+  """Learns a relevance tower from position-biased clicks with the two-tower model of Yan et
+  al., "Revisiting two tower models for unbiased learning to rank": a relevance tower and a
+  position embedding interact through a keras.layers.Bilinear into the click logit, so the
+  bias model is not restricted to click = examination x relevance.
+
+      r = tower(x)                   [B * N, E]   tfr_mlp_fwd (tower.output_units = E)
+      p = table[position]            [B * N, E]   tfr_embedding_fwd (one id per item, SUM)
+      c = bilinear((r, p))           [B, N]       tfr_bilinear_fwd (K14), ln(1e-10) where
+                                                  `mask` is 0
+      loss, d c                                   the loss's fused kernel, clicks as labels
+      d r, d p, bilinear gradients                tfr_bilinear_bwd
+      tower gradients                             tfr_mlp_bwd with d scores = d r
+      table gradient                              tfr_embedding_bwd (deterministic)
+      optimizer                                   one launch over the shared flat buffer
+
+  `tower`: a create_tower tower with output_units = bilinear.embedding_dim (the tower's output
+  layer takes at most 8 units, so E <= 8); precision fp32, tf32x3 or tf32; BN is allowed, with
+  circular padding as in the base class.  `bilinear`: a keras.layers.Bilinear(E, 1).  `loss`:
+  a loss whose fused kernel takes [B, N] logits, e.g. keras.losses.SigmoidCrossEntropyLoss
+  (not ClickEMLoss or MixtureEMLoss).  The position table is a
+  keras.layers.TokenEmbedding(num_positions, E, combiner='sum') seeded with `seed`.  Table,
+  bilinear and tower share one flat parameter buffer (_EmbeddingScorer), so checkpoints, the
+  optimizer and the data-parallel reducer cover them.  The table's rows and the bilinear block
+  are padded to multiples of 64 floats so that the tower's parameters keep the 256-byte
+  alignment of a tower's own allocation; the padding is never read and keeps its value.
+  Labels are clicks (>= 1 clicked, < 0 padding).  `predict` places every item at
+  `serving_position` unless `positions` is given, so its scores rank by relevance and
+  pipeline.fit / evaluate work unchanged."""
+
+  _ALIGN = 64
+
+  def __init__(self, tower, bilinear, loss, num_positions, serving_position=0, seed=None, **kw):
+    from ranking_b200.keras import layers as keras_layers
+    from ranking_b200.keras import losses as keras_losses
+    if isinstance(loss, (keras_losses.ClickEMLoss, keras_losses.MixtureEMLoss)):
+      raise ValueError('BilinearClickRankingTrainer needs a loss over [B, N] click logits '
+                       '(e.g. SigmoidCrossEntropyLoss), not %s' % type(loss).__name__)
+    if tower.precision not in ('fp32', 'tf32x3', 'tf32'):
+      raise ValueError('the relevance tower must use precision fp32, tf32x3 or tf32')
+    if tower.output_units != bilinear.embedding_dim:
+      raise ValueError('the relevance tower has output_units %d, the bilinear layer takes '
+                       'embedding_dim %d' % (tower.output_units, bilinear.embedding_dim))
+    if bilinear.output_dim != 1:
+      raise ValueError('the bilinear layer must have output_dim 1 (one click logit), got %d' %
+                       bilinear.output_dim)
+    if bilinear.flat.device != tower.flat.device:
+      raise ValueError('the bilinear layer and the tower must live on the same device')
+    num_positions = int(num_positions)
+    if num_positions < 1:
+      raise ValueError('num_positions must be >= 1')
+    serving_position = int(serving_position)
+    if not 0 <= serving_position < num_positions:
+      raise ValueError('serving_position must lie in [0, %d)' % num_positions)
+    e = bilinear.embedding_dim
+    rows = num_positions
+    while rows * e % self._ALIGN:
+      rows += 1
+    self.num_positions = num_positions
+    self.serving_position = serving_position
+    self.positions_table = keras_layers.TokenEmbedding(rows, e, combiner='sum', seed=seed,
+                                                       device=tower.flat.device)
+    self.bilinear = bilinear
+    self.mlp = tower
+    super().__init__(_EmbeddingScorer([self.positions_table], tower, middle=bilinear,
+                                      middle_align=self._ALIGN), loss, **kw)
+    self._pos = None
+
+  def _new_workspace(self, b, n):
+    dev, m, e = self.device, b * n, self.bilinear.embedding_dim
+    self.rel = torch.empty(m, e, dtype=torch.float32, device=dev)
+    self.pemb = torch.empty(m, e, dtype=torch.float32, device=dev)
+    self.drel = torch.empty(m, e, dtype=torch.float32, device=dev)
+    self.dpemb = torch.empty(m, e, dtype=torch.float32, device=dev)
+    self._default_pos = torch.arange(n, device=dev).clamp(max=self.num_positions - 1).to(
+        torch.int32).expand(b, n).contiguous()
+    self._serving_pos = torch.full((b, n), self.serving_position, dtype=torch.int32, device=dev)
+    emb = self.positions_table
+    self._emb_ws = torch.empty(_C.lib.tfr_embedding_workspace_bytes(m, 1, emb.vocab_size, e),
+                               dtype=torch.uint8, device=dev)
+    self._bil_ws = torch.empty(_C.lib.tfr_bilinear_workspace_bytes(m, e, 1), dtype=torch.uint8,
+                               device=dev)
+    return self.mlp._new_workspace(m)
+
+  def _set_positions(self, positions, b, n, default):
+    if positions is None:
+      self._pos = default
+      return
+    if tuple(positions.shape) != (b, n):
+      raise ValueError('positions must have shape [batch_size, list_size] = %s, got %s' %
+                       ((b, n), tuple(positions.shape)))
+    pos = positions.to(self.device, torch.int32).contiguous()
+    if bool(((pos < 0) | (pos >= self.num_positions)).any()):
+      raise ValueError('positions must lie in [0, %d)' % self.num_positions)
+    self._pos = pos
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    m, mlp, emb, bil = b * n, self.mlp, self.positions_table, self.bilinear
+    e = bil.embedding_dim
+    st = _C.stream()
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(x), m, cfg, _C.ptr(mlp.flat.data), _C.ptr(m8),
+                                _C.ptr(self.ws), _C.ptr(self.rel), mlp._precision, st))
+    _C.check(_C.lib.tfr_embedding_fwd(_C.ptr(self._pos), m, 1, _C.ptr(emb.flat.data),
+                                      emb.vocab_size, e, emb._combiner, 1, _C.ptr(self.pemb), e,
+                                      None, st))
+    _C.check(_C.lib.tfr_bilinear_fwd(_C.ptr(self.rel), _C.ptr(self.pemb), m, e, 1,
+                                      _C.ptr(bil.flat.data), _C.ptr(m8), _C.ptr(self.scores), st))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    m, mlp, emb, bil, sc = b * n, self.mlp, self.positions_table, self.bilinear, self.tower
+    e = bil.embedding_dim
+    st = _C.stream()
+    _C.check(_C.lib.tfr_bilinear_bwd(_C.ptr(self.rel), _C.ptr(self.pemb), m, e, 1,
+                                      _C.ptr(bil.flat.data), _C.ptr(m8), _C.ptr(self.dscores),
+                                      _C.ptr(self.drel), _C.ptr(self.dpemb),
+                                      ctypes.c_void_p(grads.data_ptr() + 4 * sc.n_tables),
+                                      _C.ptr(self._bil_ws), st))
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(x), m, cfg, _C.ptr(mlp.flat.data), _C.ptr(self.drel),
+                                _C.ptr(m8), _C.ptr(self.ws),
+                                ctypes.c_void_p(grads.data_ptr() + 4 * sc.tower_offset),
+                                mlp._precision, st))
+    _C.check(_C.lib.tfr_embedding_bwd(_C.ptr(self._pos), m, 1, _C.ptr(self.dpemb), e, 1,
+                                      emb.vocab_size, e, emb._combiner, 0, _C.ptr(self._emb_ws),
+                                      _C.ptr(grads), None, st))
+
+  def train_step(self, x, clicks, positions=None, sample_weight=None, mask=None):
+    """x [B, N, D] (device, fp32), clicks [B, N] (>= 1 clicked, < 0 padding), positions
+    ([B, N] int in [0, num_positions), optional: by default an item's position is its row
+    in the list, clipped to num_positions - 1, i.e. the logged display order).  Returns the
+    scalar loss as a 0-d device tensor."""
+    b, n, _ = x.shape
+    self._ensure(b, n)
+    self._set_positions(positions, b, n, self._default_pos)
+    return super().train_step(x, clicks, sample_weight=sample_weight, mask=mask)
+
+  @torch.no_grad()
+  def predict(self, x, mask=None, y_true=None, positions=None):
+    """Click logits [B, N] with every item at `serving_position` (or at `positions`)."""
+    b, n, _ = x.shape
+    self._ensure(b, n)
+    self._set_positions(positions, b, n, self._serving_pos)
+    return super().predict(x, mask=mask, y_true=y_true)
