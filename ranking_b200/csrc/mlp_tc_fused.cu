@@ -1,15 +1,21 @@
 // K5/K6 fused 3xTF32 forward of the scorer tower: every hidden Dense layer from
 // `first_layer` on, plus the output layer, in one persistent kernel.
 //
-// A CTA (two consumer warpgroups, one per SM) owns a 128-row tile of M at a time and walks
-// the tower depth-first on it.  Only the first fused layer reads its A operand (X) from
-// HBM, through the cp.async ring; every later layer takes its A fragments from Hbuf, a
-// padded 128 x 128 fp32 tile in shared memory that the previous layer's epilogue wrote.  A
-// first layer wider than 128 runs in two 128-column chunks, and the next layer consumes
-// each chunk as soon as its epilogue has written it (k 0..127, then 128..255), its
-// accumulator kept in registers meanwhile.  Each epilogue still stores H_d and the ReLU
-// sign words to the workspace, as the backward reads them; the output layer then reads the
-// last hidden layer from Hbuf.
+// A CTA (one per SM) owns a 128-row tile of M at a time and walks the tower depth-first on
+// it.  Only the first fused layer reads its A operand (X) from HBM, through the cp.async
+// ring; every later layer takes its A fragments from Hbuf, a padded 128 x 128 fp32 tile in
+// shared memory that the previous layer's epilogue wrote.  A first layer wider than 128 runs
+// in two 128-column chunks, and the next layer consumes each chunk as soon as its epilogue
+// has written it (k 0..127, then 128..255), its accumulator kept in registers meanwhile.
+//
+// Threads 0-255 are the two MMA warpgroups (setmaxnreg 208): the ring, the k loop, and the
+// half of each epilogue the next layer needs, bias + activation into Hbuf.  Threads 256-383
+// are the epilogue warpgroup (setmaxnreg 88): after each such Hbuf write it stores H_d and
+// the ReLU sign words to the workspace from Hbuf (the backward reads them), and after a
+// tile's last hidden layer it computes the output layer from Hbuf, while the MMA warps run
+// the next layer's k loop.  The hand-off is the GEMM engine's (wgmma_gemm.cuh): the MMA
+// warps arrive at kBarFull once Hbuf is written and wait at kBarFree before they overwrite
+// it; the epilogue warpgroup waits at kBarFull and arrives at kBarFree once it has read it.
 //
 // The k blocks of a tile form one linear sequence (config 2: 5 + 4 + 5 + 4 + 4 blocks), and
 // the ring prefetches stages - 1 blocks ahead along it, across layer boundaries, epilogues
@@ -22,8 +28,10 @@
 // wg::gemm_kernel, and the scores are summed in out_layer_fwd_kernel's order (per-lane fma
 // chains over k = lane, lane + 32, ..., then warp_sum).
 //
-// Hbuf rows are private to a warp: the accumulator rows of warp w (16 w .. 16 w + 15) are
-// the rows its A fragments read and the rows it scores, so Hbuf needs only __syncwarp.
+// Between an MMA warp's Hbuf write and its next layer's fragment loads only __syncwarp is
+// needed: the accumulator rows of warp w (16 w .. 16 w + 15) are the rows its A fragments
+// read.  Hbuf is not warp-private as a whole, though: the epilogue warpgroup reads every row,
+// hence kBarFree before every Hbuf write but a CTA's first.
 #include "common.cuh"
 #include "mlp.h"
 #include "wgmma_gemm.cuh"
@@ -40,6 +48,10 @@ constexpr int kSmem = kStages * kStage + wg::BM * kHPitch + 1024;   // + alignme
 static_assert(kSmem == 222208, "fused forward shared memory: 3 stages + Hbuf + slack");
 static_assert(kSmem <= wg::kSmemLimit, "fused forward exceeds the shared memory of a CTA");
 constexpr int kMaxSegs = 4 + TFR_MLP_MAX_LAYERS;
+constexpr int kHP = kHPitch / 4;                           // Hbuf pitch in floats
+// kBarFull / kBarFree: the 256 MMA threads and the 128 epilogue threads, once per Hbuf write.
+// Both sides walk the same (tile, segment with epi) sequence, so every wait has its arrive.
+constexpr int kHandoff = wg::kThreads + wg::kEpiThreads;
 
 // A run of k blocks of one layer that accumulates into one accumulator.
 struct Seg {
@@ -113,6 +125,7 @@ struct FusedCta {
   int lane, wrow;   // wrow: first of this warp's 16 tile rows
   int s;            // stage of the block being consumed
   int p_tile, p_seg, p_kb, p_s;   // the block the next copy fetches, and its stage
+  bool handed;      // Hbuf has been handed to the epilogue warpgroup before
 
   // Copies the next block of the sequence into its stage (nothing past the last tile) and
   // commits one cp.async group either way.
@@ -166,7 +179,7 @@ struct FusedCta {
       const uint32_t st = sbase + s * kStage;
       wg::cp_async_wait<kStages - 2>();
       wg::fence_proxy_async();   // cp.async writes -> visible to the tensor cores
-      __syncthreads();
+      wg::bar_sync(wg::kBarMma, wg::kThreads);
       // refill the stage of the previous block, whose MMAs every warpgroup retired
       produce();
       const int kg = (sg.kb0 + kb) * 32;   // first k of the block within the layer
@@ -197,106 +210,152 @@ struct FusedCta {
     if (sg.epi) epilogue(acc, sg, m0, two_n);
   }
 
-  // bias / activation / sign words / H_d store as wg::gemm_kernel's EPI_BIAS_ACT, plus the
-  // tile's columns into Hbuf (zero past N: the next layer's zero-filled k tail).
+  // The MMA warps' half of an epilogue: bias and activation as wg::gemm_kernel's EPI_BIAS_ACT,
+  // zero past M and N (the next layer's zero-filled k tail), into Hbuf; then Hbuf goes to the
+  // epilogue warpgroup, which stores it.
   __device__ __forceinline__ void epilogue(float (&acc)[2][32], const Seg& sg, int m0, bool two_n) {
     // accumulator element j of half h: row = lane / 4 + 8 ((j / 2) % 2),
     // column = 64 h + 8 (j / 4) + 2 (lane % 4) + j % 2
-    const int rbase = m0 + wrow + (lane >> 2);
-    const bool vec2 = (sg.N % 2) == 0 && (reinterpret_cast<uintptr_t>(sg.C) & 7u) == 0;
     float* hb = reinterpret_cast<float*>(smem + kHbufOff);
-    __syncwarp();   // this warp's earlier Hbuf reads are done
+    // the epilogue warpgroup is done with the last Hbuf (this warp's own reads of it are too)
+    if (handed) wg::bar_sync(wg::kBarFree, kHandoff);
+    else __syncwarp();
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (h == 1 && !two_n) break;
 #pragma unroll
-      for (int c32 = 0; c32 < 2; ++c32) {   // 32-column chunks of this half
-        const int chunk_col = sg.n0 + h * 64 + c32 * 32;
-        if (chunk_col >= sg.N) break;
-        uint32_t bits_out[2] = {0u, 0u};
-#pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {
-          const int j = c32 * 16 + jj;
-          const int rr = (j >> 1) & 1;
-          const int cin = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
-          const int col = sg.n0 + h * 64 + cin;
-          const int row = rbase + 8 * rr;
-          float x = acc[h][j];
-          x += col < sg.N ? __ldg(sg.bias + col) : 0.f;
-          if (a.act == TFR_ACT_RELU) x = fmaxf(x, 0.f);
-          if (row >= a.M || col >= sg.N) x = 0.f;
-          acc[h][j] = x;
-          bits_out[rr] |= (x > 0.f ? 1u : 0u) << (cin & 31);
-        }
-        if (sg.bits) {
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {
-            uint32_t w = bits_out[rr];
-            w |= __shfl_xor_sync(0xffffffffu, w, 1);
-            w |= __shfl_xor_sync(0xffffffffu, w, 2);
-            const int row = rbase + 8 * rr;
-            if ((lane & 3) == 0 && row < a.M)
-              sg.bits[static_cast<size_t>(chunk_col >> 5) * a.M + row] = w;
-          }
-        }
-      }
-#pragma unroll
       for (int j = 0; j < 32; j += 2) {
         const int cin = h * 64 + 8 * (j >> 2) + 2 * (lane & 3);
-        const int col = sg.n0 + cin;
         const int rl = wrow + (lane >> 2) + 8 * ((j >> 1) & 1);
-        const int row = m0 + rl;
-        const bool live = col < sg.N;
-        *reinterpret_cast<float2*>(hb + rl * (kHPitch / 4) + cin) =
-            make_float2(live ? acc[h][j] : 0.f, live && col + 1 < sg.N ? acc[h][j + 1] : 0.f);
-        if (row >= a.M || !live) continue;
-        const float x0 = acc[h][j], x1 = acc[h][j + 1];
-        const bool both = col + 1 < sg.N;
-        float* p = sg.C + static_cast<size_t>(row) * sg.N + col;
-        if (both && vec2) {
-          *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
-        } else {
-          p[0] = x0;
-          if (both) p[1] = x1;
+        float x[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = sg.n0 + cin + e;
+          float v = acc[h][j + e];
+          v += col < sg.N ? __ldg(sg.bias + col) : 0.f;
+          if (a.act == TFR_ACT_RELU) v = fmaxf(v, 0.f);
+          if (m0 + rl >= a.M || col >= sg.N) v = 0.f;
+          x[e] = v;
         }
+        *reinterpret_cast<float2*>(hb + rl * kHP + cin) = make_float2(x[0], x[1]);
       }
     }
     __syncwarp();   // Hbuf written before any lane of the warp reads it
-  }
-
-  // scores of this warp's 16 rows from the last hidden layer in Hbuf, in
-  // out_layer_fwd_kernel's order; RestoreList fill for masked rows
-  __device__ __forceinline__ void out_layer(int m0) {
-    const float* hb = reinterpret_cast<const float*>(smem + kHbufOff);
-    for (int r0 = 0; r0 < 16; r0 += 4) {
-      for (int o = 0; o < a.O; ++o) {
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int k = lane; k < a.Kout; k += 32) {
-          const float w = __ldg(a.Wout + static_cast<size_t>(k) * a.O + o);
-#pragma unroll
-          for (int r = 0; r < 4; ++r)
-            acc[r] = fmaf(hb[(wrow + r0 + r) * (kHPitch / 4) + k], w, acc[r]);
-        }
-#pragma unroll
-        for (int r = 0; r < 4; ++r) acc[r] = warp_sum(acc[r]);
-        const int row = m0 + wrow + r0 + lane;
-        if (lane < 4 && row < a.M) {
-          float v = (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]) +
-                    __ldg(a.bout + o);
-          if (a.mask && a.O == 1 && !a.mask[row]) v = kLogEpsilon;
-          a.scores[static_cast<size_t>(row) * a.O + o] = v;
-        }
-      }
-    }
+    wg::bar_arrive(wg::kBarFull, kHandoff);
+    handed = true;
   }
 };
 
-__global__ void __launch_bounds__(wg::kThreads, 1)
+// H_d and the ReLU sign words of one segment's columns, read back from Hbuf by the epilogue
+// warpgroup.  Warp ew takes tile rows 32 ew .. 32 ew + 31, a lane 4 adjacent columns of each,
+// so a row is stored as one 512-byte line and the 8 lanes of a 32-column plane assemble its
+// sign word with three shuffles.  PAIR (at most 64 live columns): lanes 0-15 take row i and
+// lanes 16-31 row i + 1 (a 256-byte line each).  Widths are multiples of 4 (check_dims), so a
+// lane's 4 columns are all live or none.  Lane 8 p + q keeps the word of row 8 b + q of its
+// plane and stores it once block b's 8 rows are done: a 32-byte sector per plane.
+template <bool PAIR>
+__device__ __forceinline__ void store_rows(const FusedArgs& a, const Seg& sg, const float* hb,
+                                           int m0, int ew, int lane) {
+  constexpr int STEP = PAIR ? 2 : 1;
+  const int cl = PAIR ? lane & 15 : lane, half = PAIR ? lane >> 4 : 0;
+  const int col = sg.n0 + 4 * cl;
+  const bool on = col < sg.N;
+  const bool vec4 = (reinterpret_cast<uintptr_t>(sg.C) & 15u) == 0;
+  const int r0 = m0 + 32 * ew;
+  const int rows = a.M - r0;   // live rows of this warp's 32 (all of them when > 32)
+  const int pcol = sg.n0 + 32 * (cl >> 3);   // first column of this lane's plane
+  uint32_t* bo = sg.bits && pcol < sg.N && (!PAIR || (lane & 1) == half)
+                     ? sg.bits + static_cast<size_t>(pcol >> 5) * a.M + r0 + (lane & 7)
+                     : nullptr;
+  const float* sp = hb + (32 * ew + half) * kHP + 4 * cl;
+  float* cp = sg.C + static_cast<size_t>(r0 + half) * sg.N + col;
+  uint32_t keep = 0u;
+#pragma unroll 4
+  for (int i = 0; i < 32; i += STEP) {
+    const float4 v = *reinterpret_cast<const float4*>(sp + i * kHP);
+    if (sg.bits) {
+      const uint32_t nib = (v.x > 0.f ? 1u : 0u) | (v.y > 0.f ? 2u : 0u) |
+                           (v.z > 0.f ? 4u : 0u) | (v.w > 0.f ? 8u : 0u);
+      uint32_t w = nib << (4 * (lane & 7));
+      w |= __shfl_xor_sync(0xffffffffu, w, 1);
+      w |= __shfl_xor_sync(0xffffffffu, w, 2);
+      w |= __shfl_xor_sync(0xffffffffu, w, 4);
+      if (((i + half) & 7) == (lane & 7)) keep = w;
+      if (((i + STEP) & 7) == 0 && bo && (i & ~7) + (lane & 7) < rows) bo[i & ~7] = keep;
+    }
+    if (on && i + half < rows) {
+      float* p = cp + static_cast<size_t>(i) * sg.N;
+      if (vec4) {
+        *reinterpret_cast<float4*>(p) = v;
+      } else {
+        p[0] = v.x; p[1] = v.y; p[2] = v.z; p[3] = v.w;
+      }
+    }
+  }
+}
+
+// Scores of tile rows 32 ew .. 32 ew + 31 from the last hidden layer in Hbuf, in
+// out_layer_fwd_kernel's order; RestoreList fill for masked rows.
+__device__ __forceinline__ void out_rows(const FusedArgs& a, const float* hb, int m0, int ew,
+                                         int lane) {
+  for (int r0 = 32 * ew; r0 < 32 * ew + 32; r0 += 4) {
+    for (int o = 0; o < a.O; ++o) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int k = lane; k < a.Kout; k += 32) {
+        const float w = __ldg(a.Wout + static_cast<size_t>(k) * a.O + o);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) acc[r] = fmaf(hb[(r0 + r) * kHP + k], w, acc[r]);
+      }
+#pragma unroll
+      for (int r = 0; r < 4; ++r) acc[r] = warp_sum(acc[r]);
+      const int row = m0 + r0 + lane;
+      if (lane < 4 && row < a.M) {
+        float v = (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]) +
+                  __ldg(a.bout + o);
+        if (a.mask && a.O == 1 && !a.mask[row]) v = kLogEpsilon;
+        a.scores[static_cast<size_t>(row) * a.O + o] = v;
+      }
+    }
+  }
+}
+
+// The epilogue warpgroup walks the CTA's tiles and segments as the MMA warps do and takes
+// every Hbuf they hand over; the last segment with an epilogue is the last hidden layer, whose
+// Hbuf also feeds the output layer.  It frees Hbuf after every pass but the CTA's last, which
+// nobody would wait for.
+__device__ __forceinline__ void epilogue_warpgroup(const FusedArgs& a, const float* hb) {
+  const int lane = threadIdx.x & 31, ew = (threadIdx.x - wg::kThreads) >> 5;
+  int last = 0;
+  for (int q = 0; q < a.nseg; ++q)
+    if (a.seg[q].epi) last = q;
+  for (int tile = blockIdx.x; tile < a.m_tiles; tile += gridDim.x) {
+    const int m0 = tile * wg::BM;
+    for (int q = 0; q <= last; ++q) {
+      const Seg& sg = a.seg[q];
+      if (!sg.epi) continue;
+      wg::bar_sync(wg::kBarFull, kHandoff);
+      if (sg.N - sg.n0 <= 64) store_rows<true>(a, sg, hb, m0, ew, lane);
+      else store_rows<false>(a, sg, hb, m0, ew, lane);
+      if (q == last) out_rows(a, hb, m0, ew, lane);
+      if (q != last || tile + static_cast<int>(gridDim.x) < a.m_tiles)
+        wg::bar_arrive(wg::kBarFree, kHandoff);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kHandoff, 1)
 tower_fused_fwd_kernel(const __grid_constant__ FusedArgs args) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (wg::smem_u32(smem_raw) & 1023u)) & 1023u);
+  if (threadIdx.x >= wg::kThreads) {
+    wg::setmaxnreg_dec<wg::kEpiRegs>();
+    epilogue_warpgroup(args, reinterpret_cast<const float*>(smem + kHbufOff));
+    return;
+  }
+  wg::setmaxnreg_inc<wg::kMmaRegs>();
   FusedCta cta{args, smem, wg::smem_u32(smem), static_cast<int>(threadIdx.x & 31),
-               static_cast<int>(threadIdx.x >> 5) * 16, 0, static_cast<int>(blockIdx.x), 0, 0, 0};
+               static_cast<int>(threadIdx.x >> 5) * 16, 0, static_cast<int>(blockIdx.x), 0, 0, 0,
+               false};
   // cp.async groups: stages - 1 up front, then one per consumed block (empty past the end),
   // so a block's group is complete once at most stages - 2 younger groups are pending
   for (int p = 0; p < kStages - 1; ++p) cta.produce();
@@ -307,7 +366,6 @@ tower_fused_fwd_kernel(const __grid_constant__ FusedArgs args) {
       if (args.seg[q].acc == 0) cta.run_seg(acc0, args.seg[q], m0);
       else cta.run_seg(acc1, args.seg[q], m0);
     }
-    cta.out_layer(m0);
   }
 }
 
@@ -362,7 +420,7 @@ int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
   const int grid = a.m_tiles < sms ? a.m_tiles : sms;
   TFR_CUDA_OK(cudaFuncSetAttribute(fused::tower_fused_fwd_kernel,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, fused::kSmem));
-  fused::tower_fused_fwd_kernel<<<grid, wg::kThreads, fused::kSmem, st>>>(a);
+  fused::tower_fused_fwd_kernel<<<grid, fused::kHandoff, fused::kSmem, st>>>(a);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

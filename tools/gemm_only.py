@@ -7,7 +7,9 @@ GEMMs as they would run on a transposed dZ (dZ^T [width][M]): direct orientation
 MN-major activations, B = dZ^T K-major, copied by cp.async and split in shared memory; same
 shapes and split-K count as dw1-dw3.  The last line times the
 whole 3xTF32 forward of the config-2 tower (136-256-128-64-1, the fused kernel) through
-tfr_mlp_fwd: X read once; H1, H2, H3, their sign words and the scores written once.
+tfr_mlp_fwd: X read once; H1, H2, H3, their sign words and the scores written once.  It
+also prints fwd1 + fwd2 + fwd3 from the same run, the per-layer forward's GEMMs, to compare
+against.
 usage: gemm_only.py [--reps R] [--warmup W] [--out FILE.json]"""
 import argparse
 import json
@@ -126,13 +128,17 @@ def main():
   print('dw1-dw3 %.1f us, dw1t-dw3t %.1f us (%+.1f %%)' % (dw, dwt, 100.0 * (dwt / dw - 1.0)),
         flush=True)
   fwd = time_tower_fwd(dev, g, args.reps, args.warmup)
-  print('tower fwd (tfr_mlp_fwd, M %d)  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s' % (
-      M, fwd['us'], fwd['tflops'], fwd['gbps']), flush=True)
+  per_layer = sum(r['us'] for r in step if r['gemm'].startswith('fwd'))
+  print('tower fwd (tfr_mlp_fwd, M %d)  %8.1f us  %6.1f TFLOP/s  %7.1f GB/s  '
+        '(fwd1 + fwd2 + fwd3 %.1f us, %+.1f %%)' % (
+            M, fwd['us'], fwd['tflops'], fwd['gbps'], per_layer,
+            100.0 * (fwd['us'] / per_layer - 1.0)), flush=True)
   if args.out:
     with open(args.out, 'w') as f:
       json.dump(dict(device=torch.cuda.get_device_name(dev), sms=sms, reps=args.reps,
                      gemms=rows, total_us=round(total, 2), dw_us=round(dw, 2),
-                     dwt_us=round(dwt, 2), tower_fwd=fwd), f, indent=1)
+                     dwt_us=round(dwt, 2), fwd_per_layer_us=round(per_layer, 2),
+                     tower_fwd=fwd), f, indent=1)
 
 
 def time_tower_fwd(dev, g, reps, warmup):
