@@ -11,9 +11,15 @@
 //   * operands that need no arithmetic (A in both layouts, K-major B and its pre-split lo part,
 //     every bf16 B) are copied global -> shared by cp.async 16-byte copies into a ring of 3-4
 //     stages; the 128-byte swizzle of B is applied in the destination address.  bf16 MN-major
-//     B is read by the wgmma through the descriptor's transpose bit.  Only the MN-major TF32 B
-//     of the dW GEMMs (TF32 wgmma reads K-major B only) is staged through registers, where it
-//     is transposed and, for 3xTF32, split;
+//     B is read by the wgmma through the descriptor's transpose bit.  TF32 wgmma reads K-major
+//     B only, so MN-major TF32 B is transposed (and, for 3xTF32, split) in shared memory:
+//       - in the dW GEMMs (A and B MN-major) a producer warpgroup (threads 256..383) owns the
+//         whole ring: it copies A and the raw MN-major B slab of each k block by cp.async,
+//         transposes the slab in place into the swizzled K-major tile(s), and hands the stage
+//         over on an mbarrier; the MMA warpgroups hand it back on another.  Nothing but
+//         fragment loads and wgmma issue is left on the MMA warps;
+//       - with K-major A (the single-pass TF32 forward) the third warpgroup is the epilogue's,
+//         and the MMA warps stage B through registers themselves;
 //   * one wgmma group stays in flight across k blocks (two A fragment register sets);
 //   * the copies for the next tile start before the epilogue of the current one;
 //   * the epilogue: bias / activation, ReLU masks (from an fp32 array or from 1-bit sign
@@ -68,10 +74,12 @@ constexpr int kStagingBytes = BM * kStagingPitch * 4;
 //             MMA threads wait before writing the next one: 384.  Once per tile but a CTA's
 //             last, which nobody would wait for.
 //   kBarEpi:  bar.sync over the 128 epilogue threads, between the row pass and the column sums.
-constexpr int kBarMma = 1, kBarFull = 2, kBarFree = 3, kBarEpi = 4;
+// A producer kernel uses kBarMma the same way, and kBarProd (bar.sync over its 128 producer
+// threads) around the in-place transpose; its stage ring runs on mbarriers (see producer_ring).
+constexpr int kBarMma = 1, kBarFull = 2, kBarFree = 3, kBarEpi = 4, kBarProd = 5;
 // Registers after setmaxnreg: 2 x 128 x 208 + 128 x 88 = 64,512 of the SM's 65,536.  The
 // epilogue's row loop needs 88 without spills: it holds the tile's mask words and running
-// column sums beside the unrolled rows.
+// column sums beside the unrolled rows.  The producer warpgroup runs on the same 88.
 constexpr int kMmaRegs = 208, kEpiRegs = 88;
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_ACT = 1, EPI_MASK_POS = 2, EPI_MASK_BITS = 3 };
@@ -113,7 +121,19 @@ __host__ __device__ constexpr int col_tiles(int gn, bool fold) {
   return (gn - (fold ? folded_cols(gn) : 0) + BN - 1) / BN;
 }
 
-// Bytes of one swizzled B tile (hi or lo): 128 rows, 136 when the kernel folds.
+// The kernels whose stage ring a producer warpgroup runs: the same dW layout.
+template <typename T, bool A_MN, bool B_MN>
+__host__ __device__ constexpr bool has_producer() {
+  return sizeof(T) == 4 && A_MN && B_MN;
+}
+template <typename T, bool A_MN, bool B_MN>
+__host__ __device__ constexpr int block_threads() {
+  return A_MN && !has_producer<T, A_MN, B_MN>() ? kThreads : kThreads + kEpiThreads;
+}
+
+// Bytes of one swizzled B tile (hi or lo): 128 rows, 136 when the kernel folds.  A producer
+// kernel first copies the raw MN-major slab of the same k block into it, 32 k rows of 128
+// columns then 32 k rows of the kFoldMax folded ones: the same byte count.
 __host__ __device__ constexpr int b_tile_bytes(bool fold) {
   return fold ? kTileBytes + kFoldMax * 128 : kTileBytes;
 }
@@ -121,25 +141,32 @@ __host__ __device__ constexpr int b_tile_bytes(bool fold) {
 __host__ __device__ constexpr int stage_bytes(int passes, bool fold = false) {
   return (passes == 3 ? 2 : 1) * b_tile_bytes(fold) + kATileBytes;
 }
+// A producer ring's full and empty mbarriers, kMaxStages of each.
+constexpr int kRingBarBytes = 2 * kMaxStages * 8;
 // What follows the stages: the staging tile of a staged kernel (its column sums live in
-// global memory), else the [8][colsum_cols] column-sum accumulator.
-__host__ __device__ constexpr int tail_bytes(int colsum_cols, bool staged) {
-  return staged ? kStagingBytes : kWarps * colsum_cols * 4;
+// global memory), else the [8][colsum_cols] column-sum accumulator and, with a producer, the
+// ring's mbarriers.
+__host__ __device__ constexpr int tail_bytes(int colsum_cols, bool staged, bool prod = false) {
+  return staged ? kStagingBytes : kWarps * colsum_cols * 4 + (prod ? kRingBarBytes : 0);
 }
 // Stages that fit beside the tail and the 1 KB alignment slack; at most kMaxStages.  The one
 // place that sizes the shared memory of a launch.
-__host__ __device__ constexpr int num_stages(int passes, int colsum_cols, bool staged, bool fold = false) {
-  return (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes, fold) < kMaxStages
-             ? (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged)) / stage_bytes(passes, fold)
+__host__ __device__ constexpr int num_stages(int passes, int colsum_cols, bool staged, bool fold = false,
+                                             bool prod = false) {
+  return (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged, prod)) / stage_bytes(passes, fold) < kMaxStages
+             ? (kSmemLimit - 1024 - tail_bytes(colsum_cols, staged, prod)) / stage_bytes(passes, fold)
              : kMaxStages;
 }
 static_assert(num_stages(3, 1024, false, true) >= 3, "3xTF32 needs three stages beside a 1024-column colsum");
-static_assert(num_stages(3, 0, false, true) == kMaxStages, "the 3xTF32 dW GEMMs keep four stages");
+static_assert(num_stages(3, 0, false, true, true) == kMaxStages, "the 3xTF32 dW GEMMs keep four stages");
+static_assert(num_stages(1, 0, false, true, true) == kMaxStages, "the TF32 dW GEMMs keep four stages");
 static_assert(num_stages(3, 1024, true) >= 3, "3xTF32 needs three stages beside the staging tile");
-inline size_t smem_bytes(int passes, int colsum_cols, bool staged, bool fold) {
-  return (size_t)num_stages(passes, colsum_cols, staged, fold) * stage_bytes(passes, fold) +
-         (size_t)tail_bytes(colsum_cols, staged) + 1024;
+inline size_t smem_bytes(int passes, int colsum_cols, bool staged, bool fold, bool prod = false) {
+  return (size_t)num_stages(passes, colsum_cols, staged, fold, prod) * stage_bytes(passes, fold) +
+         (size_t)tail_bytes(colsum_cols, staged, prod) + 1024;
 }
+static_assert(kMaxStages * stage_bytes(3, true) + kRingBarBytes + 1024 <= kSmemLimit,
+              "a 3xTF32 dW ring of four folding stages fits in shared memory");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -205,6 +232,23 @@ __device__ __forceinline__ void bar_sync(int id, int threads) {
 }
 __device__ __forceinline__ void bar_arrive(int id, int threads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void mbar_init(uint64_t* b, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
+  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(b))
+               : "memory");
+}
+// Returns once the phase of parity `parity` has completed.  On a fresh barrier the phase
+// before the first (parity 1) counts as completed.
+__device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WAIT;\n\t}" ::"r"(smem_u32(b)), "r"(parity)
+      : "memory");
 }
 // Every warp of a warpgroup executes these.
 template <int R>
@@ -287,14 +331,90 @@ template <> struct Elem<__nv_bfloat16> { static constexpr int EPC = 8; static co
 // Byte offset of 16-byte chunk `kc` of row `row` in a K-major 128B-swizzled tile.
 __device__ __forceinline__ int swz_chunk(int row, int kc) { return row * 128 + (((kc ^ row) & 7) << 4); }
 
-// The register-staged operand: an MN-major fp32 B tile ([k][n], n contiguous) of 128 columns
-// x 32 k, transposed into the K-major swizzled tile(s) and, for 3xTF32, split into hi / lo.
-// A warp takes 8 consecutive column chunks (one 128-byte line per k row) of 4 consecutive k
-// rows, so all 32 lanes of a scalar K-major store write the same 16-byte k chunk position of
-// their rows and differ only in the row's swizzle phase (row mod 8) and in k mod 4.  Store
-// step j of a lane writes column r + ((j + s) & 3) of its chunk, s = (lane mod 8) / 2: the 8
-// lanes of a k row then write rows of 8 different phases, and the 32 lanes hit 32 different
-// banks.  (With s = 0 they would write rows of 2 phases: 4 ways of bank conflict.)
+// Stores columns r .. r + 3 of k row k of an MN-major fp32 B slab at their K-major places in
+// the swizzled tile(s) and, for 3xTF32 (SPLIT), split into hi / lo.  The caller gives a warp 8
+// consecutive column chunks (one 128-byte line per k row) of 4 consecutive k rows, so all 32
+// lanes of a scalar K-major store write the same 16-byte k chunk position of their rows and
+// differ only in the row's swizzle phase (row mod 8) and in k mod 4.  Store step j of a lane
+// writes column r + ((j + s) & 3) of its chunk, s = (lane mod 8) / 2: the 8 lanes of a k row
+// then write rows of 8 different phases, and the 32 lanes hit 32 different banks.  (With
+// s = 0 they would write rows of 2 phases: 4 ways of bank conflict.)
+template <bool SPLIT>
+__device__ __forceinline__ void store_mn_chunk(unsigned char* hi, unsigned char* lo, float4 v, int k, int r) {
+  const int s = (threadIdx.x & 7) >> 1;
+  // rotate the chunk left by s with selects (a dynamic index would go to local memory)
+  float e0 = v.x, e1 = v.y, e2 = v.z, e3 = v.w;
+  if (s & 1) {
+    const float t = e0;
+    e0 = e1; e1 = e2; e2 = e3; e3 = t;
+  }
+  if (s & 2) {
+    float t = e0; e0 = e2; e2 = t;
+    t = e1; e1 = e3; e3 = t;
+  }
+  const float e[4] = {e0, e1, e2, e3};   // e[j]: column r + ((j + s) & 3)
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int off = swz_chunk(r + ((j + s) & 3), k >> 2) + (k & 3) * 4;
+    if (SPLIT) {
+      const float h = tf32_rn(e[j]);
+      *reinterpret_cast<float*>(hi + off) = h;
+      *reinterpret_cast<float*>(lo + off) = e[j] - h;
+    } else {
+      *reinterpret_cast<float*>(hi + off) = e[j];
+    }
+  }
+}
+// Stores a 4 x 4 block of an MN-major fp32 B slab, v[i] = columns r .. r + 3 of k row 4 kc + i,
+// at its K-major places: per column one 16-byte store of its 4 k (split into hi / lo for
+// 3xTF32).  Store step j of a lane writes column r + ((j + s) & 3), s = (lane mod 8) / 2, as
+// in store_mn_chunk: when the 8 lanes of a quarter warp hold 8 consecutive 4-column groups of
+// the same kc, they write rows of 8 different swizzle phases, all 32 banks once.
+template <bool SPLIT>
+__device__ __forceinline__ void store_mn_block(unsigned char* hi, unsigned char* lo, const float4 (&v)[4],
+                                               int kc, int r) {
+  const int s = (threadIdx.x & 7) >> 1;
+  float4 c0 = make_float4(v[0].x, v[1].x, v[2].x, v[3].x), c1 = make_float4(v[0].y, v[1].y, v[2].y, v[3].y);
+  float4 c2 = make_float4(v[0].z, v[1].z, v[2].z, v[3].z), c3 = make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
+  if (s & 1) {   // rotate the columns left by s with selects
+    const float4 t = c0;
+    c0 = c1; c1 = c2; c2 = c3; c3 = t;
+  }
+  if (s & 2) {
+    float4 t = c0; c0 = c2; c2 = t;
+    t = c1; c1 = c3; c3 = t;
+  }
+  const float4 c[4] = {c0, c1, c2, c3};   // c[j]: column r + ((j + s) & 3)
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int off = swz_chunk(r + ((j + s) & 3), kc);
+    if (SPLIT) {
+      const float4 h = make_float4(tf32_rn(c[j].x), tf32_rn(c[j].y), tf32_rn(c[j].z), tf32_rn(c[j].w));
+      *reinterpret_cast<float4*>(hi + off) = h;
+      *reinterpret_cast<float4*>(lo + off) = make_float4(c[j].x - h.x, c[j].y - h.y, c[j].z - h.z, c[j].w - h.w);
+    } else {
+      *reinterpret_cast<float4*>(hi + off) = c[j];
+    }
+  }
+}
+// Stores element (k, folded column c) of an MN-major slab at K-major row BN + c.  The 32
+// lanes of a warp store 4 k of one 16-byte chunk position into 8 rows of 8 different swizzle
+// phases: 32 different banks.
+template <bool SPLIT>
+__device__ __forceinline__ void store_mn_tail(unsigned char* hi, unsigned char* lo, float v, int k, int c) {
+  const int off = swz_chunk(BN + c, k >> 2) + (k & 3) * 4;
+  if (SPLIT) {
+    const float h = tf32_rn(v);
+    *reinterpret_cast<float*>(hi + off) = h;
+    *reinterpret_cast<float*>(lo + off) = v - h;
+  } else {
+    *reinterpret_cast<float*>(hi + off) = v;
+  }
+}
+
+// The register-staged operand of the K-major-A kernel: an MN-major fp32 B tile ([k][n], n
+// contiguous) of 128 columns x 32 k, loaded by the 256 MMA threads, transposed into the K-major
+// swizzled tile(s) by store_mn_chunk and, for 3xTF32, split into hi / lo.
 struct BTileMN {
   float4 v[4];
   __device__ __forceinline__ static void chunk(int i, int& k, int& r) {
@@ -321,60 +441,160 @@ struct BTileMN {
   }
   template <bool SPLIT>
   __device__ __forceinline__ void store(unsigned char* hi, unsigned char* lo) const {
-    const int s = (threadIdx.x & 7) >> 1;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       int k, r;
       chunk(i, k, r);
-      // rotate the chunk left by s with selects (a dynamic index would go to local memory)
-      float e0 = v[i].x, e1 = v[i].y, e2 = v[i].z, e3 = v[i].w;
-      if (s & 1) {
-        const float t = e0;
-        e0 = e1; e1 = e2; e2 = e3; e3 = t;
-      }
-      if (s & 2) {
-        float t = e0; e0 = e2; e2 = t;
-        t = e1; e1 = e3; e3 = t;
-      }
-      const float e[4] = {e0, e1, e2, e3};   // e[j]: column r + ((j + s) & 3)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int off = swz_chunk(r + ((j + s) & 3), k >> 2) + (k & 3) * 4;
-        if (SPLIT) {
-          const float h = tf32_rn(e[j]);
-          *reinterpret_cast<float*>(hi + off) = h;
-          *reinterpret_cast<float*>(lo + off) = e[j] - h;
-        } else {
-          *reinterpret_cast<float*>(hi + off) = e[j];
-        }
-      }
+      store_mn_chunk<SPLIT>(hi, lo, v[i], k, r);
     }
   }
 };
 
-// The folded remainder of a register-staged B tile: tile columns 128..135 x 32 k, one element
-// per thread (k = tid / 8, column tid % 8), stored at K-major rows 128..135; columns past
-// `cols` are zero.  The 32 lanes of a warp write 4 k of one 16-byte chunk position into 8 rows
-// of 8 different swizzle phases: 32 different banks.
-struct BTailMN {
-  float v;
-  __device__ __forceinline__ void load(const float* base, int ld, int c0, int cols, int k0, int ks) {
-    const int k = threadIdx.x >> 3, c = threadIdx.x & 7;
-    v = (c < cols && k0 + k < ks) ? __ldg(base + static_cast<size_t>(k0 + k) * ld + c0 + c) : 0.f;
-  }
-  template <bool SPLIT>
-  __device__ __forceinline__ void store(unsigned char* hi, unsigned char* lo) const {
-    const int k = threadIdx.x >> 3, c = threadIdx.x & 7;
-    const int off = swz_chunk(BN + c, k >> 2) + (k & 3) * 4;
-    if (SPLIT) {
-      const float h = tf32_rn(v);
-      *reinterpret_cast<float*>(hi + off) = h;
-      *reinterpret_cast<float*>(lo + off) = v - h;
+// The producer warpgroup of a dW kernel (TF32, A and B MN-major): it runs the stage ring of the
+// two MMA warpgroups.  It walks the CTA's (tile, k block) sequence as they do, across tiles,
+// block g in stage g mod stages, and per block
+//   issues:   once the MMA warps have released the stage (empty[s]), the cp.async copies of the
+//             block's A tile (MN-major, padded) and of its raw MN-major B slab into the stage's
+//             B tile (the pre-split lo slab into the lo tile): 128 columns, then the folded
+//             remainder's 8 (zero on a tile without it, whose m64n136 reads them too).  One
+//             cp.async group per block;
+//   finishes it, depth = stages - 2 blocks later and before it waits to issue the next one:
+//             once the block's group has landed, each thread reads two 4 x 4 blocks (4 k rows
+//             of 4 columns) and 2 folded elements of the slab, and after a barrier over the
+//             producer threads writes them back transposed into the swizzled K-major tile, one
+//             16-byte store per column of a block, split for 3xTF32 (hi = tf32_rn(x),
+//             lo = x - hi, as the A split); then it fences the writes to the async proxy and
+//             arrives at full[s].
+// The MMA warps hold only the stage whose group they issue and the one of the group still in
+// flight before it, so with 4 stages a block's copies have two blocks' time to land.  Block b of
+// a thread covers k chunk slot / 4 and column group 8 (slot % 4) + lane % 8, slot = 4 warp +
+// lane / 8 + 16 b: a quarter warp reads 128 contiguous bytes of a k row, and stores rows of 8
+// different swizzle phases (store_mn_block).
+template <bool P3, bool PRE_B, bool FOLD>
+__device__ __forceinline__ void producer_ring(const Args& args, unsigned char* smem, int stages,
+                                              uint64_t* full, uint64_t* empty) {
+  constexpr int kBTile = b_tile_bytes(FOLD);
+  constexpr int kStage = stage_bytes(P3 ? 3 : 1, FOLD);
+  constexpr int kAOff = (P3 ? 2 : 1) * kBTile;
+  constexpr int kSlabPitch = BN * 4;   // bytes per k row of the raw slab
+  const int pt = threadIdx.x - kThreads, lane = pt & 31, pw = pt >> 5;
+  const float* A = static_cast<const float*>(args.A);
+  const float* B = static_cast<const float*>(args.B);
+  const float* Blo = static_cast<const float*>(args.B_lo);
+  const int nkb_total = (args.GK + Elem<float>::BK - 1) / Elem<float>::BK;
+  const int tiles_mn = args.m_tiles * args.n_tiles;
+  const int total = tiles_mn * args.splits;
+  const int fold = FOLD ? folded_cols(args.GN) : 0;
+  const uint32_t smem_base = smem_u32(smem);
+
+  // raw slab of k rows k0 .. k0 + 31: columns n0 .. n0 + 127, then `tail` folded ones
+  auto copy_slab = [&](const float* src, uint32_t dst, int n0, int k0, int tail) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int c = pt + i * kEpiThreads;
+      const int k = c >> 5, nc = c & 31, n = n0 + nc * 4;
+      const int cnt = k0 + k < args.GK ? min(max(args.GN - n, 0), 4) : 0;
+      const float* p = cnt > 0 ? src + static_cast<size_t>(k0 + k) * args.ldb + n : src;
+      cp_async16(dst + k * kSlabPitch + nc * 16, p, cnt * 4);
+    }
+    if (FOLD && pt < 64) {   // [32 k][8 columns], two chunks per k row
+      const int k = pt >> 1, h = pt & 1;
+      const int cnt = k0 + k < args.GK ? min(max(tail - 4 * h, 0), 4) : 0;
+      const float* p = cnt > 0 ? src + static_cast<size_t>(k0 + k) * args.ldb + n0 + BN + 4 * h : src;
+      cp_async16(dst + kTileBytes + k * 32 + h * 16, p, cnt * 4);
+    }
+  };
+  // the slab in tile `t`, transposed in place (and split into t, lo)
+  auto transpose = [&](unsigned char* t, unsigned char* lo, auto split) {
+    constexpr bool SPLIT = decltype(split)::value;
+    // opaque per call: keeps ptxas from holding every store offset in registers across blocks
+    int qw = pw * 4 + (lane >> 3), q = pt;
+    asm volatile("" : "+r"(qw), "+r"(q));
+    float4 v[2][4];
+    float tv[2];
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      const int slot = qw + 16 * b, kc = slot >> 2, r = 4 * (8 * (slot & 3) + (lane & 7));
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        v[b][i] = *reinterpret_cast<const float4*>(t + (4 * kc + i) * kSlabPitch + r * 4);
+    }
+    if (FOLD) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        tv[e] = *reinterpret_cast<const float*>(t + kTileBytes + ((q >> 3) + 16 * e) * 32 + (q & 7) * 4);
+    }
+    bar_sync(kBarProd, kEpiThreads);   // the whole slab is read before any of it is overwritten
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      const int slot = qw + 16 * b;
+      store_mn_block<SPLIT>(t, lo, v[b], slot >> 2, 4 * (8 * (slot & 3) + (lane & 7)));
+    }
+    if (FOLD) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) store_mn_tail<SPLIT>(t, lo, tv[e], (q >> 3) + 16 * e, q & 7);
+    }
+  };
+  // `younger`: cp.async groups committed after the block's own, which may still be pending
+  auto finish = [&](int s, int younger) {
+    if (younger > 0) cp_async_wait<1>();
+    else cp_async_wait<0>();
+    bar_sync(kBarProd, kEpiThreads);   // the copies of every producer thread have landed
+    unsigned char* sb = smem + s * kStage;
+    if (PRE_B) {
+      transpose(sb, nullptr, std::false_type{});
+      transpose(sb + kBTile, nullptr, std::false_type{});
     } else {
-      *reinterpret_cast<float*>(hi + off) = v;
+      transpose(sb, sb + kBTile, std::integral_constant<bool, P3>{});
+    }
+    fence_proxy_async();   // st.shared writes -> visible to the tensor cores
+    __syncwarp();
+    if (lane == 0) mbar_arrive(full + s);   // one arrival per producer warp
+  };
+
+  const int depth = stages - 2;
+  int is = 0, fs = 0, pending = 0;   // stage of the next block to issue / to finish
+  uint32_t eph = 1;                  // parity of the empty phase the issue waits for
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const int z = tile / tiles_mn;
+    const int rt = tile - z * tiles_mn;
+    const int m0 = (rt / args.n_tiles) * BM, n0 = (rt % args.n_tiles) * BN;
+    const int kb0 = z * args.kb_per_split;
+    const int nkb = max(min(nkb_total, kb0 + args.kb_per_split) - kb0, 0);
+    const int tail = FOLD && n0 + BN + fold == args.GN ? fold : 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+      // the oldest block first: its transpose does not wait for a stage to come free
+      if (pending == depth) {
+        finish(fs, depth - 1);
+        fs = fs + 1 == stages ? 0 : fs + 1;
+        --pending;
+      }
+      mbar_wait(empty + is, eph);
+      const uint32_t st = smem_base + is * kStage;
+      const int k0 = (kb0 + kb) * Elem<float>::BK;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {   // A: [32 k rows][32 chunks of m]
+        const int c = pt + i * kEpiThreads;
+        const int k = c >> 5, mc = c & 31, m = m0 + mc * 4;
+        const int cnt = (k0 + k < args.GK && m < args.GM) ? min(4, args.GM - m) : 0;
+        const float* p = cnt > 0 ? A + static_cast<size_t>(k0 + k) * args.lda + m : A;
+        cp_async16(st + kAOff + k * kAPitchMN + mc * 16, p, cnt * 4);
+      }
+      copy_slab(B, st, n0, k0, tail);
+      if (PRE_B) copy_slab(Blo, st + kBTile, n0, k0, tail);
+      cp_async_commit();
+      if (++is == stages) {
+        is = 0;
+        eph ^= 1u;
+      }
+      ++pending;
     }
   }
-};
+  for (; pending > 0; --pending) {
+    finish(fs, pending - 1);
+    fs = fs + 1 == stages ? 0 : fs + 1;
+  }
+}
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   uint32_t r;
@@ -625,16 +845,17 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
 // [8][colsum_cols] floats.  FOLD (launched when GN has a remainder to fold): the last column
 // tile owns it, B tiles have 136 rows and wide tiles issue m64n136.
 template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16, bool FOLD>
-__global__ void __launch_bounds__(A_MN ? kThreads : kThreads + kEpiThreads, 1)
+__global__ void __launch_bounds__(block_threads<T, A_MN, B_MN>(), 1)
 gemm_kernel(const Args args) {
   constexpr bool STAGED = !A_MN;
+  constexpr bool PROD = has_producer<T, A_MN, B_MN>();   // a producer warpgroup runs the ring
   constexpr bool F32 = sizeof(T) == 4;
   constexpr int EPC = Elem<T>::EPC;
   constexpr int BK = Elem<T>::BK;
   constexpr int KSTEP = F32 ? 8 : 16;   // k of one wgmma
   constexpr int NKS = BK / KSTEP;
   constexpr bool P3 = PASSES == 3;
-  constexpr bool REG_B = F32 && B_MN;   // TF32 MN-major B: transposed through registers
+  constexpr bool REG_B = F32 && B_MN && !PROD;   // TF32 MN-major B through the MMA warps' registers
   constexpr int kBTile = b_tile_bytes(FOLD);   // offset of the B lo tile
   constexpr int kStage = stage_bytes(PASSES, FOLD);
   constexpr int kAOff = (P3 ? 2 : 1) * kBTile;
@@ -644,18 +865,31 @@ gemm_kernel(const Args args) {
   static_assert(!FOLD || folds<T, A_MN, B_MN>(), "only TF32 with A and B MN-major folds");
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int stages = num_stages(PASSES, args.colsum_cols, STAGED, FOLD);
+  const int stages = num_stages(PASSES, args.colsum_cols, STAGED, FOLD, PROD);
   float* cacc = reinterpret_cast<float*>(smem + stages * kStage);   // staged: the staging tile
-  if (STAGED) {
+  // producer ring: full[s] (one arrival per producer warp) and empty[s] (one per MMA warp)
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + stages * kStage + kWarps * args.colsum_cols * 4);
+  uint64_t* empty = full + kMaxStages;
+  if (STAGED || PROD) {
+    if (PROD) {
+      if (threadIdx.x == 0) {
+        for (int i = 0; i < stages; ++i) {
+          mbar_init(full + i, kEpiThreads / 32);
+          mbar_init(empty + i, kWarps);
+        }
+      }
+      __syncthreads();
+    }
     if (threadIdx.x >= kThreads) {
       setmaxnreg_dec<kEpiRegs>();
-      epilogue_warpgroup<OUT_BF16>(args, cacc);
+      if constexpr (PROD) producer_ring<P3, PRE_B, FOLD>(args, smem, stages, full, empty);
+      else epilogue_warpgroup<OUT_BF16>(args, cacc);
       return;
     }
     setmaxnreg_inc<kMmaRegs>();
   }
   auto mma_sync = [] {   // barrier over the MMA warpgroups
-    if (STAGED) bar_sync(kBarMma, kThreads);
+    if (STAGED || PROD) bar_sync(kBarMma, kThreads);
     else __syncthreads();
   };
 
@@ -720,18 +954,14 @@ gemm_kernel(const Args args) {
   // cp.async groups: a tile's prologue commits stages - 2 groups (blocks 0 .. stages - 3),
   // every k block one more (block kb + stages - 2), empty ones included, so that block kb's
   // group is complete once at most stages - 3 younger groups are pending.
+  // A producer kernel's MMA warps copy nothing: the producer warpgroup runs the ring.
   BTileMN tb, tbl;
-  BTailMN tt, ttl;   // the folded remainder (hi / pre-split lo)
   auto load_b = [&](int n0, int kb) {
     tb.load(reinterpret_cast<const float*>(B), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
     if (PRE_B) tbl.load(reinterpret_cast<const float*>(Blo), args.ldb, n0, args.GN - n0, kb * BK, args.GK);
-    if (FOLD) {   // zeros for a tile without the remainder: its m64n136 reads them too
-      const int cols = has_tail(n0) ? fold : 0;
-      tt.load(reinterpret_cast<const float*>(B), args.ldb, n0 + BN, cols, kb * BK, args.GK);
-      if (PRE_B) ttl.load(reinterpret_cast<const float*>(Blo), args.ldb, n0 + BN, cols, kb * BK, args.GK);
-    }
   };
   auto prologue = [&](int tile) {
+    if (PROD) return;
     const int z = tile / tiles_mn;
     const int r = tile - z * tiles_mn;
     const int m0 = (r / args.n_tiles) * BM, n0 = (r % args.n_tiles) * BN;
@@ -745,6 +975,10 @@ gemm_kernel(const Args args) {
   };
 
   if (blockIdx.x < total) prologue(blockIdx.x);
+  // stage of block kb and, with a producer, the parity of its full phase: a producer ring
+  // runs on across tiles
+  int s = 0;
+  uint32_t fph = 0;
   for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
     const int z = tile / tiles_mn;
     const int r = tile - z * tiles_mn;
@@ -769,50 +1003,50 @@ gemm_kernel(const Args args) {
     // that barrier goes to the stage of block kb - 2 and loads block kb + stages - 2 (copies
     // run stages - 2 blocks ahead), and the stage of block kb, last read by group
     // kb - stages <= kb - 3, may be written before the barrier.
+    // With a producer the ring runs on the stage barriers instead: block kb waits for full[s]
+    // and, once `wait_group 1` has retired group kb - 1, releases that group's stage at
+    // empty[s - 1]; each MMA warp arrives for itself (wait_group is warp-wide), so neither
+    // warpgroup waits for the other.
     uint32_t frag_hi[2][NKS][4], frag_lo[2][NKS][4];
-    int s = 0;   // stage of block kb
+    if (!PROD) s = 0;
     auto kblock = [&](int kb, auto set) {
       constexpr int F = decltype(set)::value;   // fragment set: compile-time, stays in registers
       const uint32_t st = smem_base + s * kStage;
-      if (REG_B) {
-        unsigned char* sb = smem + s * kStage;
-        if (PRE_B) {
-          tb.template store<false>(sb, nullptr);
-          tbl.template store<false>(sb + kBTile, nullptr);
-        } else {
-          tb.template store<P3>(sb, sb + kBTile);
-        }
-        if (FOLD) {
+      if (PROD) {
+        mbar_wait(full + s, fph);   // the producer fenced its stores before it arrived
+      } else {
+        if (REG_B) {
+          unsigned char* sb = smem + s * kStage;
           if (PRE_B) {
-            tt.template store<false>(sb, nullptr);
-            ttl.template store<false>(sb + kBTile, nullptr);
+            tb.template store<false>(sb, nullptr);
+            tbl.template store<false>(sb + kBTile, nullptr);
           } else {
-            tt.template store<P3>(sb, sb + kBTile);
+            tb.template store<P3>(sb, sb + kBTile);
           }
         }
-      }
-      if (stages == 4) cp_async_wait<1>(); else cp_async_wait<0>();
-      if (P3 && !B_MN && !PRE_B) {   // K-major B split on the fly: each thread its own chunks
-        unsigned char* sb = smem + s * kStage;
+        if (stages == 4) cp_async_wait<1>(); else cp_async_wait<0>();
+        if (P3 && !B_MN && !PRE_B) {   // K-major B split on the fly: each thread its own chunks
+          unsigned char* sb = smem + s * kStage;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int c = threadIdx.x + i * kThreads;
-          const int off = swz_chunk(c >> 3, c & 7);
-          const float4 x = *reinterpret_cast<const float4*>(sb + off);
-          const float4 h = make_float4(tf32_rn(x.x), tf32_rn(x.y), tf32_rn(x.z), tf32_rn(x.w));
-          *reinterpret_cast<float4*>(sb + off) = h;
-          *reinterpret_cast<float4*>(sb + kBTile + off) =
-              make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+          for (int i = 0; i < 4; ++i) {
+            const int c = threadIdx.x + i * kThreads;
+            const int off = swz_chunk(c >> 3, c & 7);
+            const float4 x = *reinterpret_cast<const float4*>(sb + off);
+            const float4 h = make_float4(tf32_rn(x.x), tf32_rn(x.y), tf32_rn(x.z), tf32_rn(x.w));
+            *reinterpret_cast<float4*>(sb + off) = h;
+            *reinterpret_cast<float4*>(sb + kBTile + off) =
+                make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+          }
         }
+        fence_proxy_async();   // cp.async and st.shared writes -> visible to the tensor cores
+        mma_sync();
+        {
+          const int nb = kb + stages - 2;
+          if (nb < nkb) copy_block(m0, n0, kb0, nb, s >= 2 ? s - 2 : s + stages - 2);
+          cp_async_commit();
+        }
+        if (REG_B && kb + 1 < nkb) load_b(n0, kb0 + kb + 1);   // in flight while the tensor cores run
       }
-      fence_proxy_async();   // cp.async and st.shared writes -> visible to the tensor cores
-      mma_sync();
-      {
-        const int nb = kb + stages - 2;
-        if (nb < nkb) copy_block(m0, n0, kb0, nb, s >= 2 ? s - 2 : s + stages - 2);
-        cp_async_commit();
-      }
-      if (REG_B && kb + 1 < nkb) load_b(n0, kb0 + kb + 1);   // in flight while the tensor cores run
       {
         // a K tail that is no multiple of BK is zero-filled: skip its all-zero k steps
         const int krem = args.GK - (kb0 + kb) * BK;
@@ -916,16 +1150,24 @@ gemm_kernel(const Args args) {
         else by_width(std::integral_constant<int, 1>{});
         wgmma_wait<1>();   // retires group kb - 1; group kb stays in flight
       }
-      s = s + 1 == stages ? 0 : s + 1;
+      if (PROD && kb > 0 && lane == 0) mbar_arrive(empty + (s == 0 ? stages - 1 : s - 1));
+      if (++s == stages) {
+        s = 0;
+        fph ^= 1u;
+      }
     };
     for (int kb = 0; kb < nkb; kb += 2) {   // unrolled by two: the fragment set is a constant
       kblock(kb, std::integral_constant<int, 0>{});
       if (kb + 1 < nkb) kblock(kb + 1, std::integral_constant<int, 1>{});
     }
     wgmma_wait<0>();
-    // every warpgroup is done with the stages: start the next tile's copies, then the epilogue
-    mma_sync();
-    if (tile + gridDim.x < total) prologue(tile + gridDim.x);
+    if (PROD) {   // the tile's last stage; the producer is already filling the next tile's
+      if (nkb > 0 && lane == 0) mbar_arrive(empty + (s == 0 ? stages - 1 : s - 1));
+    } else {
+      // every warpgroup is done with the stages: start the next tile's copies, then the epilogue
+      mma_sync();
+      if (tile + gridDim.x < total) prologue(tile + gridDim.x);
+    }
 
     // accumulator element j of half h: row = 16 wq + lane / 4 + 8 ((j / 2) % 2),
     // column = 64 h + 8 (j / 4) + 2 (lane % 4) + j % 2
@@ -1094,10 +1336,10 @@ int launch_grid(Args a, cudaStream_t st, int* ctas) {
   const int sms = num_sms();
   const int grid = total < sms ? total : sms;
   if (ctas) *ctas = grid;
-  const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN, FOLD);
+  const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN, FOLD, has_producer<T, A_MN, B_MN>());
   auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, FOLD>;
   TFR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, A_MN ? kThreads : kThreads + kEpiThreads, smem, st>>>(a);
+  kern<<<grid, block_threads<T, A_MN, B_MN>(), smem, st>>>(a);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }
