@@ -435,12 +435,36 @@ int tfr_mlp_bwd(const void* X, int M, const tfr_mlp_cfg* cfg,
 /* Gradient of the tower's loss with respect to its input columns [col0, col0 + ncols):
  *   dX[m, c] (row pitch ldx) = sum_o dZ_0[m, o] W_0[col0 + c, o]
  * where dZ_0 is the gradient at the first Dense layer's pre-activation that the preceding
- * tfr_mlp_bwd (same cfg, M, params, workspace) left in the workspace.  Needs at least one
- * hidden layer, precision TFR_PREC_TF32X3 or TFR_PREC_TF32 and no input BatchNormalization
+ * tfr_mlp_bwd or tfr_mlp_bwd_tasks (same cfg, M, params, workspace) left in the workspace.
+ * Needs at least one hidden layer, precision TFR_PREC_TF32X3 or TFR_PREC_TF32 and no input BatchNormalization
  * (TFR_INVALID_ARGUMENT otherwise, before any CUDA call).  Does not change the workspace, so
  * tfr_mlp_bwd's results are the same with or without this call. */
 int tfr_mlp_input_grad(const tfr_mlp_cfg* cfg, int M, const float* params, void* workspace,
                        int col0, int ncols, float* dX, int ldx, int precision, void* stream);
+
+/* Multi-task scoring: one tower whose O = dims[n_dense] output units are O ranking tasks, in
+ * a task-major ("planar") score layout that the per-list loss kernels read directly.
+ *   score_planes [O, M]: score_planes[o * M + m] is row m's score for task o, so plane o is
+ *   task o's [B, N] score matrix.  Unmasked values are bit-identical to tfr_mlp_fwd's
+ *   scores_out[m * O + o]; if mask (uint8 [M]) is given, masked rows of EVERY plane are set to
+ *   ln(1e-10) (RestoreList per task).
+ * precision: TFR_PREC_FP32, TFR_PREC_TF32X3 or TFR_PREC_TF32.  1 <= O <= 8.  Anything else, and
+ * NULL X / params / workspace / score_planes, is TFR_INVALID_ARGUMENT before any CUDA call.
+ * The workspace is tfr_mlp_workspace_bytes(cfg, M), as for tfr_mlp_fwd. */
+int tfr_mlp_fwd_tasks(const void* X, int M, const tfr_mlp_cfg* cfg, const float* params,
+                      const uint8_t* mask, void* workspace, float* score_planes,
+                      int precision, void* stream);
+
+/* Backward of tfr_mlp_fwd_tasks (same X / workspace): the gradients tfr_mlp_bwd produces from
+ * the interleaved signal dS[m, o] = w_o * dscore_planes[o * M + m], with rows the mask clears
+ * set to 0 for every task.  task_weights_host: O host floats (the per-task loss weights), NULL
+ * for all 1.  Same limits as tfr_mlp_fwd_tasks, plus dscore_planes / grads not NULL and every
+ * weight finite (TFR_INVALID_ARGUMENT before any CUDA call).  tfr_mlp_input_grad may follow.
+ * With O = 1, weight 1, the results are tfr_mlp_bwd's bits. */
+int tfr_mlp_bwd_tasks(const void* X, int M, const tfr_mlp_cfg* cfg, const float* params,
+                      const float* dscore_planes, const float* task_weights_host,
+                      const uint8_t* mask, void* workspace, float* grads,
+                      int precision, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K11  DocumentInteractionAttention (keras/layers.py:420-588): listwise self-attention over

@@ -155,6 +155,8 @@ _SIGNATURES = {
     'tfr_mlp_workspace_bytes': (C.c_size_t, [C.POINTER(MlpCfg), _I]),
     'tfr_mlp_fwd': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _I, _P]),
     'tfr_mlp_bwd': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _P, _I, _P]),
+    'tfr_mlp_fwd_tasks': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _I, _P]),
+    'tfr_mlp_bwd_tasks': (_I, [_P, _I, C.POINTER(MlpCfg), _P, _P, _P, _P, _P, _P, _I, _P]),
     'tfr_mlp_input_grad': (_I, [C.POINTER(MlpCfg), _I, _P, _P, _I, _I, _P, _I, _I, _P]),
     'tfr_din_param_count': (C.c_size_t, [C.POINTER(DinCfg)]),
     'tfr_din_workspace_bytes': (C.c_size_t, [C.POINTER(DinCfg), _I, _I]),

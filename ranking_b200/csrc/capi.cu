@@ -1,5 +1,6 @@
 // C-ABI glue: error string, scorer-tower dispatch, fused optimizer.
 #include <atomic>
+#include <cmath>
 #include <cstring>
 
 #include "common.cuh"
@@ -290,6 +291,73 @@ extern "C" int tfr_mlp_bwd(const void* Xv, int M, const tfr_mlp_cfg* cfg,
       set_error("precision %d is not available in this build", precision);
       return TFR_UNSUPPORTED;
   }
+}
+
+// Limits of the task-major entry points, checked before any CUDA call (make_mlp_plan asks the
+// device for its SM count).
+static int check_tasks_args(const tfr_mlp_cfg* cfg, int precision) {
+  TFR_REQUIRE(cfg != nullptr, "cfg must not be NULL");
+  TFR_REQUIRE(cfg->n_dense >= 1 && cfg->n_dense <= TFR_MLP_MAX_LAYERS,
+              "n_dense %d must be in [1, %d]", cfg->n_dense, TFR_MLP_MAX_LAYERS);
+  const int O = cfg->dims[cfg->n_dense];
+  TFR_REQUIRE(O >= 1 && O <= 8, "task count (output_units) %d must be in [1, 8]", O);
+  TFR_REQUIRE(precision == TFR_PREC_FP32 || precision == TFR_PREC_TF32X3 ||
+                  precision == TFR_PREC_TF32,
+              "task-major scores need precision fp32, tf32x3 or tf32 (got %d)", precision);
+  return TFR_OK;
+}
+
+extern "C" int tfr_mlp_fwd_tasks(const void* Xv, int M, const tfr_mlp_cfg* cfg,
+                                 const float* params, const uint8_t* mask, void* workspace,
+                                 float* score_planes, int precision, void* stream) {
+  int rc = check_tasks_args(cfg, precision);
+  if (rc) return rc;
+  const float* X = static_cast<const float*>(Xv);
+  TFR_REQUIRE(X && params && workspace && score_planes, "NULL argument");
+  MlpPlan p;
+  rc = make_mlp_plan(cfg, M, &p);
+  if (rc) return rc;
+  TFR_REQUIRE(!(p.use_bn || p.input_bn) || p.bn_state, "cfg->bn_state must be set with BN");
+  if (M == 0) return TFR_OK;
+  if (precision == TFR_PREC_FP32)
+    return mlp_simt_fwd(X, M, p, params, mask, ws_base(workspace), score_planes,
+                        (cudaStream_t)stream, true);
+  return mlp_tc_fwd(X, M, p, params, mask, ws_base(workspace), score_planes,
+                    precision == TFR_PREC_TF32X3 ? 3 : 1, (cudaStream_t)stream, true);
+}
+
+extern "C" int tfr_mlp_bwd_tasks(const void* Xv, int M, const tfr_mlp_cfg* cfg,
+                                 const float* params, const float* dscore_planes,
+                                 const float* task_weights_host, const uint8_t* mask,
+                                 void* workspace, float* grads, int precision, void* stream) {
+  int rc = check_tasks_args(cfg, precision);
+  if (rc) return rc;
+  const float* X = static_cast<const float*>(Xv);
+  TFR_REQUIRE(X && params && workspace && dscore_planes && grads, "NULL argument");
+  const int O = cfg->dims[cfg->n_dense];
+  TaskWeights tw{};
+  bool unit = true;
+  for (int o = 0; o < O; ++o) {
+    tw.w[o] = task_weights_host ? task_weights_host[o] : 1.f;
+    TFR_REQUIRE(std::isfinite(tw.w[o]), "task weight %d is not finite", o);
+    unit = unit && tw.w[o] == 1.f;
+  }
+  MlpPlan p;
+  rc = make_mlp_plan(cfg, M, &p);
+  if (rc) return rc;
+  TFR_REQUIRE(!(p.use_bn || p.input_bn) || p.bn_state, "cfg->bn_state must be set with BN");
+  if (M == 0) {
+    TFR_CUDA_OK(cudaMemsetAsync(grads, 0, p.n_params * sizeof(float), (cudaStream_t)stream));
+    return TFR_OK;
+  }
+  // One task of weight 1: the planar signal is the interleaved one, and tfr_mlp_bwd already
+  // zeroes masked rows of a single output.
+  const TaskWeights* twp = O == 1 && unit ? nullptr : &tw;
+  if (precision == TFR_PREC_FP32)
+    return mlp_simt_bwd(X, M, p, params, dscore_planes, mask, ws_base(workspace), grads,
+                        (cudaStream_t)stream, twp);
+  return mlp_tc_bwd(X, M, p, params, dscore_planes, mask, ws_base(workspace), grads,
+                    precision == TFR_PREC_TF32X3 ? 3 : 1, (cudaStream_t)stream, twp);
 }
 
 extern "C" int tfr_mlp_input_grad(const tfr_mlp_cfg* cfg, int M, const float* params,

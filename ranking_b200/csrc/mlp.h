@@ -65,21 +65,31 @@ int mlp_input_bn_fwd(const float* X, int M, const MlpPlan& p, const float* param
 int mlp_input_bn_bwd(const float* X, int M, const MlpPlan& p, const float* params, float* ws,
                      const float* dxin, float* grads, cudaStream_t st);
 
+// Loss weights of the task-major ("planar") score layout of tfr_mlp_fwd_tasks / _bwd_tasks:
+// score plane o is scores[o * M + m], and the output-layer backward reads the signal
+// w[o] * dscores[o * M + m], zeroed on masked rows.  Passed by value to the kernels.
+struct TaskWeights {
+  float w[8];
+};
+
 // Returns 0 on success and fills `p`; sets the error string otherwise.
 int make_mlp_plan(const tfr_mlp_cfg* cfg, int M, MlpPlan* p);
 
+// planar / tw: the task-major layout (TaskWeights); the defaults are tfr_mlp_fwd / _bwd's.
 int mlp_simt_fwd(const float* X, int M, const MlpPlan& p, const float* params,
-                 const uint8_t* mask, float* ws, float* scores, cudaStream_t st);
+                 const uint8_t* mask, float* ws, float* scores, cudaStream_t st,
+                 bool planar = false);
 int mlp_simt_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                  const float* dscores, const uint8_t* mask, float* ws, float* grads,
-                 cudaStream_t st);
+                 cudaStream_t st, const TaskWeights* tw = nullptr);
 
 // tensor-core (wgmma) path; passes = 1 (TF32) or 3 (3xTF32, fp32-faithful)
 int mlp_tc_fwd(const float* X, int M, const MlpPlan& p, const float* params,
-               const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st);
+               const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st,
+               bool planar = false);
 int mlp_tc_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                const float* dscores, const uint8_t* mask, float* ws, float* grads,
-               int passes, cudaStream_t st);
+               int passes, cudaStream_t st, const TaskWeights* tw = nullptr);
 
 // bf16 tensor-core path (wgmma bf16): X and all activations are bf16 in HBM
 int mlp_bf16_fwd(const void* X, int M, const MlpPlan& p, const float* params,
@@ -100,10 +110,11 @@ int mlp_tc_split_params(const MlpPlan& p, const float* params, float* ws, int pa
                         cudaStream_t st);
 int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
                     const float* params, const uint8_t* mask, float* ws, float* scores,
-                    int passes, cudaStream_t st);
+                    int passes, cudaStream_t st, bool planar = false);
 int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, const MlpPlan& p,
                      const float* params, const float* dscores, const uint8_t* mask,
-                     float* ws, float* grads, int passes, cudaStream_t st);
+                     float* ws, float* grads, int passes, cudaStream_t st,
+                     const TaskWeights* tw = nullptr);
 // Tower input gradient for columns [col0, col0 + ncols) after mlp_tc_bwd (no input BN,
 // at least one hidden layer): tfr_mlp_input_grad.
 int mlp_tc_input_grad(int M, const MlpPlan& p, const float* params, float* ws, int col0,
@@ -140,14 +151,20 @@ int mlp_tc_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ld
 bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& p, int passes);
 int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
                      const float* params, const uint8_t* mask, float* ws, float* scores,
-                     cudaStream_t st);
+                     cudaStream_t st, bool planar = false);
 
 // pieces of the CUDA-core path reused by the tensor-core path
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,
-                      const uint8_t* mask, float* scores, cudaStream_t st);
+                      const uint8_t* mask, float* scores, cudaStream_t st, bool planar = false);
 int mlp_out_layer_bwd2(const float* H, int M, int K, int O, const float* W, const float* dS,
                        const uint8_t* mask, int act, int rows_per, float* dH, float* slots,
                        size_t slot_stride, cudaStream_t st);
+// mlp_out_layer_bwd2's slots from the planar signal tw.w[o] * dS[o * M + m], zero on masked
+// rows (every O).
+int mlp_out_layer_bwd2_tasks(const float* H, int M, int K, int O, const float* W,
+                             const float* dS, const TaskWeights& tw, const uint8_t* mask, int act,
+                             int rows_per, float* dH, float* slots, size_t slot_stride,
+                             cudaStream_t st);
 int mlp_reduce2(const float* srcA, int slotsA, size_t strideA, size_t nA, const float* srcB,
                 int slotsB, size_t strideB, size_t nB, float* out, cudaStream_t st);
 int mlp_colsum(const float* dZ, int M, int N, int rows_per, int splits, float* partial,

@@ -117,11 +117,14 @@ static int launch_gemm(GemmArgs g, int splits, cudaStream_t st) {
 
 // ------------------------------------------------------- output layer fwd ---
 // scores[m, o] = H[m, :] . W[:, o] + b[o]; RestoreList fill for masked rows
-// (keras/layers.py:265).  One warp per row.
-__global__ void __launch_bounds__(256)
-out_layer_fwd_kernel(const float* __restrict__ H, int M, int K, int O,
-                     const float* __restrict__ W, const float* __restrict__ bias,
-                     const uint8_t* __restrict__ mask, float* __restrict__ scores) {
+// (keras/layers.py:265).  One warp per row.  kPlanar: task-major scores[o * M + m], with the
+// fill on every plane (tfr_mlp_fwd_tasks); otherwise [M, O], filled only when O == 1.
+template <bool kPlanar>
+__device__ __forceinline__ void out_layer_fwd(const float* __restrict__ H, int M, int K, int O,
+                                              const float* __restrict__ W,
+                                              const float* __restrict__ bias,
+                                              const uint8_t* __restrict__ mask,
+                                              float* __restrict__ scores) {
   // one warp per 4 consecutive rows: 4 independent row loads in flight per lane
   const int lane = threadIdx.x & 31;
   const int row0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 4;
@@ -139,22 +142,40 @@ out_layer_fwd_kernel(const float* __restrict__ H, int M, int K, int O,
     if (lane < 4 && row0 + lane < M) {
       const int row = row0 + lane;
       float v = (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]) + bias[o];
-      if (mask && O == 1 && !mask[row]) v = kLogEpsilon;
-      scores[(size_t)row * O + o] = v;
+      if (mask && (kPlanar || O == 1) && !mask[row]) v = kLogEpsilon;
+      scores[kPlanar ? (size_t)o * M + row : (size_t)row * O + o] = v;
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+out_layer_fwd_kernel(const float* __restrict__ H, int M, int K, int O,
+                     const float* __restrict__ W, const float* __restrict__ bias,
+                     const uint8_t* __restrict__ mask, float* __restrict__ scores) {
+  out_layer_fwd<false>(H, M, K, O, W, bias, mask, scores);
+}
+
+__global__ void __launch_bounds__(256)
+out_layer_fwd_tasks_kernel(const float* __restrict__ H, int M, int K, int O,
+                           const float* __restrict__ W, const float* __restrict__ bias,
+                           const uint8_t* __restrict__ mask, float* __restrict__ scores) {
+  out_layer_fwd<true>(H, M, K, O, W, bias, mask, scores);
 }
 
 // ------------------------------------------------------- output layer bwd ---
 // Rows [z*rows_per, ...): dH[m, k] = (sum_o dS[m, o] W[k, o]) * act'(H[m, k]);
 // partial[z][k*O + o] = sum_m H[m, k] dS[m, o]; partial[z][K*O + o] = sum_m dS[m, o].
+// kPlanar: dS[m, o] is tw.w[o] * dS[o * M + m], zero on masked rows for every O.
 constexpr int kMaxOut = 8;
-__global__ void __launch_bounds__(1024)
-out_layer_bwd_kernel(const float* __restrict__ H, int M, int K, int O,
-                     const float* __restrict__ W, const float* __restrict__ dS,
-                     const uint8_t* __restrict__ mask, int act, int rows_per,
-                     float* __restrict__ dH, float* __restrict__ partial,
-                     size_t partial_stride) {
+
+template <bool kPlanar>
+__device__ __forceinline__ void out_layer_bwd(const float* __restrict__ H, int M, int K, int O,
+                                              const float* __restrict__ W,
+                                              const float* __restrict__ dS,
+                                              const uint8_t* __restrict__ mask, int act,
+                                              int rows_per, float* __restrict__ dH,
+                                              float* __restrict__ partial, size_t partial_stride,
+                                              const TaskWeights& tw) {
   const int k = threadIdx.x;
   const int z = blockIdx.x;
   const int mbeg = z * rows_per, mend = min(M, mbeg + rows_per);
@@ -166,10 +187,16 @@ out_layer_bwd_kernel(const float* __restrict__ H, int M, int K, int O,
     db[o] = 0.f;
   }
   for (int m = mbeg; m < mend; ++m) {
-    const bool live = !(mask && O == 1 && !mask[m]);
+    const bool live = !(mask && (kPlanar || O == 1) && !mask[m]);
     float ds[kMaxOut];
+    if (kPlanar) {
 #pragma unroll
-    for (int o = 0; o < kMaxOut; ++o) ds[o] = (o < O && live) ? dS[(size_t)m * O + o] : 0.f;
+      for (int o = 0; o < kMaxOut; ++o)
+        ds[o] = (o < O && live) ? dS[(size_t)o * M + m] * tw.w[o] : 0.f;
+    } else {
+#pragma unroll
+      for (int o = 0; o < kMaxOut; ++o) ds[o] = (o < O && live) ? dS[(size_t)m * O + o] : 0.f;
+    }
     if (k < K) {
       const float h = H[(size_t)m * K + k];
       float dh = 0.f;
@@ -191,6 +218,25 @@ out_layer_bwd_kernel(const float* __restrict__ H, int M, int K, int O,
     for (int o = 0; o < O; ++o) p[(size_t)k * O + o] = dw[o];
   if (k == 0)
     for (int o = 0; o < O; ++o) p[(size_t)K * O + o] = db[o];
+}
+
+__global__ void __launch_bounds__(1024)
+out_layer_bwd_kernel(const float* __restrict__ H, int M, int K, int O,
+                     const float* __restrict__ W, const float* __restrict__ dS,
+                     const uint8_t* __restrict__ mask, int act, int rows_per,
+                     float* __restrict__ dH, float* __restrict__ partial,
+                     size_t partial_stride) {
+  out_layer_bwd<false>(H, M, K, O, W, dS, mask, act, rows_per, dH, partial, partial_stride,
+                       TaskWeights{});
+}
+
+__global__ void __launch_bounds__(1024)
+out_layer_bwd_tasks_kernel(const float* __restrict__ H, int M, int K, int O,
+                           const float* __restrict__ W, const float* __restrict__ dS,
+                           const uint8_t* __restrict__ mask, int act, int rows_per,
+                           float* __restrict__ dH, float* __restrict__ partial,
+                           size_t partial_stride, const TaskWeights tw) {
+  out_layer_bwd<true>(H, M, K, O, W, dS, mask, act, rows_per, dH, partial, partial_stride, tw);
 }
 
 // partial[z][N cols] column sums of dZ rows handled by split z.
@@ -340,12 +386,17 @@ out_layer_bwd2_o1_kernel(const float4* __restrict__ H4, int M, int K4,
 
 // The same float4 streaming for 2 <= O <= 4 outputs (groupwise scoring: O = group_size): the
 // slot layout is the generic one, { dW[K * O] (k-major, o fastest), db[O], pad to 4, csum[K] }.
-template <int O>
-__global__ void __launch_bounds__(256)
-out_layer_bwd2_vec_kernel(const float4* __restrict__ H4, int M, int K4, const float* __restrict__ W,
-                          const float* __restrict__ dS, int act, int rows_per, int RL,
-                          float4* __restrict__ dH4, float* __restrict__ slots,
-                          size_t slot_stride) {
+// kPlanar (1 <= O <= 8, tfr_mlp_bwd_tasks): the signal is tw.w[o] * dS[o * M + m], zero on
+// rows `mask` clears; the interleaved instantiations take no mask.
+template <int O, bool kPlanar>
+__device__ __forceinline__ void out_layer_bwd2_vec(const float4* __restrict__ H4, int M, int K4,
+                                                   const float* __restrict__ W,
+                                                   const float* __restrict__ dS, int act,
+                                                   int rows_per, int RL,
+                                                   float4* __restrict__ dH4,
+                                                   float* __restrict__ slots, size_t slot_stride,
+                                                   const uint8_t* __restrict__ mask,
+                                                   const TaskWeights& tw) {
   extern __shared__ float sm[];   // [RL][round4(K * O + O) + K]
   const int k4 = threadIdx.x % K4, rl = threadIdx.x / K4;
   const int K = K4 * 4;
@@ -367,8 +418,15 @@ out_layer_bwd2_vec_kernel(const float4* __restrict__ H4, int M, int K4, const fl
 #pragma unroll 4
     for (int m = mbeg + rl; m < mend; m += RL) {
       float ds[O];
+      if (kPlanar) {
+        const bool live = !(mask && !mask[m]);
+        const float* q = dS + m;
 #pragma unroll
-      for (int o = 0; o < O; ++o) ds[o] = __ldg(dS + (size_t)m * O + o);
+        for (int o = 0; o < O; ++o, q += M) ds[o] = live ? __ldg(q) * tw.w[o] : 0.f;
+      } else {
+#pragma unroll
+        for (int o = 0; o < O; ++o) ds[o] = __ldg(dS + (size_t)m * O + o);
+      }
       const float4 h4 = H4[(size_t)m * K4 + k4];
       const float h[4] = {h4.x, h4.y, h4.z, h4.w};
       float dh[4];
@@ -417,6 +475,29 @@ out_layer_bwd2_vec_kernel(const float4* __restrict__ H4, int M, int K4, const fl
     for (int r = 0; r < RL; ++r) acc += sm[(size_t)r * per + i];
     out[i] = acc;
   }
+}
+
+template <int O>
+__global__ void __launch_bounds__(256)
+out_layer_bwd2_vec_kernel(const float4* __restrict__ H4, int M, int K4, const float* __restrict__ W,
+                          const float* __restrict__ dS, int act, int rows_per, int RL,
+                          float4* __restrict__ dH4, float* __restrict__ slots,
+                          size_t slot_stride) {
+  out_layer_bwd2_vec<O, false>(H4, M, K4, W, dS, act, rows_per, RL, dH4, slots, slot_stride,
+                               nullptr, TaskWeights{});
+}
+
+// (256, 1): lets ptxas keep the O weights and accumulators in registers (it chose 64 and
+// spilled at O = 3 without the hint).
+template <int O>
+__global__ void __launch_bounds__(256, 1)
+out_layer_bwd2_vec_tasks_kernel(const float4* __restrict__ H4, int M, int K4,
+                                const float* __restrict__ W, const float* __restrict__ dS,
+                                int act, int rows_per, int RL, float4* __restrict__ dH4,
+                                float* __restrict__ slots, size_t slot_stride,
+                                const uint8_t* __restrict__ mask, const TaskWeights tw) {
+  out_layer_bwd2_vec<O, true>(H4, M, K4, W, dS, act, rows_per, RL, dH4, slots, slot_stride, mask,
+                              tw);
 }
 
 // out[i] = sum over slots of srcA (i < nA) or srcB (nA <= i < nA + nB): the weight
@@ -598,11 +679,53 @@ int mlp_out_layer_bwd2(const float* H, int M, int K, int O, const float* W, cons
   return TFR_OK;
 }
 
+int mlp_out_layer_bwd2_tasks(const float* H, int M, int K, int O, const float* W,
+                             const float* dS, const TaskWeights& tw, const uint8_t* mask, int act,
+                             int rows_per, float* dH, float* slots, size_t slot_stride,
+                             cudaStream_t st) {
+  const int blocks = (M + rows_per - 1) / rows_per;
+  if (K % 4 == 0 && K <= 1024 && (reinterpret_cast<uintptr_t>(H) & 15) == 0 &&
+      (!dH || (reinterpret_cast<uintptr_t>(dH) & 15) == 0)) {
+    const int K4 = K / 4;
+    const int RL = 256 / K4;
+    const size_t smem = (size_t)RL * (((K * O + O + 3) & ~3) + K) * sizeof(float);
+    auto launch = [&](auto kernel) -> int {
+      if (smem > 48 * 1024)
+        TFR_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+      kernel<<<blocks, 256, smem, st>>>(reinterpret_cast<const float4*>(H), M, K4, W, dS, act,
+                                        rows_per, RL, reinterpret_cast<float4*>(dH), slots,
+                                        slot_stride, mask, tw);
+      TFR_LAUNCH_OK();
+      return TFR_OK;
+    };
+    switch (O) {
+      case 1: return launch(out_layer_bwd2_vec_tasks_kernel<1>);
+      case 2: return launch(out_layer_bwd2_vec_tasks_kernel<2>);
+      case 3: return launch(out_layer_bwd2_vec_tasks_kernel<3>);
+      case 4: return launch(out_layer_bwd2_vec_tasks_kernel<4>);
+      case 5: return launch(out_layer_bwd2_vec_tasks_kernel<5>);
+      case 6: return launch(out_layer_bwd2_vec_tasks_kernel<6>);
+      case 7: return launch(out_layer_bwd2_vec_tasks_kernel<7>);
+      default: return launch(out_layer_bwd2_vec_tasks_kernel<8>);
+    }
+  }
+  // An unaligned H is the tower input itself (no hidden layer, no input BN), so there is no
+  // dH and no column sums to write: out_layer_bwd_kernel's per-split {dW, db} is the slot
+  // prefix that is read.
+  TFR_REQUIRE(dH == nullptr, "planar output-layer backward needs a 16-byte aligned H (K = %d)", K);
+  out_layer_bwd_tasks_kernel<<<blocks, ((K + 31) / 32) * 32, 0, st>>>(
+      H, M, K, O, W, dS, mask, act, rows_per, nullptr, slots, slot_stride, tw);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,
-                      const uint8_t* mask, float* scores, cudaStream_t st) {
+                      const uint8_t* mask, float* scores, cudaStream_t st, bool planar) {
   const int rows_per_block = 32;
-  out_layer_fwd_kernel<<<(M + rows_per_block - 1) / rows_per_block, 256, 0, st>>>(
-      H, M, K, O, W, bias, mask, scores);
+  auto kernel = planar ? out_layer_fwd_tasks_kernel : out_layer_fwd_kernel;
+  kernel<<<(M + rows_per_block - 1) / rows_per_block, 256, 0, st>>>(H, M, K, O, W, bias, mask,
+                                                                     scores);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }
@@ -623,7 +746,7 @@ int mlp_reduce_partials(const float* partial, int splits, size_t stride, size_t 
 }
 
 int mlp_simt_fwd(const float* X, int M, const MlpPlan& p, const float* params,
-                 const uint8_t* mask, float* ws, float* scores, cudaStream_t st) {
+                 const uint8_t* mask, float* ws, float* scores, cudaStream_t st, bool planar) {
   const int L = p.n_dense - 1;  // hidden layers
   const float* in = X;
   if (p.input_bn) {
@@ -648,12 +771,12 @@ int mlp_simt_fwd(const float* X, int M, const MlpPlan& p, const float* params,
   }
   const int K = p.dims[L], O = p.dims[L + 1];
   return mlp_out_layer_fwd(in, M, K, O, params + p.w_off[L], params + p.b_off[L], mask, scores,
-                           st);
+                           st, planar);
 }
 
 int mlp_simt_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                  const float* dscores, const uint8_t* mask, float* ws, float* grads,
-                 cudaStream_t st) {
+                 cudaStream_t st, const TaskWeights* tw) {
   const int L = p.n_dense - 1;
   float* partial = ws + p.partial_off;
   const size_t pstride = p.partial_stride;
@@ -669,9 +792,14 @@ int mlp_simt_bwd(const float* X, int M, const MlpPlan& p, const float* params,
     const int K = p.dims[L], O = p.dims[L + 1];
     const float* H = L > 0 ? ws + p.act_off[L - 1] : X0;
     const int threads = ((K + 31) / 32) * 32;
-    out_layer_bwd_kernel<<<splits, threads, 0, st>>>(
-        H, M, K, O, params + p.w_off[L], dscores, mask, L > 0 ? mact : TFR_ACT_NONE,
-        rows_per, (L > 0 || p.input_bn) ? dz_cur : nullptr, partial, pstride);
+    const int act = L > 0 ? mact : TFR_ACT_NONE;
+    float* dH = (L > 0 || p.input_bn) ? dz_cur : nullptr;
+    if (tw)
+      out_layer_bwd_tasks_kernel<<<splits, threads, 0, st>>>(
+          H, M, K, O, params + p.w_off[L], dscores, mask, act, rows_per, dH, partial, pstride, *tw);
+    else
+      out_layer_bwd_kernel<<<splits, threads, 0, st>>>(
+          H, M, K, O, params + p.w_off[L], dscores, mask, act, rows_per, dH, partial, pstride);
     TFR_LAUNCH_OK();
     const size_t n = (size_t)K * O + O;
     reduce_partials_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(partial, splits, pstride, n,

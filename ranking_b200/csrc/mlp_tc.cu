@@ -163,15 +163,16 @@ int mlp_tc_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ld
 }
 
 int mlp_tc_fwd(const float* X, int M, const MlpPlan& p, const float* params,
-               const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st) {
-  return mlp_tc_fwd_from(0, X, M, p, params, mask, ws, scores, passes, st);
+               const uint8_t* mask, float* ws, float* scores, int passes, cudaStream_t st,
+               bool planar) {
+  return mlp_tc_fwd_from(0, X, M, p, params, mask, ws, scores, passes, st, planar);
 }
 
 // Layers first_layer .. L-1 and the output layer.  first_layer > 0: `X` is the activation
 // that feeds Dense `first_layer` (the caller produced it and already split the parameters).
 int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
                     const float* params, const uint8_t* mask, float* ws, float* scores,
-                    int passes, cudaStream_t st) {
+                    int passes, cudaStream_t st, bool planar) {
   int rc = check_dims(p);
   if (rc) return rc;
   if (first_layer == 0) {
@@ -179,7 +180,7 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
     if (rc) return rc;
   }
   if (mlp_tc_fused_fwd_ok(first_layer, X, M, p, passes))
-    return mlp_tc_fused_fwd(first_layer, X, M, p, params, mask, ws, scores, st);
+    return mlp_tc_fused_fwd(first_layer, X, M, p, params, mask, ws, scores, st, planar);
   const int L = p.n_dense - 1;
   const float* in = X;
   if (p.input_bn && first_layer == 0) {
@@ -201,13 +202,13 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
     in = ws + p.act_off[d];
   }
   return mlp_out_layer_fwd(in, M, p.dims[L], p.dims[L + 1], params + p.w_off[L],
-                           params + p.b_off[L], mask, scores, st);
+                           params + p.b_off[L], mask, scores, st, planar);
 }
 
 int mlp_tc_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                const float* dscores, const uint8_t* mask, float* ws, float* grads,
-               int passes, cudaStream_t st) {
-  return mlp_tc_bwd_until(0, nullptr, X, M, p, params, dscores, mask, ws, grads, passes, st);
+               int passes, cudaStream_t st, const TaskWeights* tw) {
+  return mlp_tc_bwd_until(0, nullptr, X, M, p, params, dscores, mask, ws, grads, passes, st, tw);
 }
 
 // Backward of the output layer and of Dense L-1 .. stop_layer.  With stop_layer > 0 the
@@ -215,7 +216,8 @@ int mlp_tc_bwd(const float* X, int M, const MlpPlan& p, const float* params,
 // column sums taken); `tail` then describes where that signal and its column sums live.
 int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, const MlpPlan& p,
                      const float* params, const float* dscores, const uint8_t* mask,
-                     float* ws, float* grads, int passes, cudaStream_t st) {
+                     float* ws, float* grads, int passes, cudaStream_t st,
+                     const TaskWeights* tw) {
   int rc = check_dims(p);
   if (rc) return rc;
   const int L = p.n_dense - 1;
@@ -235,10 +237,12 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
     // `splits` partial slots and reduced.
     const int K = p.dims[L], O = p.dims[L + 1];
     const float* H = L > 0 ? ws + p.act_off[L - 1] : X0;
-    rc = mlp_out_layer_bwd2(H, M, K, O, params + p.w_off[L], dscores, mask,
-                            L > 0 ? mact : TFR_ACT_NONE, p.out_rows,
-                            (L > 0 || p.input_bn) ? dz_cur : nullptr, oslots, p.oslot_stride,
-                            st);
+    const int act = L > 0 ? mact : TFR_ACT_NONE;
+    float* dH = (L > 0 || p.input_bn) ? dz_cur : nullptr;
+    rc = tw ? mlp_out_layer_bwd2_tasks(H, M, K, O, params + p.w_off[L], dscores, *tw, mask, act,
+                                       p.out_rows, dH, oslots, p.oslot_stride, st)
+            : mlp_out_layer_bwd2(H, M, K, O, params + p.w_off[L], dscores, mask, act, p.out_rows,
+                                 dH, oslots, p.oslot_stride, st);
     if (rc) return rc;
     // out-layer gradient: [K*O + O] summed over the block slots
     rc = mlp_reduce2(oslots, p.out_slots, p.oslot_stride, (size_t)K * O + O, nullptr, 0, 0, 0,

@@ -295,7 +295,9 @@ __device__ __forceinline__ void store_rows(const FusedArgs& a, const Seg& sg, co
 }
 
 // Scores of tile rows 32 ew .. 32 ew + 31 from the last hidden layer in Hbuf, in
-// out_layer_fwd_kernel's order; RestoreList fill for masked rows.
+// out_layer_fwd_kernel's order; RestoreList fill for masked rows.  kPlanar: task-major
+// scores[o * M + row] with the fill on every plane, as out_layer_fwd_kernel<true>.
+template <bool kPlanar>
 __device__ __forceinline__ void out_rows(const FusedArgs& a, const float* hb, int m0, int ew,
                                          int lane) {
   for (int r0 = 32 * ew; r0 < 32 * ew + 32; r0 += 4) {
@@ -312,8 +314,9 @@ __device__ __forceinline__ void out_rows(const FusedArgs& a, const float* hb, in
       if (lane < 4 && row < a.M) {
         float v = (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]) +
                   __ldg(a.bout + o);
-        if (a.mask && a.O == 1 && !a.mask[row]) v = kLogEpsilon;
-        a.scores[static_cast<size_t>(row) * a.O + o] = v;
+        if (a.mask && (kPlanar || a.O == 1) && !a.mask[row]) v = kLogEpsilon;
+        a.scores[kPlanar ? static_cast<size_t>(o) * a.M + row : static_cast<size_t>(row) * a.O + o] =
+            v;
       }
     }
   }
@@ -323,6 +326,7 @@ __device__ __forceinline__ void out_rows(const FusedArgs& a, const float* hb, in
 // every Hbuf they hand over; the last segment with an epilogue is the last hidden layer, whose
 // Hbuf also feeds the output layer.  It frees Hbuf after every pass but the CTA's last, which
 // nobody would wait for.
+template <bool kPlanar>
 __device__ __forceinline__ void epilogue_warpgroup(const FusedArgs& a, const float* hb) {
   const int lane = threadIdx.x & 31, ew = (threadIdx.x - wg::kThreads) >> 5;
   int last = 0;
@@ -336,20 +340,20 @@ __device__ __forceinline__ void epilogue_warpgroup(const FusedArgs& a, const flo
       wg::bar_sync(wg::kBarFull, kHandoff);
       if (sg.N - sg.n0 <= 64) store_rows<true>(a, sg, hb, m0, ew, lane);
       else store_rows<false>(a, sg, hb, m0, ew, lane);
-      if (q == last) out_rows(a, hb, m0, ew, lane);
+      if (q == last) out_rows<kPlanar>(a, hb, m0, ew, lane);
       if (q != last || tile + static_cast<int>(gridDim.x) < a.m_tiles)
         wg::bar_arrive(wg::kBarFree, kHandoff);
     }
   }
 }
 
-__global__ void __launch_bounds__(kHandoff, 1)
-tower_fused_fwd_kernel(const __grid_constant__ FusedArgs args) {
+template <bool kPlanar>
+__device__ __forceinline__ void tower_fused_fwd(const FusedArgs& args) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (wg::smem_u32(smem_raw) & 1023u)) & 1023u);
   if (threadIdx.x >= wg::kThreads) {
     wg::setmaxnreg_dec<wg::kEpiRegs>();
-    epilogue_warpgroup(args, reinterpret_cast<const float*>(smem + kHbufOff));
+    epilogue_warpgroup<kPlanar>(args, reinterpret_cast<const float*>(smem + kHbufOff));
     return;
   }
   wg::setmaxnreg_inc<wg::kMmaRegs>();
@@ -369,6 +373,17 @@ tower_fused_fwd_kernel(const __grid_constant__ FusedArgs args) {
   }
 }
 
+__global__ void __launch_bounds__(kHandoff, 1)
+tower_fused_fwd_kernel(const __grid_constant__ FusedArgs args) {
+  tower_fused_fwd<false>(args);
+}
+
+// tfr_mlp_fwd_tasks: the same kernel with task-major score planes (out_rows<true>).
+__global__ void __launch_bounds__(kHandoff, 1)
+tower_fused_fwd_tasks_kernel(const __grid_constant__ FusedArgs args) {
+  tower_fused_fwd<true>(args);
+}
+
 }  // namespace fused
 
 bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& p, int passes) {
@@ -385,7 +400,7 @@ bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& 
 
 int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
                      const float* params, const uint8_t* mask, float* ws, float* scores,
-                     cudaStream_t st) {
+                     cudaStream_t st, bool planar) {
   const int L = p.n_dense - 1, f = first_layer;
   fused::FusedArgs a{};
   a.X = X; a.ldx = p.dims[f];
@@ -418,9 +433,10 @@ int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
 
   const int sms = num_sms();
   const int grid = a.m_tiles < sms ? a.m_tiles : sms;
-  TFR_CUDA_OK(cudaFuncSetAttribute(fused::tower_fused_fwd_kernel,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, fused::kSmem));
-  fused::tower_fused_fwd_kernel<<<grid, fused::kHandoff, fused::kSmem, st>>>(a);
+  auto kernel = planar ? fused::tower_fused_fwd_tasks_kernel : fused::tower_fused_fwd_kernel;
+  TFR_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   fused::kSmem));
+  kernel<<<grid, fused::kHandoff, fused::kSmem, st>>>(a);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

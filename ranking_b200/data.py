@@ -491,6 +491,76 @@ def elwc_batches(paths, batch_size, list_size, context_feature_spec, example_fea
     yield flush()
 
 
+def elwc_multilabel_batches(paths, batch_size, list_size, context_feature_spec,
+                            example_feature_spec, label_spec, sample_weight_feature=None,
+                            drop_remainder=True, pin_memory=True):
+  """Multi-task batches (the reference's `MultiLabelDatasetBuilder._features_and_labels`,
+  keras/pipeline.py:1196-1221): yields (x [B, list_size, Dc + De], labels {task: [B,
+  list_size]}, mask [B, list_size] bool, weights [B, list_size] or None).
+
+  `label_spec` maps each task to the example feature holding its label (dim 1); give those
+  features the default -1 so that an item without a task's label is invalid for that task.
+  Padded slots are -1 in every task.  `sample_weight_feature` names an example feature (dim 1)
+  holding the per-item weight shared by the tasks.  Label and weight columns are removed from
+  x; `mask` is the decoder's list mask (real items, whatever their labels)."""
+  ex_spec = dict(example_feature_spec)
+  label_spec = dict(label_spec)
+  if not label_spec:
+    raise ValueError('label_spec must map at least one task to a label feature')
+  special = {}
+  for task, name in label_spec.items():
+    special.setdefault(name, []).append(task)
+  if sample_weight_feature is not None:
+    if sample_weight_feature in special:
+      raise ValueError('%r is both a label and the sample weight' % sample_weight_feature)
+    special[sample_weight_feature] = []
+  off, cols, where = 0, [], {}
+  for name in ex_spec:
+    dim = int(ex_spec[name][0])
+    if name in special:
+      if dim != 1:
+        raise ValueError('label and weight features must have dim 1 (%r has %d)' % (name, dim))
+      where[name] = off
+    else:
+      cols.extend(range(off, off + dim))
+    off += dim
+  missing = sorted(set(special) - set(where))
+  if missing:
+    raise ValueError('features %s are not in example_feature_spec' % missing)
+  buf = []
+
+  def flush():
+    out = parse_from_example_list(buf, list_size, context_feature_spec, ex_spec,
+                                  pin_memory=False)
+    ex, mask = out['examples'], out['mask']
+    pin = pin_memory and torch.cuda.is_available()
+    labels = {}
+    for task, name in label_spec.items():
+      y = torch.where(mask, ex[:, :, where[name]], torch.full_like(ex[:, :, 0], -1.))
+      labels[task] = y.pin_memory() if pin else y
+    weights = None
+    if sample_weight_feature is not None:
+      weights = ex[:, :, where[sample_weight_feature]].contiguous()
+      weights = weights.pin_memory() if pin else weights
+    feats = ex[:, :, cols]
+    if out['context'].shape[1]:
+      ctx = out['context'].unsqueeze(1).expand(-1, list_size, -1)
+      feats = torch.cat([ctx, feats], 2)
+    x = feats.contiguous()
+    if pin:
+      x, mask = x.pin_memory(), mask.pin_memory()
+    return x, labels, mask, weights
+
+  for path in ([paths] if isinstance(paths, str) else paths):
+    for rec in read_tfrecords(path):
+      buf.append(rec)
+      if len(buf) == batch_size:
+        yield flush()
+        buf = []
+  if buf and not drop_remainder:
+    yield flush()
+
+
 class Prefetcher(object):
   """Runs a batch iterator (e.g. `elwc_batches(..., pin_memory=True)`: TFRecord read +
   native ELWC decode into pinned buffers) in a background thread, `depth` batches ahead, so

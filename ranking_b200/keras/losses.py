@@ -156,6 +156,9 @@ def _keras_reduce(losses, sample_weight, reduction):
 
 class _RankingLoss(object):
   """keras/losses.py:247-285."""
+  # `fused_fwd_bwd(y_true, y_pred, sample_weight, grad_out, per_list, total2)` over one [B, N]
+  # score matrix: the losses a multi-task step can run on a task's score plane.
+  fused_single_score = True
 
   def __init__(self, reduction=Reduction.AUTO, name=None, ragged=False):
     Reduction.validate(reduction)
@@ -518,6 +521,7 @@ class MeanSquaredLoss(_PointwiseLoss):
 
 class CoupledRankDistilLoss(_RankingLoss):
   """keras/losses.py:1659-1750."""
+  fused_single_score = False   # autograd only
 
   def __init__(self, reduction=Reduction.AUTO, name=None, ragged=False, sample_size=8,
                topk=None, temperature=1.):
@@ -546,6 +550,7 @@ class CoupledRankDistilLoss(_RankingLoss):
 
 class OrdinalLoss(_PointwiseLoss):
   """keras/losses.py:1603-1656: y_pred [B, N, ordinal_size]."""
+  fused_single_score = False   # multi-column scores
 
   def __init__(self, reduction=Reduction.AUTO, name=None, ragged=False,
                ordinal_size=1, use_fraction_label=False):
@@ -563,6 +568,7 @@ class ClickEMLoss(_PointwiseLoss):
   clicks.  A pointwise loss: AUTO / SUM_OVER_BATCH_SIZE divide the summed item losses by
   B * N, padded slots included.  Not a RankingLossKey member (neither is it in the
   reference), so `get` does not build it."""
+  fused_single_score = False   # two score columns
 
   def __init__(self, reduction=Reduction.AUTO, name=None, exam_loss_weight=1.0,
                rel_loss_weight=1.0, ragged=False):
@@ -604,6 +610,7 @@ class MixtureEMLoss(_RankingLoss):
   """keras/losses.py:1421-1496: y_pred [B, N, model_num], y_true clicks.  As in the
   reference, `lambda_weight` and `temperature` are accepted and kept in the config but the
   loss is built without them (keras/losses.py:1484-1489), so neither changes its value."""
+  fused_single_score = False   # model_num score columns
 
   def __init__(self, reduction=Reduction.AUTO, name=None, lambda_weight=None,
                temperature=1.0, alpha=1.0, ragged=False):

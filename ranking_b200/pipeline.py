@@ -132,12 +132,16 @@ class PipelineHparams:
   def validate(self):
     if not isinstance(self.loss, str):
       raise ValueError('multi-task loss maps are not supported by the fused step')
+    self.validate_loop()
+    if self.loss_weights is not None and not isinstance(self.loss_weights, (int, float)):
+      raise ValueError('loss_weights must be None or a scalar')
+
+  def validate_loop(self):
+    """The checks that do not depend on the loss: optimizer and loop lengths."""
     if self.optimizer not in ('adagrad', 'sgd'):
       raise ValueError("optimizer must be 'adagrad' or 'sgd', got %r" % (self.optimizer,))
     if self.num_epochs < 1 or self.steps_per_epoch < 1 or self.validation_steps < 0:
       raise ValueError('num_epochs / steps_per_epoch must be >= 1, validation_steps >= 0')
-    if self.loss_weights is not None and not isinstance(self.loss_weights, (int, float)):
-      raise ValueError('loss_weights must be None or a scalar')
 
 
 class ModelFitPipeline(object):
@@ -155,7 +159,7 @@ class ModelFitPipeline(object):
 
   def __init__(self, tower_fn, train_batches_fn, valid_batches_fn, hparams,
                process_group=None, log_fn=print):
-    hparams.validate()
+    self._validate_hparams(hparams)
     self._hparams = hparams
     self._tower_fn = tower_fn
     self._train_fn = train_batches_fn
@@ -163,6 +167,10 @@ class ModelFitPipeline(object):
     self._group = process_group
     self._log = log_fn
     self.history = []
+
+  @staticmethod
+  def _validate_hparams(hparams):
+    hparams.validate()
 
   def build_loss(self):
     from ranking_b200.keras import losses as keras_losses
@@ -180,13 +188,30 @@ class ModelFitPipeline(object):
       raise ValueError('best_exporter_metric %r is not among %s' % (key, sorted(logs)))
     return logs[key]
 
-  def train_and_validate(self, verbose=0):
+  def _make_trainer(self, tower):
     from ranking_b200 import train as train_lib
     hp = self._hparams
+    return train_lib.RankingTrainer(tower, self.build_loss(), optimizer=hp.optimizer,
+                                    learning_rate=hp.learning_rate, process_group=self._group)
+
+  def _train_step(self, trainer, batch, dev):
+    x, y = batch
+    return trainer.train_step(x.to(dev, non_blocking=True), y.to(dev, non_blocking=True))
+
+  def _validation_logs(self, trainer, vb, dev):
+    logs = evaluate(trainer, vb, self.build_metrics())
+    vloss = 0.0
+    loss_obj = trainer.loss
+    for x, y in vb:
+      xd, yd = x.to(dev), y.to(dev)
+      vloss += float(loss_obj(yd, trainer.predict(xd, mask=(yd >= 0)).clone()))
+    logs['loss'] = vloss / max(len(vb), 1)
+    return logs
+
+  def train_and_validate(self, verbose=0):
+    hp = self._hparams
     tower = self._tower_fn()
-    trainer = train_lib.RankingTrainer(tower, self.build_loss(), optimizer=hp.optimizer,
-                                       learning_rate=hp.learning_rate,
-                                       process_group=self._group)
+    trainer = self._make_trainer(tower)
     os.makedirs(hp.model_dir, exist_ok=True)
     ckpt = os.path.join(hp.model_dir, 'ckpt.pt')
     best_dir = os.path.join(hp.model_dir, 'best_checkpoint')
@@ -200,11 +225,11 @@ class ModelFitPipeline(object):
       loss_sum, n = 0.0, 0
       while step < (epoch + 1) * hp.steps_per_epoch:
         try:
-          x, y = next(train_it)
+          batch = next(train_it)
         except StopIteration:
           train_it = iter(self._train_fn())
-          x, y = next(train_it)
-        loss = trainer.train_step(x.to(dev, non_blocking=True), y.to(dev, non_blocking=True))
+          batch = next(train_it)
+        loss = self._train_step(trainer, batch, dev)
         step += 1
         loss_sum += float(loss)
         n += 1
@@ -212,13 +237,7 @@ class ModelFitPipeline(object):
       if self._valid_fn is not None and hp.validation_steps > 0:
         import itertools
         vb = list(itertools.islice(iter(self._valid_fn()), hp.validation_steps))
-        logs.update(evaluate(trainer, vb, self.build_metrics()))
-        vloss = 0.0
-        loss_obj = trainer.loss
-        for x, y in vb:
-          xd, yd = x.to(dev), y.to(dev)
-          vloss += float(loss_obj(yd, trainer.predict(xd, mask=(yd >= 0)).clone()))
-        logs['loss'] = vloss / max(len(vb), 1)
+        logs.update(self._validation_logs(trainer, vb, dev))
       else:
         logs['loss'] = logs['train_loss']
       self.history.append(logs)
@@ -243,3 +262,100 @@ class ModelFitPipeline(object):
           break
     self.trainer = trainer
     return self.history
+
+
+class MultiTaskPipeline(ModelFitPipeline):
+  """`MultiTaskPipeline` (keras/pipeline.py:733-824) over `MultiTaskRankingTrainer`:
+  `hparams.loss` maps each task to a loss key (dict order = the tower's output units) and
+  `hparams.loss_weights` is None or a dict over those tasks.  The epoch loop, checkpoints,
+  best checkpoint, early stopping and ReduceLROnPlateau are `ModelFitPipeline`'s.
+
+  Batches are (x, labels {task: [B, N]}, mask, sample_weight or None), as
+  `data.elwc_multilabel_batches` yields them, or (x, labels).  Validation logs use Keras'
+  multi-output names: `loss` (sum_t w_t <task>_loss), `<task>_loss`, and
+  `<task>_metric/ndcg_1`, `_5`, `_10`, `<task>_metric/ndcg`; with `use_weighted_metrics` also
+  `<task>_weighted_metric/...` under the sample weights.  `best_exporter_metric` may name any
+  of them."""
+
+  TOPNS = (1, 5, 10, None)
+
+  def __init__(self, tower_fn, train_batches_fn, valid_batches_fn, hparams,
+               process_group=None, log_fn=print):
+    super().__init__(tower_fn, train_batches_fn, valid_batches_fn, hparams,
+                     process_group=process_group, log_fn=log_fn)
+    self.tasks = list(hparams.loss)
+
+  @staticmethod
+  def _validate_hparams(hparams):
+    # PipelineHparams.validate() refuses loss maps (the single-task step); the loop checks
+    # are shared.
+    if not isinstance(hparams.loss, dict) or not hparams.loss:
+      raise ValueError('MultiTaskPipeline needs hparams.loss as a dict task -> loss key')
+    if len(hparams.loss) > 8:
+      raise ValueError('at most 8 tasks, got %d' % len(hparams.loss))
+    weights = hparams.loss_weights
+    if weights is not None:
+      if not isinstance(weights, dict):
+        raise ValueError('loss_weights must be None or a dict over the tasks')
+      unknown = sorted(set(weights) - set(hparams.loss))
+      if unknown:
+        raise ValueError('loss_weights name unknown tasks %s' % unknown)
+    hparams.validate_loop()
+
+  def build_loss(self):
+    from ranking_b200.keras import losses as keras_losses
+    kw = {}
+    if self._hparams.loss_reduction not in (None, 'auto'):
+      kw['reduction'] = self._hparams.loss_reduction
+    return {t: keras_losses.get(key, **kw) for t, key in self._hparams.loss.items()}
+
+  def _make_trainer(self, tower):
+    from ranking_b200 import train as train_lib
+    hp = self._hparams
+    return train_lib.MultiTaskRankingTrainer(tower, self.build_loss(),
+                                             loss_weights=hp.loss_weights,
+                                             optimizer=hp.optimizer,
+                                             learning_rate=hp.learning_rate,
+                                             process_group=self._group)
+
+  @staticmethod
+  def _unpack(batch, dev, non_blocking=False):
+    x, labels = batch[0], batch[1]
+    mask = batch[2] if len(batch) > 2 else None
+    weights = batch[3] if len(batch) > 3 else None
+    mv = lambda t: None if t is None else t.to(dev, non_blocking=non_blocking)
+    return mv(x), {t: mv(y) for t, y in labels.items()}, mv(mask), mv(weights)
+
+  def _train_step(self, trainer, batch, dev):
+    x, labels, mask, weights = self._unpack(batch, dev, non_blocking=True)
+    return trainer.train_step(x, labels, sample_weight=weights, mask=mask)
+
+  def _validation_logs(self, trainer, vb, dev):
+    hp = self._hparams
+    groups = {t: keras_metrics.MetricGroup(topns=self.TOPNS) for t in self.tasks}
+    wgroups = {t: keras_metrics.MetricGroup(topns=self.TOPNS) for t in self.tasks} \
+        if hp.use_weighted_metrics else {}
+    tloss = {t: 0.0 for t in self.tasks}
+    for batch in vb:
+      x, labels, mask, weights = self._unpack(batch, dev)
+      scores = trainer.predict(x, mask=mask, labels=labels)
+      for t in self.tasks:
+        s = scores[t].clone()
+        groups[t].update_state(labels[t], s)
+        if t in wgroups:
+          wgroups[t].update_state(labels[t], s, weights)
+        tloss[t] += float(trainer.losses[t](labels[t], s, weights))
+    logs = {}
+    total = 0.0
+    for i, t in enumerate(self.tasks):
+      for prefix, gs in (('_metric/', groups), ('_weighted_metric/', wgroups)):
+        if t not in gs:
+          continue
+        gs[t].all_reduce(trainer.group)
+        for key, v in gs[t].result().items():
+          if key.startswith('metric/ndcg'):
+            logs[t + prefix + key[len('metric/'):]] = v
+      logs[t + '_loss'] = tloss[t] / max(len(vb), 1)
+      total += trainer.loss_weights[i] * logs[t + '_loss']
+    logs['loss'] = total
+    return logs

@@ -168,6 +168,135 @@ class RankingTrainer(object):
     return self.scores
 
 
+_MAX_TASKS = 8
+
+
+class MultiTaskRankingTrainer(RankingTrainer):
+  """Fused step for several ranking tasks on one tower (the reference's multi-task
+  `UnivariateScorer` with `MultiTaskPipeline`'s per-task losses and `loss_weights`,
+  keras/model.py:755-777 and keras/pipeline.py:733-824).
+
+  `losses` is an ordered dict task -> `ranking_b200.keras.losses` object; dict order is the
+  order of the tower's output units, so `tower.output_units == len(losses)`.  `loss_weights`
+  maps tasks to weights (missing: 1.0).  One step is
+
+      tfr_mlp_fwd_tasks          task-major score planes [T, B, N], RestoreList on each
+      loss_t.fused_fwd_bwd       one per task, on plane t, into dscore plane t
+      tfr_mlp_bwd_tasks          output-layer backward applies w_t as it reads plane t
+      optimizer / all-reduce     as RankingTrainer
+
+  and returns sum_t w_t L_t (each L_t reduced by its own loss's reduction), the Keras
+  compile-time `loss_weights` semantics, as a 0-d device tensor; `task_losses` holds the
+  [T] per-task values of the last step."""
+
+  def __init__(self, tower, losses, loss_weights=None, **kw):
+    losses = dict(losses)
+    if not losses:
+      raise ValueError('losses must name at least one task')
+    if len(losses) > _MAX_TASKS:
+      raise ValueError('at most %d tasks, got %d' % (_MAX_TASKS, len(losses)))
+    for name, loss in losses.items():
+      if not getattr(loss, 'fused_single_score', False):
+        raise ValueError('task %r: %s has no single-score fused step' %
+                         (name, type(loss).__name__))
+    weights = dict(loss_weights or {})
+    unknown = sorted(set(weights) - set(losses))
+    if unknown:
+      raise ValueError('loss_weights name unknown tasks %s (tasks: %s)' %
+                       (unknown, list(losses)))
+    if tower.output_units != len(losses):
+      raise ValueError('the tower has %d output units for %d tasks' %
+                       (tower.output_units, len(losses)))
+    if tower._precision not in (_C.PREC_FP32, _C.PREC_TF32X3, _C.PREC_TF32):
+      raise ValueError('multi-task towers need precision fp32, tf32x3 or tf32')
+    self.tasks = list(losses)
+    self.losses = losses
+    self.loss_weights = [float(weights.get(t, 1.0)) for t in self.tasks]
+    if not all(w == w and abs(w) != float('inf') for w in self.loss_weights):
+      raise ValueError('loss weights must be finite: %s' % self.loss_weights)
+    super().__init__(tower, losses[self.tasks[0]], **kw)
+    t = len(self.tasks)
+    self._w_host = (ctypes.c_float * t)(*self.loss_weights)
+    # tfr_weighted_sum over the [T, 2] task totals {L_t, sum of weights}: (w_t, 0) pairs
+    self._w_pairs = torch.tensor([[w, 0.0] for w in self.loss_weights], dtype=torch.float32,
+                                 device=self.device).reshape(-1)
+    self.total2 = torch.zeros(2, dtype=torch.float32, device=self.device)
+
+  def _ensure(self, b, n):
+    if self._shape == (b, n):
+      return
+    t, dev = len(self.tasks), self.device
+    self.scores = torch.empty(t, b, n, dtype=torch.float32, device=dev)
+    self.dscores = torch.empty(t, b, n, dtype=torch.float32, device=dev)
+    self.per_list = torch.empty(t, 2, b, dtype=torch.float32, device=dev)
+    self.task_totals = torch.zeros(t, 2, dtype=torch.float32, device=dev)
+    self.task_losses = self.task_totals[:, 0]
+    self.ws = self._new_workspace(b, n)
+    self._shape = (b, n)
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    t = self.tower
+    _C.check(_C.lib.tfr_mlp_fwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data), _C.ptr(m8),
+                                      _C.ptr(self.ws), _C.ptr(self.scores), t._precision,
+                                      _C.stream()))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    t = self.tower
+    _C.check(_C.lib.tfr_mlp_bwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data),
+                                      _C.ptr(self.dscores), self._w_host, _C.ptr(m8),
+                                      _C.ptr(self.ws), _C.ptr(grads), t._precision,
+                                      _C.stream()))
+
+  def _labels(self, labels):
+    missing = [t for t in self.tasks if t not in labels]
+    if missing or len(labels) != len(self.tasks):
+      raise ValueError('labels must map exactly the tasks %s (got %s)' %
+                       (self.tasks, sorted(labels)))
+    return [labels[t] for t in self.tasks]
+
+  def train_step(self, x, labels, sample_weight=None, mask=None):
+    """x [B, N, D] (device), labels {task: [B, N]} (label < 0: no label for that task),
+    sample_weight [B, N] or [B] shared by the tasks, mask [B, N] the list mask (default: any
+    task has a label >= 0).  Returns sum_t w_t L_t as a 0-d device tensor (no host sync)."""
+    b, n, d = x.shape
+    ys = self._labels(labels)
+    self._ensure(b, n)
+    x = self._prep_x(x)
+    if mask is None:
+      mask = ys[0] >= 0
+      for y in ys[1:]:
+        mask = mask | (y >= 0)
+    m8 = mask.reshape(-1).to(torch.uint8).contiguous()
+    cfg = ctypes.byref(self.tower._run_cfg(training=True))
+    grads = self.reducer.grads() if self.reducer is not None else self.grads
+    self.grads = grads
+    x = self._circular_pad(x, mask)
+    self._forward(x, None, m8, cfg, True)
+    for i, task in enumerate(self.tasks):
+      self.losses[task].fused_fwd_bwd(ys[i], self.scores[i], sample_weight, self.dscores[i],
+                                      self.per_list[i], self.task_totals[i])
+    _C.check(_C.lib.tfr_weighted_sum(_C.ptr(self.task_totals), _C.ptr(self._w_pairs),
+                                     2 * len(self.tasks), 1.0, _C.ptr(self.total2),
+                                     _C.stream()))
+    self._backward(x, m8, cfg, grads)
+    self._apply(grads)
+    return self.total2[0]
+
+  @torch.no_grad()
+  def predict(self, x, mask=None, labels=None):
+    """{task: [B, N] score view}; masked items (`mask`, else items without any label >= 0
+    when `labels` is given) hold ln(1e-10) in every task's plane."""
+    if mask is None and labels is not None:
+      ys = self._labels(labels)
+      mask = ys[0] >= 0
+      for y in ys[1:]:
+        mask = mask | (y >= 0)
+    scores = super().predict(x, mask=mask)
+    return {t: scores[i] for i, t in enumerate(self.tasks)}
+
+
 class GroupwiseRankingTrainer(RankingTrainer):
   """Fused step for groupwise scoring (tfr.model._GroupwiseRankingModel, model.py:273-421):
   `tower` is the group score function over the concatenated member features
