@@ -69,14 +69,18 @@ def attention_logits(x, p, l, heads, h):
   return torch.einsum('bjhd,bihd->bhij', k, q)
 
 
-def forward(x, list_mask, flat, heads, h, layers, rate=0.0, keeps=None, noise_add=None):
+def forward(x, list_mask, flat, heads, h, layers, rate=0.0, keeps=None, noise_add=None,
+            relu_gate=None):
   """x [B, N, D] (float64), list_mask [B, N] bool or None -> [B, N, h].  `keeps` (from
-  keep_masks) applies dropout at `rate`; `noise_add` [B, N, h] is added after the ReLU."""
+  keep_masks) applies dropout at `rate`; `noise_add` [B, N, h] is added after the ReLU.
+  `relu_gate` [B, N, h] ({0, 1}), when given, multiplies the input projection in place of
+  its ReLU: the gate decisions of a kernel call replayed."""
   b, n, d = x.shape
   p = unflatten(flat, d, h, heads, layers)
   if list_mask is None:
-    list_mask = torch.ones(b, n, dtype=torch.bool)
-  x = torch.relu(x @ p['w_in'] + p['b_in'])
+    list_mask = torch.ones(b, n, dtype=torch.bool, device=x.device)
+  z = x @ p['w_in'] + p['b_in']
+  x = torch.relu(z) if relu_gate is None else z * relu_gate
   if noise_add is not None:
     x = x + noise_add
   to_mask = list_mask.reshape(b, 1, 1, n)
