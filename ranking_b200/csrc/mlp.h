@@ -146,9 +146,10 @@ int mlp_tc_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ld
 // Fused 3xTF32 forward of Dense first_layer .. L (mlp_tc_fused.cu): one persistent kernel,
 // bit-identical to the per-layer walk.  _ok says whether the tower fits it: no BN / dropout /
 // input BN, ReLU or no activation, Dense first_layer at most 256 wide, every later hidden
-// layer at most 128, at most 8 output units, at least one hidden layer.  Expects the
-// parameters already split.
-bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& p, int passes);
+// layer at most 128, at most 8 output units, at least one hidden layer, X and the workspace
+// 16-byte aligned (its operands move by TMA).  Expects the parameters already split.
+bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& p, int passes,
+                         const float* ws);
 int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
                      const float* params, const uint8_t* mask, float* ws, float* scores,
                      cudaStream_t st, bool planar = false);

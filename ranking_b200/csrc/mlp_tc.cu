@@ -179,7 +179,7 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
     rc = split_params(p, params, ws, passes, st);
     if (rc) return rc;
   }
-  if (mlp_tc_fused_fwd_ok(first_layer, X, M, p, passes))
+  if (mlp_tc_fused_fwd_ok(first_layer, X, M, p, passes, ws))
     return mlp_tc_fused_fwd(first_layer, X, M, p, params, mask, ws, scores, st, planar);
   const int L = p.n_dense - 1;
   const float* in = X;
