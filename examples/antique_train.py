@@ -57,6 +57,8 @@ def main():
   ap.add_argument('--num_attention_heads', type=int, default=1)
   ap.add_argument('--head_size', type=int, default=128)
   ap.add_argument('--num_attention_layers', type=int, default=1)
+  ap.add_argument('--din_precision', choices=('fp32', 'tf32'), default='fp32',
+                  help='DocumentInteractionAttention precision: fp32, or tf32 tensor cores')
   args = ap.parse_args()
 
   vocab = data.Vocabulary.from_file(args.vocab_file)
@@ -86,7 +88,7 @@ def main():
   if args.use_document_interaction:
     din = tfr.keras.layers.DocumentInteractionAttention(
         args.num_attention_heads, args.head_size, args.num_attention_layers,
-        dropout=args.dropout_rate, seed=1234)
+        dropout=args.dropout_rate, seed=1234, precision=args.din_precision)
     trainer = tfr.train.DINEmbeddingRankingTrainer(
         tables, features, din, tower, tfr.keras.losses.get(args.loss), **kw)
   else:

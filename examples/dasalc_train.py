@@ -54,6 +54,8 @@ def main():
   ap.add_argument('--num_attention_heads', type=int, default=2)
   ap.add_argument('--head_size', type=int, default=100)
   ap.add_argument('--seed', type=int, default=1234)
+  ap.add_argument('--din_precision', choices=('fp32', 'tf32'), default='fp32',
+                  help='DocumentInteractionAttention precision: fp32, or tf32 tensor cores')
   args = ap.parse_args()
 
   d = args.num_features
@@ -79,7 +81,8 @@ def main():
 
   din = tfr.keras.layers.DocumentInteractionAttention(
       args.num_attention_heads, args.head_size, args.num_attention_layers,
-      dropout=args.dropout_rate, input_noise_stddev=args.input_noise_stddev, seed=args.seed)
+      dropout=args.dropout_rate, input_noise_stddev=args.input_noise_stddev, seed=args.seed,
+      precision=args.din_precision)
   scorer = dasalc.DASALCScorer(d, args.hidden_layer_dims, args.head_size,
                                dropout=args.dropout_rate,
                                input_noise_stddev=args.input_noise_stddev,

@@ -42,6 +42,8 @@ def main():
   ap.add_argument('--num_heads', type=int, default=2)
   ap.add_argument('--head_size', type=int, default=64)
   ap.add_argument('--num_layers', type=int, default=2)
+  ap.add_argument('--din_precision', choices=('fp32', 'tf32'), default='fp32',
+                  help='DocumentInteractionAttention precision: fp32, or tf32 tensor cores')
   args = ap.parse_args()
 
   hidden = [int(h) for h in args.hidden_layer_dims.split(',')]
@@ -56,7 +58,8 @@ def main():
                                           learning_rate=args.learning_rate)
   elif args.scorer == 'din':
     din = tfr.keras.layers.DocumentInteractionAttention(
-        args.num_heads, args.head_size, args.num_layers, dropout=args.dropout_rate)
+        args.num_heads, args.head_size, args.num_layers, dropout=args.dropout_rate,
+        precision=args.din_precision)
     din.build(args.num_features)
     tower = tfr.keras.layers.create_tower(
         hidden, 1, activation='relu', use_batch_norm=True, dropout=args.dropout_rate,

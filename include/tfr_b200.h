@@ -494,6 +494,13 @@ int tfr_mlp_bwd_tasks(const void* X, int M, const tfr_mlp_cfg* cfg, const float*
  *                   e = ((b * H + head) * N + i) * N + j
  *   site 3 + 2 l    output dropout of layer l, element e = m * h + c
  *   an element is dropped iff u < dropout; kept values are scaled by 1 / (1 - dropout).
+ * Precision (tfr_din_cfg.precision):
+ *   TFR_PREC_FP32   (0, a zeroed struct)  projection GEMMs and input gradient in 3xTF32,
+ *                   attention core (q.k, P~ v and their backward) in FP32 CUDA-core FMA
+ *   TFR_PREC_TF32                         projection GEMMs and input gradient in one TF32
+ *                   pass, attention core on wgmma TF32 (operands truncated to TF32, fp32
+ *                   accumulate); softmax, masking and dropout in fp32 with the same draws
+ *   any other value: TFR_INVALID_ARGUMENT.  The workspace is the same in both.
  * Limits (TFR_INVALID_ARGUMENT before any CUDA call): D % 4 == 0, h % 4 == 0, h <= 128,
  * 1 <= H * h <= 512, 1 <= L <= 8, N <= 1024.  Two identical calls give identical bits.
  * ------------------------------------------------------------------------- */
@@ -510,6 +517,7 @@ typedef struct {
   float input_noise_stddev;     /* sigma; 0 = no GaussianNoise */
   int32_t training;             /* 1: dropout and noise active; 0: inference */
   uint64_t seed;                /* vary per step; same value -> same draws */
+  int32_t precision;            /* TFR_PREC_FP32 (default) or TFR_PREC_TF32 */
 } tfr_din_cfg;
 
 /* 0 when the configuration is out of range (tfr_last_error says why) */
@@ -527,8 +535,8 @@ int tfr_din_bwd(const float* X, const uint8_t* list_mask, int B, int N, const tf
  *   dX[m, c] (row pitch ldx) (=, or += when accumulate) sum_o dZ_in[m, o] W_in[col0 + c, o]
  * dZ_in is the gradient at the input projection's pre-activation, i.e. the ReLU gate of
  * relu(X W_in + b_in) taken before the GaussianNoise.  It is what the preceding tfr_din_bwd
- * (same X, list_mask, B, N, cfg, params, workspace) left in the workspace.  One 3xTF32 GEMM
- * (K = h) in column chunks of at most 3 H h; with accumulate = 1 each chunk goes through the
+ * (same X, list_mask, B, N, cfg, params, workspace) left in the workspace.  One GEMM (K = h;
+ * 3xTF32, or TF32 under TFR_PREC_TF32) in column chunks of at most 3 H h; with accumulate = 1 each chunk goes through the
  * workspace's scratch and is then added, so the result is exactly fp32(dX + G) with G the
  * accumulate = 0 result.  Never writes dZ_in: several windows can be taken, in any order, and
  * tfr_din_bwd's gradients are the same with or without this call.  Two identical calls give

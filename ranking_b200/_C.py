@@ -83,7 +83,7 @@ class DinCfg(C.Structure):
   _fields_ = [('input_dim', C.c_int32), ('head_size', C.c_int32), ('num_heads', C.c_int32),
               ('num_layers', C.c_int32), ('dropout', C.c_float),
               ('input_noise_stddev', C.c_float), ('training', C.c_int32),
-              ('seed', C.c_uint64)]
+              ('seed', C.c_uint64), ('precision', C.c_int32)]
 
 
 class DasalcCfg(C.Structure):

@@ -20,9 +20,12 @@
 // gradients go through the 3xTF32 engine's split-K partials and fixed-order reductions.
 // The input gradient (tfr_din_input_grad) is one more 3xTF32 GEMM, dX = dZ_in W_in^T, over the
 // dZ_in the backward leaves in the workspace.
+// precision TFR_PREC_TF32 runs every projection GEMM above in one TF32 pass instead of three,
+// and the attention core on the tensor cores (din_tc.cu); the workspace is the same.
 #include <cstring>
 
 #include "common.cuh"
+#include "din.cuh"
 #include "mlp.h"
 #include "tc_gemm.cuh"
 
@@ -33,13 +36,14 @@ constexpr int kThreads = 256;
 constexpr int kRows = kThreads / 4;   // query (or key) rows per pass of a CTA
 constexpr int kKT = 32;               // items per shared-memory tile
 constexpr int kMaxH = 128;
-constexpr float kMaskAdder = -1e9f;   // Keras Softmax's adder for masked logits
 constexpr float kLnEps = 1e-12f;
 
 struct DinPlan {
   int D, h, H, L, HH, B, N, M;
   float drop, noise;
   int training;
+  int passes;   // of every projection GEMM: 3 (3xTF32) or 1 (TF32)
+  bool tc;      // attention core on the TF32 tensor cores (din_tc.cu) instead of FP32 SIMT
   unsigned long long seed;
   size_t layer_off[TFR_DIN_MAX_LAYERS], layer_size, n_params;
   // workspace (floats)
@@ -79,12 +83,17 @@ int make_din_plan(const tfr_din_cfg* c, int B, int N, DinPlan* p) {
   TFR_REQUIRE(c->input_noise_stddev >= 0.f, "input_noise_stddev must be >= 0");
   TFR_REQUIRE(B >= 0 && N >= 0, "batch and list size must be >= 0");
   TFR_REQUIRE(N <= TFR_DIN_MAX_LIST, "list_size %d exceeds %d", N, TFR_DIN_MAX_LIST);
+  TFR_REQUIRE(c->precision == TFR_PREC_FP32 || c->precision == TFR_PREC_TF32,
+              "precision %d must be TFR_PREC_FP32 (%d) or TFR_PREC_TF32 (%d)", c->precision,
+              TFR_PREC_FP32, TFR_PREC_TF32);
   std::memset(p, 0, sizeof(*p));
   p->D = c->input_dim; p->h = c->head_size; p->H = c->num_heads; p->L = c->num_layers;
   p->HH = p->H * p->h;
   p->B = B; p->N = N; p->M = B * N;
   p->drop = c->dropout; p->noise = c->input_noise_stddev;
   p->training = c->training != 0; p->seed = c->seed;
+  p->tc = c->precision == TFR_PREC_TF32;
+  p->passes = p->tc ? 1 : 3;
   const int h = p->h, HH = p->HH;
   const size_t M = (size_t)p->M;
   size_t off = (size_t)p->D * h + h;
@@ -131,15 +140,6 @@ int make_din_plan(const tfr_din_cfg* c, int B, int N, DinPlan* p) {
   p->cs_off = w; w += (size_t)p->splits * p->cs_stride;
   p->ws_floats = w;
   return TFR_OK;
-}
-
-// Counter-based uniform in [0, 1): splitmix64 of (site seed, element), as the tower's dropout.
-__device__ __forceinline__ float din_uniform(unsigned long long s, unsigned long long e) {
-  unsigned long long z = s + 0x9E3779B97F4A7C15ull * (e + 1);
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  z ^= z >> 31;
-  return (float)(z >> 40) * (1.0f / 16777216.0f);
 }
 
 __host__ __device__ inline unsigned long long site_seed(unsigned long long seed, int site) {
@@ -548,14 +548,15 @@ add_mask_kernel(const float* __restrict__ tmp, const float* __restrict__ a0, siz
 
 unsigned blocks_for(size_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
-// 3xTF32 GEMM C = A B (+ bias, act), B split on the fly.
+// 3xTF32 (passes 3, B split on the fly) or TF32 (passes 1) GEMM C = A B (+ bias, act).
 int gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, float* C,
-         int ldc, int GM, int GN, int GK, const float* bias, int act, cudaStream_t st) {
+         int ldc, int GM, int GN, int GK, const float* bias, int act, int passes,
+         cudaStream_t st) {
   tc::GemmDesc g{};
   g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.B_lo = nullptr;
   g.C = C; g.ldc = ldc;
   g.GM = GM; g.GN = GN; g.GK = GK;
-  g.a_mn = a_mn; g.b_mn = b_mn; g.passes = 3; g.split_b = 1;
+  g.a_mn = a_mn; g.b_mn = b_mn; g.passes = passes; g.split_b = 1;
   g.epi = bias ? tc::EPI_BIAS_ACT : tc::EPI_STORE;
   g.bias = bias; g.act = act;
   g.splits = 1;
@@ -569,8 +570,8 @@ int gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, f
 int weight_grad(const DinPlan& p, float* ws, const float* A, int lda, int Kin, const float* dZ,
                 int ldz, int Nout, const float* colsum_src, float* grads_w, cudaStream_t st) {
   return mlp_tc_weight_grad(A, lda, Kin, dZ, ldz, Nout, p.M, p.splits, ws + p.part_off,
-                            p.part_stride, colsum_src, p.splits, p.cs_stride, true, grads_w, 3,
-                            st);
+                            p.part_stride, colsum_src, p.splits, p.cs_stride, true, grads_w,
+                            p.passes, st);
 }
 
 template <int KD>
@@ -611,7 +612,7 @@ int din_fwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
   pack_qkv_kernel<<<dim3(32, p.L), 256, 0, st>>>(params, p, ws);
   TFR_LAUNCH_OK();
   int rc = gemm(X, p.D, 0, params, h, 1, ws + p.a0_off, h, M, h, p.D, params + (size_t)p.D * h,
-                TFR_ACT_RELU, st);
+                TFR_ACT_RELU, p.passes, st);
   if (rc) return rc;
   if (p.noisy()) {
     noise_kernel<<<blocks_for((size_t)M * h, 256), 256, 0, st>>>(
@@ -624,14 +625,16 @@ int din_fwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     const float* wqkv = ws + p.wqkv_off + l * p.wqkv_stride;
     float* qkv = ws + p.qkv_off[l];
     rc = gemm(xl, h, 0, wqkv, 3 * HH, 1, qkv, 3 * HH, M, 3 * HH, h, wqkv + (size_t)h * 3 * HH,
-              TFR_ACT_NONE, st);
+              TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
-    rc = TFR_DIN_DISPATCH(attn_fwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
-                          ws + p.o_off[l], ws + p.lse_off[l], st);
+    rc = p.tc ? din_tc_attn_fwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
+                                ws + p.o_off[l], ws + p.lse_off[l], st)
+              : TFR_DIN_DISPATCH(attn_fwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
+                                 ws + p.o_off[l], ws + p.lse_off[l], st);
     if (rc) return rc;
     float* y = ws + p.xh_off[l];
     rc = gemm(ws + p.o_off[l], HH, 0, params + p.wo(l), h, 1, y, h, M, h, HH, params + p.bo(l),
-              TFR_ACT_NONE, st);
+              TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
     const bool last = l + 1 == p.L;
     ln_fwd_kernel<<<blocks_for(M, 8), 256, 0, st>>>(
@@ -669,11 +672,16 @@ int din_bwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     if (rc) return rc;
     rc = weight_grad(p, ws, ws + p.o_off[l], HH, HH, dy, h, h, cs, grads + p.wo(l), st);
     if (rc) return rc;
-    rc = gemm(dy, h, 0, params + p.wo(l), h, 0, dO, HH, M, HH, h, nullptr, TFR_ACT_NONE, st);
+    rc = gemm(dy, h, 0, params + p.wo(l), h, 0, dO, HH, M, HH, h, nullptr, TFR_ACT_NONE, p.passes,
+              st);
     if (rc) return rc;
     const float* qkv = ws + p.qkv_off[l];
-    rc = TFR_DIN_DISPATCH(attn_bwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
-                          ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv, st);
+    rc = p.tc ? din_tc_attn_bwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
+                                ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv,
+                                st)
+              : TFR_DIN_DISPATCH(attn_bwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
+                                 ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv,
+                                 st);
     if (rc) return rc;
     // Q / K / V projections: one dW GEMM each (the flat layout keeps them apart)
     const float* xl = layer_input(p, ws, l);
@@ -686,7 +694,8 @@ int din_bwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     }
     // dX_l = dQKV [Wq | Wk | Wv]^T + residual branch (+ ReLU mask of the input projection)
     const float* wqkv = ws + p.wqkv_off + l * p.wqkv_stride;
-    rc = gemm(dqkv, 3 * HH, 0, wqkv, 3 * HH, 0, tmp, h, M, h, 3 * HH, nullptr, TFR_ACT_NONE, st);
+    rc = gemm(dqkv, 3 * HH, 0, wqkv, 3 * HH, 0, tmp, h, M, h, 3 * HH, nullptr, TFR_ACT_NONE,
+              p.passes, st);
     if (rc) return rc;
     add_mask_kernel<<<blocks_for((size_t)M * h, 256), 256, 0, st>>>(
         tmp, l == 0 ? ws + p.a0_off : nullptr, (size_t)M * h, dres);
@@ -721,7 +730,7 @@ int din_input_grad(const DinPlan& p, const float* params, float* ws, int col0, i
     const int nc = ncols - c0 < chunk ? ncols - c0 : chunk;
     float* out = accumulate ? scratch : dX + c0;
     int rc = gemm(dres, h, 0, params + (size_t)(col0 + c0) * h, h, 0, out, accumulate ? nc : ldx,
-                  p.M, nc, h, nullptr, TFR_ACT_NONE, st);
+                  p.M, nc, h, nullptr, TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
     if (accumulate) {
       add_cols_kernel<<<blocks_for((size_t)p.M * nc, 256), 256, 0, st>>>(scratch, (size_t)p.M,

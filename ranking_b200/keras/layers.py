@@ -18,6 +18,8 @@ _LOG_EPSILON = math.log(1e-10)
 
 _PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32x3': _C.PREC_TF32X3,
                'tf32': _C.PREC_TF32, 'bf16': _C.PREC_BF16}
+# DocumentInteractionAttention builds no 3xTF32 or bf16 attention core
+_DIN_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32}
 
 
 def _activation_enum(activation):
@@ -657,11 +659,17 @@ class DocumentInteractionAttention(torch.nn.Module):
   input dimension comes from the first call (or `build`).  Called as `din((x, list_mask))`;
   `train()` / `eval()` select Keras' `training`.  Gradients flow to the parameters only:
   inputs must not require grad.  Limits: input dim and head_size multiples of 4, head_size
-  <= 128, num_heads * head_size <= 512, num_layers <= 8, list_size <= 1024."""
+  <= 128, num_heads * head_size <= 512, num_layers <= 8, list_size <= 1024.
+
+  `precision`: None / 'fp32' (default) runs the projections in 3xTF32 and the attention core
+  in FP32; 'tf32' runs the projections in one TF32 pass and the attention core on the TF32
+  tensor cores (csrc/din_tc.cu), as TensorFlow's default TF32 matmuls and einsums do.  The
+  parameters are the same in both, so `set_precision` can switch a trained layer."""
 
   def __init__(self, num_heads, head_size, num_layers=1, dropout=0.5, name=None,
-               input_noise_stddev=None, seed=None, device='cuda', **kwargs):
+               input_noise_stddev=None, seed=None, device='cuda', precision=None, **kwargs):
     super().__init__()
+    self.set_precision(precision)
     self.num_heads = int(num_heads)
     self.head_size = int(head_size)
     self.num_layers = int(num_layers)
@@ -683,6 +691,16 @@ class DocumentInteractionAttention(torch.nn.Module):
   def built(self):
     return self._cfg is not None
 
+  def set_precision(self, precision):
+    """None / 'fp32': 3xTF32 projections, FP32 attention core; 'tf32': all on TF32 tensor
+    cores.  Takes effect from the next call."""
+    if precision is None:
+      precision = 'fp32'
+    if precision not in _DIN_PRECISIONS:
+      raise ValueError('precision must be one of %s' % sorted(_DIN_PRECISIONS))
+    self.precision = precision
+    self._precision = _DIN_PRECISIONS[precision]
+
   def _make_cfg(self, input_dim):
     cfg = _C.DinCfg()
     cfg.input_dim = int(input_dim)
@@ -693,6 +711,7 @@ class DocumentInteractionAttention(torch.nn.Module):
     cfg.input_noise_stddev = float(self.input_noise_stddev or 0.0)
     cfg.training = 1
     cfg.seed = 0
+    cfg.precision = self._precision
     return cfg
 
   def build(self, input_dim):
@@ -740,6 +759,7 @@ class DocumentInteractionAttention(torch.nn.Module):
     ctypes.memmove(ctypes.byref(cfg), ctypes.byref(self._cfg), ctypes.sizeof(cfg))
     training = self.training if training is None else training
     cfg.training = int(bool(training))
+    cfg.precision = self._precision
     if training and (self.dropout > 0 or self.input_noise_stddev):
       self._calls += 1
     cfg.seed = (self._base << 32) | (self._calls & 0xFFFFFFFF)
@@ -772,9 +792,12 @@ class DocumentInteractionAttention(torch.nn.Module):
     return _DINFn.apply(x, self.flat, m8, self)
 
   def get_config(self):
-    return {'num_heads': self.num_heads, 'head_size': self.head_size,
-            'num_layers': self.num_layers, 'dropout': self.dropout,
-            'input_noise_stddev': self.input_noise_stddev}
+    cfg = {'num_heads': self.num_heads, 'head_size': self.head_size,
+           'num_layers': self.num_layers, 'dropout': self.dropout,
+           'input_noise_stddev': self.input_noise_stddev}
+    if self.precision != 'fp32':   # the default is left out, as before the option existed
+      cfg['precision'] = self.precision
+    return cfg
 
 
 _COMBINERS = {'sum': _C.COMBINER_SUM, 'mean': _C.COMBINER_MEAN, 'sqrtn': _C.COMBINER_SQRTN}

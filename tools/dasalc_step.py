@@ -9,7 +9,12 @@ latent-cross kernels' times (torch.profiler, in a run of their own) against thei
 bounds; and lists/s of a batched PyTorch autograd formulation of the same model (fp32, TF32
 off, torch.optim.Adagrad) on the same card, with the card's name and power limit.  Needs a
 CUDA device.
-  python tools/dasalc_step.py [--steps 30] [--warmup 5]
+
+--din_precision fp32,tf32 times the trainer with each DocumentInteractionAttention precision
+('cuda', 'cuda_tf32'), and the PyTorch model runs with TF32 off ('pytorch') and on
+('pytorch_tf32'), the arms alternated as in tools/din_step.py; each trainer's attention kernels
+are timed with torch.profiler in a run of their own, against the TF32 data-sheet bound.
+  python tools/dasalc_step.py [--steps 30] [--warmup 5] [--din_precision fp32[,tf32]]
 """
 import argparse
 import ctypes
@@ -23,7 +28,8 @@ sys.path.insert(0, os.path.join(ROOT, 'tools'))
 
 import torch  # noqa: E402
 
-from din_step import card, timed  # noqa: E402
+from din_step import (alternated, attention_flop, attention_kernels, card,  # noqa: E402
+                      set_torch_tf32)
 
 B, N, D, W, HS, H, L = 128, 200, 136, 512, 100, 2, 4
 RATE, NOISE, MOM, LR = 0.4, 1.5, 0.9, 0.05
@@ -38,11 +44,12 @@ def batch(seed):
   return x.cuda(), y.cuda()
 
 
-def cuda_trainer():
+def cuda_trainer(precision='fp32'):
   import ranking_b200 as tfr
   from ranking_b200.research import dasalc
   din = tfr.keras.layers.DocumentInteractionAttention(H, HS, L, dropout=RATE,
-                                                      input_noise_stddev=NOISE, seed=1)
+                                                      input_noise_stddev=NOISE, seed=1,
+                                                      precision=precision)
   sc = dasalc.DASALCScorer(D, W, HS, dropout=RATE, input_noise_stddev=NOISE,
                            batch_norm_moment=MOM, seed=2)
   return tfr.train.DASALCRankingTrainer(din, sc, tfr.keras.losses.get('softmax_loss'),
@@ -202,32 +209,46 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--steps', type=int, default=30)
   ap.add_argument('--warmup', type=int, default=5)
+  ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--din_precision', default='fp32',
+                  help='comma-separated DocumentInteractionAttention precisions: fp32, tf32')
   args = ap.parse_args()
   if not torch.cuda.is_available():
     raise SystemExit('dasalc_step.py needs a CUDA device')
-  torch.backends.cuda.matmul.allow_tf32 = False
-  torch.backends.cudnn.allow_tf32 = False
+  set_torch_tf32(False)
   res = {'shape': {'B': B, 'N': N, 'D': D, 'hidden': W, 'heads': H, 'head_size': HS,
                    'layers': L}}
   res.update(card())
   x, y = batch(0)
-  tr = cuda_trainer()
-  sec = timed(lambda: tr.train_step(x, y), args.steps, args.warmup)
-  ph = phases(tr, x, y, max(20, args.steps))
-  total = sum(ph.values())
-  res['cuda'] = {'lists_per_s': round(B / sec, 1), 'step_ms': round(sec * 1e3, 3),
-                 'timed_steps': args.steps, 'phases_ms': ph,
-                 'din_share': round((ph['din_fwd'] + ph['din_bwd']) / total, 3),
-                 'scorer_share': round((ph['scorer_fwd'] + ph['scorer_bwd']) / total, 3)}
-  res['cross_kernels'] = cross_kernels(tr, x, y, 10)
-  del tr
-  torch.cuda.empty_cache()
+  precs = args.din_precision.split(',')
+  trainers = {p: cuda_trainer(p) for p in precs}
+  key = lambda p: 'cuda' if p == 'fp32' else 'cuda_' + p
+  arms = [(key(p), (lambda tr: lambda: tr.train_step(x, y))(tr), False)
+          for p, tr in trainers.items()]
   try:
     step = torch_step_fn(x, y)
-    ps = timed(step, max(20, args.steps), args.warmup)
-    res['pytorch'] = {'lists_per_s': round(B / ps, 1), 'step_ms': round(ps * 1e3, 3)}
+    arms += [('pytorch', step, False), ('pytorch_tf32', step, True)]
   except torch.cuda.OutOfMemoryError:
     res['pytorch'] = 'out of memory'
+  secs = alternated(arms, args.steps, args.warmup, args.rounds)
+  afwd, abwd = attention_flop(B, N, H, HS, L)
+  for p, tr in trainers.items():
+    sec = secs[key(p)]
+    ph = phases(tr, x, y, max(20, args.steps))
+    total = sum(ph.values())
+    res[key(p)] = {'lists_per_s': round(B / sec, 1), 'step_ms': round(sec * 1e3, 3),
+                   'timed_steps': args.steps * args.rounds, 'phases_ms': ph,
+                   'din_share': round((ph['din_fwd'] + ph['din_bwd']) / total, 3),
+                   'scorer_share': round((ph['scorer_fwd'] + ph['scorer_bwd']) / total, 3),
+                   'attention_gflop': {'fwd': round(afwd / 1e9, 1), 'bwd': round(abwd / 1e9, 1)},
+                   'attention_kernels': attention_kernels(lambda: tr.train_step(x, y), 10,
+                                                          afwd, abwd)}
+    if p == 'fp32':
+      res['cross_kernels'] = cross_kernels(tr, x, y, 10)
+  for name in ('pytorch', 'pytorch_tf32'):
+    if name in secs:
+      res[name] = {'lists_per_s': round(B / secs[name], 1),
+                   'step_ms': round(secs[name] * 1e3, 3)}
   print(json.dumps(res))
 
 

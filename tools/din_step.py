@@ -9,7 +9,14 @@ gradient, DIN backward, optimizer), also with CUDA events; algorithmic FLOPs and
 the FP32 data-sheet rate and HBM bandwidth; and lists/s of a batched PyTorch autograd
 formulation of the same model (einsum projections, scaled_dot_product_attention, layer_norm,
 fp32 with TF32 off, torch.optim.Adagrad) on the same card.  Needs a CUDA device.
-  python tools/din_step.py [--steps 30] [--warmup 5]
+
+--din_precision fp32,tf32 times the trainer with each DocumentInteractionAttention precision
+('cuda', 'cuda_tf32'), and the PyTorch model runs with TF32 off ('pytorch') and on
+('pytorch_tf32', torch.backends.cuda.matmul / cudnn allow_tf32): every arm is warmed up, then
+the arms take turns for --rounds rounds of --steps steps.  Each trainer's attention kernels
+are then timed with torch.profiler, in a run of its own, against the TF32 data-sheet bound of
+their FLOPs.
+  python tools/din_step.py [--steps 30] [--warmup 5] [--din_precision fp32[,tf32]]
 """
 import argparse
 import ctypes
@@ -61,9 +68,66 @@ def timed(step, steps, warmup):
   return t0.elapsed_time(t1) / 1e3 / steps
 
 
-def cuda_trainer():
+def set_torch_tf32(on):
+  torch.backends.cuda.matmul.allow_tf32 = on
+  torch.backends.cudnn.allow_tf32 = on
+
+
+def alternated(arms, steps, warmup, rounds):
+  """{name: s per step} of arms [(name, step, torch_tf32)]: each warmed up, then `rounds`
+  rounds in which every arm runs `steps` timed steps in turn."""
+  for _, step, tf32 in arms:
+    set_torch_tf32(tf32)
+    for _ in range(warmup):
+      step()
+  tot = {name: 0.0 for name, _, _ in arms}
+  for _ in range(rounds):
+    for name, step, tf32 in arms:
+      set_torch_tf32(tf32)
+      tot[name] += timed(step, steps, 0) / rounds
+  set_torch_tf32(False)
+  return tot
+
+
+ATTENTION_KERNELS = ('attn_fwd_kernel', 'attn_bwd_dq_kernel', 'attn_bwd_dkv_kernel',
+                     'attn_fwd_tc_kernel', 'attn_bwd_dq_tc_kernel', 'attn_bwd_dkv_tc_kernel')
+
+
+def attention_flop(b, n, heads, hs, layers):
+  """Forward (q.k, P~ v) and backward (S and dP in both passes, dQ, dK, dV) FLOPs."""
+  one = 2.0 * b * heads * n * n * hs * layers
+  return 2 * one, 7 * one
+
+
+def attention_kernels(step, steps, fwd_flop, bwd_flop):
+  """ms per training step of the DIN's attention kernels (torch.profiler, CUDA activities,
+  `steps` steps) and their share of the TF32 data-sheet bound of the attention FLOPs."""
+  from torch.profiler import ProfilerActivity, profile
+  for _ in range(3):
+    step()
+  torch.cuda.synchronize()
+  with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(steps):
+      step()
+    torch.cuda.synchronize()
+  us = dict.fromkeys(ATTENTION_KERNELS, 0.0)
+  for evt in prof.events():
+    for k in ATTENTION_KERNELS:
+      if k + '<' in evt.name and evt.device_time > 0:
+        us[k] += evt.device_time / steps
+  fwd = sum(v for k, v in us.items() if 'fwd' in k)
+  bwd = sum(v for k, v in us.items() if 'bwd' in k)
+  out = {k: round(v / 1e3, 3) for k, v in us.items() if v > 0}
+  out['fwd_ms'], out['bwd_ms'] = round(fwd / 1e3, 3), round(bwd / 1e3, 3)
+  out['fwd_share_of_tf32_bound'] = round(fwd_flop / TF32_PEAK * 1e6 / fwd, 4) if fwd else None
+  out['bwd_share_of_tf32_bound'] = round(bwd_flop / TF32_PEAK * 1e6 / bwd, 4) if bwd else None
+  return out
+
+
+def cuda_trainer(precision='fp32'):
   import ranking_b200 as tfr
-  din = tfr.keras.layers.DocumentInteractionAttention(H, HS, L, dropout=0.0, seed=1).build(D)
+  din = tfr.keras.layers.DocumentInteractionAttention(H, HS, L, dropout=0.0, seed=1,
+                                                      precision=precision).build(D)
   tower = tfr.keras.layers.create_tower(HIDDEN, 1, activation='relu', use_batch_norm=False,
                                         dropout=0, input_dim=D + HS, seed=2,
                                         precision='tf32x3')
@@ -190,37 +254,50 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--steps', type=int, default=30)
   ap.add_argument('--warmup', type=int, default=5)
+  ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--din_precision', default='fp32',
+                  help='comma-separated DocumentInteractionAttention precisions: fp32, tf32')
   args = ap.parse_args()
   if not torch.cuda.is_available():
     raise SystemExit('din_step.py needs a CUDA device')
-  torch.backends.cuda.matmul.allow_tf32 = False
-  torch.backends.cudnn.allow_tf32 = False
+  set_torch_tf32(False)
   res = {'shape': {'B': B, 'N': N, 'D': D, 'heads': H, 'head_size': HS, 'layers': L,
                    'tower': HIDDEN}}
   res.update(card())
   x, y = batch(0)
-  tr = cuda_trainer()
-  sec = timed(lambda: tr.train_step(x, y), args.steps, args.warmup)
-  gemm_flop, attn_flop, byts = work()
-  t_min = max(gemm_flop / (TF32_PEAK / 3) + attn_flop / FP32_PEAK, byts / HBM_BW)
-  res['cuda'] = {'lists_per_s': round(B / sec, 1), 'step_ms': round(sec * 1e3, 3),
-                 'timed_steps': args.steps,
-                 'gemm_gflop': round(gemm_flop / 1e9, 1),
-                 'attention_gflop': round(attn_flop / 1e9, 1),
-                 'bytes_gb': round(byts / 1e9, 2),
-                 'compute_bound_ms': round((gemm_flop / (TF32_PEAK / 3) +
-                                            attn_flop / FP32_PEAK) * 1e3, 3),
-                 'hbm_bound_ms': round(byts / HBM_BW * 1e3, 3),
-                 'share_of_bound': round(t_min / sec, 4),
-                 'phases_ms': phases(tr, x, y, max(20, args.steps))}
-  del tr
-  torch.cuda.empty_cache()
+  precs = args.din_precision.split(',')
+  trainers = {p: cuda_trainer(p) for p in precs}
+  key = lambda p: 'cuda' if p == 'fp32' else 'cuda_' + p
+  arms = [(key(p), (lambda tr: lambda: tr.train_step(x, y))(tr), False)
+          for p, tr in trainers.items()]
   try:
     step = torch_step_fn(x, y)
-    ps = timed(step, max(20, args.steps), args.warmup)
-    res['pytorch'] = {'lists_per_s': round(B / ps, 1), 'step_ms': round(ps * 1e3, 3)}
+    arms += [('pytorch', step, False), ('pytorch_tf32', step, True)]
   except torch.cuda.OutOfMemoryError:
     res['pytorch'] = 'out of memory'
+  secs = alternated(arms, args.steps, args.warmup, args.rounds)
+  gemm_flop, attn_flop, byts = work()
+  afwd, abwd = attention_flop(B, N, H, HS, L)
+  for p, tr in trainers.items():
+    sec = secs[key(p)]
+    gemm_rate = TF32_PEAK if p == 'tf32' else TF32_PEAK / 3
+    attn_rate = TF32_PEAK if p == 'tf32' else FP32_PEAK
+    bound = gemm_flop / gemm_rate + attn_flop / attn_rate
+    res[key(p)] = {'lists_per_s': round(B / sec, 1), 'step_ms': round(sec * 1e3, 3),
+                   'timed_steps': args.steps * args.rounds,
+                   'gemm_gflop': round(gemm_flop / 1e9, 1),
+                   'attention_gflop': round(attn_flop / 1e9, 1),
+                   'bytes_gb': round(byts / 1e9, 2),
+                   'compute_bound_ms': round(bound * 1e3, 3),
+                   'hbm_bound_ms': round(byts / HBM_BW * 1e3, 3),
+                   'share_of_bound': round(max(bound, byts / HBM_BW) / sec, 4),
+                   'phases_ms': phases(tr, x, y, max(20, args.steps)),
+                   'attention_kernels': attention_kernels(lambda: tr.train_step(x, y), 10,
+                                                          afwd, abwd)}
+  for name in ('pytorch', 'pytorch_tf32'):
+    if name in secs:
+      res[name] = {'lists_per_s': round(B / secs[name], 1),
+                   'step_ms': round(secs[name] * 1e3, 3)}
   print(json.dumps(res))
 
 
