@@ -607,6 +607,86 @@ int tfr_dasalc_bwd(const float* X, int M, const tfr_dasalc_cfg* cfg, const float
 int tfr_symmetric_log1p_clip(const float* X, size_t n, float cutoff, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * K15  TFR-BERT (extension/premade/tfrbert_task.py TFRBertScorer over tf-models-official's
+ * BertEncoder).  tf-models is not part of the reference, so the formulas below are the
+ * contract.  S sequences (the items of the lists, flattened) of L tokens each: ids
+ * w[s, t] in [0, V), token mask tau[s, t] in {0, 1} (uint8) and type ids k[s, t] in [0, T_v),
+ * int32 / uint8 [S, L] row-major.  E = hidden_size, H heads of dh = E / H, I = intermediate.
+ *   x0[s, t] = dropout_h(LN_e(Word[w] + Pos[t] + Type[k]))
+ *   per layer (post-LN):
+ *     [q | k | v] = x Wqkv + bqkv                        heads contiguous in each block, as the
+ *                                                        DIN's
+ *     P   = softmax_j(q_i . k_j / sqrt(dh) - 1e9 (1 - tau_j))   (the DIN's rule: a sequence with
+ *           no valid token attends 1/L to every token)
+ *     o   = dropout_a(P) v,  y = o Wo + bo,  x' = LN_1(dropout_h(y) + x)
+ *     u   = x' W1 + b1,  a = gelu(u) = 0.5 u (1 + tanh(sqrt(2/pi) (u + 0.044715 u^3)))
+ *     x'' = LN_2(dropout_h(a W2 + b2) + x')
+ *   pooled[s] = tanh(x_L[s, 0] Wp + bp)                  ([CLS] row)
+ *   score[s]  = dropout_s(pooled[s]) . w_s + b_s          (TFRBertScorer: Dropout + Dense(1))
+ * Every LayerNorm: (z - mean) / sqrt(var + 1e-12) * gamma + beta, population variance.
+ * Flat parameter layout (floats, in this order; gradients use the same):
+ *   word [V, E], position [max_position, E], type [T_v, E], gamma_e [E], beta_e [E],
+ *   per layer: Wqkv [E, 3E] (columns: q, then k, then v), bqkv [3E], Wo [E, E], bo [E],
+ *              gamma_1 [E], beta_1 [E], W1 [E, I], b1 [I], W2 [I, E], b2 [E], gamma_2 [E],
+ *              beta_2 [E],
+ *   Wp [E, E], bp [E], w_s [E], b_s [1].
+ *   Kernels are [in, out] row-major (Keras Dense kernels).
+ * Random draws (training only), with u(s, e) the tower's counter hash (see K11) and site seeds
+ * s = seed * 0x100000001B3 + site; an element is dropped iff u < rate, kept values are scaled
+ * by 1 / (1 - rate):
+ *   site 1           dropout_h of the embedding output, element e = m * E + c (m = s L + t)
+ *   site 2 + 3 l     dropout_a of layer l, e = ((s H + head) L + i) L + j
+ *   site 3 + 3 l     dropout_h of layer l's attention output y, e = m * E + c
+ *   site 4 + 3 l     dropout_h of layer l's FFN output, e = m * E + c
+ *   site 2 + 3 NL    dropout_s of the pooled vector, e = s * E + c
+ * Out-of-range ids (w outside [0, V), k outside [0, T_v)) add no row in the forward, get no
+ * gradient, and are counted into *bad_ids (an int device counter, optional) by the forward.
+ * Precision (tfr_bert_cfg.precision): TFR_PREC_FP32 (0, a zeroed struct) runs every GEMM in
+ * 3xTF32 and the attention core in FP32 CUDA-core FMA; TFR_PREC_TF32 runs the GEMMs in one
+ * TF32 pass and the attention core on wgmma TF32 (as tfr_din_cfg).  LayerNorm, GELU, softmax,
+ * masking, dropout and the head are fp32 in both.
+ * Limits (TFR_INVALID_ARGUMENT before any CUDA call, and 0 from the size queries): dh = E / H
+ * a multiple of 4 in [4, 128], E <= 1024, I a multiple of 4 in [4, 4096], 1 <= layers <= 24,
+ * 1 <= L <= max_position <= 512, 1 <= T_v <= 16, 1 <= V < 2^30, dropout rates in [0, 1),
+ * S >= 0, S * L * max(I, 3E) < 2^31; NULL ids / mask / type ids / params / workspace / scores
+ * (and dscores / grads in the backward).  Deterministic: no float atomics, so two identical
+ * calls give identical bits.
+ * ------------------------------------------------------------------------- */
+#define TFR_BERT_MAX_LAYERS 24
+#define TFR_BERT_MAX_HIDDEN 1024
+#define TFR_BERT_MAX_INTERMEDIATE 4096
+#define TFR_BERT_MAX_POSITION 512
+#define TFR_BERT_MAX_TYPES 16
+
+typedef struct {
+  int32_t vocab_size;           /* V */
+  int32_t hidden_size;          /* E */
+  int32_t num_heads;            /* H */
+  int32_t intermediate_size;    /* I */
+  int32_t num_layers;
+  int32_t max_position;         /* rows of the position table */
+  int32_t type_vocab_size;      /* T_v */
+  float hidden_dropout;         /* dropout_h */
+  float attention_dropout;      /* dropout_a */
+  float output_dropout;         /* dropout_s (TFRBertScorer's bert_output_dropout) */
+  int32_t training;             /* 1: dropout active; 0: inference */
+  uint64_t seed;                /* vary per step; same value -> same draws */
+  int32_t precision;            /* TFR_PREC_FP32 (default) or TFR_PREC_TF32 */
+} tfr_bert_cfg;
+
+size_t tfr_bert_param_count(const tfr_bert_cfg* cfg);
+size_t tfr_bert_workspace_bytes(const tfr_bert_cfg* cfg, int S, int L);
+/* scores [S].  The workspace keeps what tfr_bert_bwd needs. */
+int tfr_bert_fwd(const int32_t* word_ids, const uint8_t* input_mask, const int32_t* type_ids,
+                 int S, int L, const tfr_bert_cfg* cfg, const float* params, void* workspace,
+                 float* scores, int* bad_ids, void* stream);
+/* dscores [S] -> grads (flat, parameter layout; every element written).  Must follow a
+ * tfr_bert_fwd with the same inputs, cfg, params and workspace. */
+int tfr_bert_bwd(const int32_t* word_ids, const uint8_t* input_mask, const int32_t* type_ids,
+                 int S, int L, const tfr_bert_cfg* cfg, const float* params,
+                 const float* dscores, void* workspace, float* grads, void* stream);
+
+/* ---------------------------------------------------------------------------
  * K12  pooled embedding bags (tf.feature_column.embedding_column over a categorical column;
  * Keras Embedding + a reduction over the token axis).  ids [R, T] int32, table [V, E] fp32.
  * Bag r holds the ids ids[r, 0..T) in [0, V); -1 marks an empty slot.  Any other id (< -1 or
@@ -907,6 +987,18 @@ int tfr_ranking_parse_tokens(int format, const uint8_t* const* records,
 int tfr_optimizer_step(float* params, const float* grads, float* accum, size_t n,
                        int kind, float lr, float eps, float grad_scale,
                        void* stream);
+
+/* AdamW, the update of tf-models-official's AdamWeightDecay (BERT's optimizer), over n floats
+ * with m and v the first and second moments (zero before step 1), t = step >= 1:
+ *   g *= grad_scale;  m = beta1 m + (1 - beta1) g;  v = beta2 v + (1 - beta2) g^2
+ *   p -= lr * weight_decay * p                        (elements whose decay_mask byte is
+ *                                                      nonzero; NULL: every element)
+ *   p -= lr * sqrt(1 - beta2^t) / (1 - beta1^t) * m / (sqrt(v) + eps)   (Keras Adam form)
+ * The step factor is formed on the host in double.  TFR_INVALID_ARGUMENT for NULL params /
+ * grads / m / v, step < 1, or beta1 / beta2 outside [0, 1). */
+int tfr_adamw_step(float* params, const float* grads, float* m, float* v,
+                   const uint8_t* decay_mask, size_t n, float lr, float beta1, float beta2,
+                   float eps, float weight_decay, int64_t step, float grad_scale, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K7  data-parallel step: all-reduce(SUM) of the flat gradient fused with the optimizer,

@@ -93,6 +93,15 @@ class DasalcCfg(C.Structure):
               ('seed', C.c_uint64), ('bn_state', C.c_void_p)]
 
 
+class BertCfg(C.Structure):
+  _fields_ = [('vocab_size', C.c_int32), ('hidden_size', C.c_int32), ('num_heads', C.c_int32),
+              ('intermediate_size', C.c_int32), ('num_layers', C.c_int32),
+              ('max_position', C.c_int32), ('type_vocab_size', C.c_int32),
+              ('hidden_dropout', C.c_float), ('attention_dropout', C.c_float),
+              ('output_dropout', C.c_float), ('training', C.c_int32), ('seed', C.c_uint64),
+              ('precision', C.c_int32)]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
@@ -197,6 +206,12 @@ _SIGNATURES = {
     'tfr_allreduce_optimizer_step': (_I, [_P, _P, _I, _I, C.c_uint32, _P, _P, _P, C.c_size_t,
                                           _I, _F, _F, _F, _P]),
     'tfr_optimizer_step': (_I, [_P, _P, _P, C.c_size_t, _I, _F, _F, _F, _P]),
+    'tfr_adamw_step': (_I, [_P, _P, _P, _P, _P, C.c_size_t, _F, _F, _F, _F, _F, C.c_int64, _F,
+                            _P]),
+    'tfr_bert_param_count': (C.c_size_t, [C.POINTER(BertCfg)]),
+    'tfr_bert_workspace_bytes': (C.c_size_t, [C.POINTER(BertCfg), _I, _I]),
+    'tfr_bert_fwd': (_I, [_P, _P, _P, _I, _I, C.POINTER(BertCfg), _P, _P, _P, _P, _P]),
+    'tfr_bert_bwd': (_I, [_P, _P, _P, _I, _I, C.POINTER(BertCfg), _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES)

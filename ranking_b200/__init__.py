@@ -20,5 +20,6 @@ from ranking_b200 import train
 from ranking_b200 import data
 from ranking_b200 import pipeline
 from ranking_b200 import research
+from ranking_b200 import extension
 
 __version__ = '0.1.0'

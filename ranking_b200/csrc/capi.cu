@@ -202,6 +202,23 @@ optimizer_kernel(float* __restrict__ params, const float* __restrict__ grads,
   }
 }
 
+
+// AdamWeightDecay; step_size = lr sqrt(1 - beta2^t) / (1 - beta1^t) (host, double).
+__global__ void __launch_bounds__(256)
+adamw_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ m,
+             float* __restrict__ v, const uint8_t* __restrict__ decay_mask, size_t n, float lr,
+             float beta1, float beta2, float eps, float wd, float step_size, float grad_scale) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float g = grads[i] * grad_scale;
+  const float mi = beta1 * m[i] + (1.f - beta1) * g;
+  const float vi = beta2 * v[i] + (1.f - beta2) * g * g;
+  m[i] = mi;
+  v[i] = vi;
+  float p = params[i];
+  if (!decay_mask || decay_mask[i]) p -= lr * wd * p;
+  params[i] = p - step_size * mi / (sqrtf(vi) + eps);
+}
 }  // namespace tfr
 
 using namespace tfr;
@@ -388,6 +405,26 @@ extern "C" int tfr_optimizer_step(float* params, const float* grads, float* accu
   if (n == 0) return TFR_OK;
   optimizer_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       params, grads, accum, n, kind, lr, eps, grad_scale);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" int tfr_adamw_step(float* params, const float* grads, float* m, float* v,
+                              const uint8_t* decay_mask, size_t n, float lr, float beta1,
+                              float beta2, float eps, float weight_decay, int64_t step,
+                              float grad_scale, void* stream) {
+  TFR_REQUIRE(params && grads && m && v, "NULL argument");
+  TFR_REQUIRE(step >= 1, "AdamW step %lld must be >= 1", (long long)step);
+  TFR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f,
+              "beta1 %g and beta2 %g must be in [0, 1)", (double)beta1, (double)beta2);
+  if (n == 0) return TFR_OK;
+  const double t = (double)step;
+  const float step_size =
+      (float)((double)lr * std::sqrt(1.0 - std::pow((double)beta2, t)) /
+              (1.0 - std::pow((double)beta1, t)));
+  adamw_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      params, grads, m, v, decay_mask, n, lr, beta1, beta2, eps, weight_decay, step_size,
+      grad_scale);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

@@ -548,10 +548,57 @@ add_mask_kernel(const float* __restrict__ tmp, const float* __restrict__ a0, siz
 
 unsigned blocks_for(size_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
-// 3xTF32 (passes 3, B split on the fly) or TF32 (passes 1) GEMM C = A B (+ bias, act).
-int gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, float* C,
-         int ldc, int GM, int GN, int GK, const float* bias, int act, int passes,
-         cudaStream_t st) {
+// grads[w .. w + Kin * Nout + Nout) = {A^T dZ, column sums of dZ} over the plan's row splits.
+int weight_grad(const DinPlan& p, float* ws, const float* A, int lda, int Kin, const float* dZ,
+                int ldz, int Nout, const float* colsum_src, float* grads_w, cudaStream_t st) {
+  return din_weight_grad(A, lda, Kin, dZ, ldz, Nout, p.M, p.splits, ws + p.part_off,
+                         p.part_stride, colsum_src, p.cs_stride, grads_w, p.passes, st);
+}
+
+template <int KD>
+int attn_fwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+             unsigned long long s, float* O, float* lse, cudaStream_t st) {
+  attn_fwd_kernel<KD><<<B * H, kThreads, 0, st>>>(qkv, lmask, N, H, h, 1.f / sqrtf((float)h),
+                                                  drop, s, O, lse);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+template <int KD>
+int attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+             unsigned long long s, const float* O, const float* lse, const float* dO,
+             float* dsum, float* dqkv, cudaStream_t st) {
+  const float scale = 1.f / sqrtf((float)h);
+  attn_bwd_dq_kernel<KD><<<B * H, kThreads, 0, st>>>(qkv, lmask, N, H, h, scale, drop, s, O, lse,
+                                                     dO, dsum, dqkv);
+  TFR_LAUNCH_OK();
+  attn_bwd_dkv_kernel<KD><<<B * H, kThreads, 0, st>>>(qkv, lmask, N, H, h, scale, drop, s, lse,
+                                                      dsum, dO, dqkv);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+}  // namespace
+
+#define TFR_DIN_DISPATCH(fn, ...)                                        \
+  (h <= 16 ? fn<4>(__VA_ARGS__) : h <= 32 ? fn<8>(__VA_ARGS__)           \
+   : h <= 64 ? fn<16>(__VA_ARGS__) : fn<32>(__VA_ARGS__))
+
+int din_attn_fwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+                 unsigned long long dseed, float* O, float* lse, cudaStream_t st) {
+  return TFR_DIN_DISPATCH(attn_fwd, qkv, lmask, B, N, H, h, drop, dseed, O, lse, st);
+}
+
+int din_attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+                 unsigned long long dseed, const float* O, const float* lse, const float* dO,
+                 float* dsum, float* dqkv, cudaStream_t st) {
+  return TFR_DIN_DISPATCH(attn_bwd, qkv, lmask, B, N, H, h, drop, dseed, O, lse, dO, dsum, dqkv,
+                          st);
+}
+
+int din_gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, float* C,
+             int ldc, int GM, int GN, int GK, const float* bias, int act, int passes,
+             cudaStream_t st) {
   tc::GemmDesc g{};
   g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.B_lo = nullptr;
   g.C = C; g.ldc = ldc;
@@ -563,43 +610,16 @@ int gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, f
   return tc::gemm(g, st);
 }
 
-// grads[w .. w + Kin * Nout + Nout) = {A^T dZ, column sums of dZ}: A [M, Kin] (ld lda),
-// dZ [M, Nout] (ld ldz), split over M into the plan's row splits, reduced in fixed order.
-// Always in the direct orientation: the tower's fewer-tile-units rule would swap the q / k / v
-// slices at h = 64 with two heads, which changes their rounding.
-int weight_grad(const DinPlan& p, float* ws, const float* A, int lda, int Kin, const float* dZ,
-                int ldz, int Nout, const float* colsum_src, float* grads_w, cudaStream_t st) {
-  return mlp_tc_weight_grad(A, lda, Kin, dZ, ldz, Nout, p.M, p.splits, ws + p.part_off,
-                            p.part_stride, colsum_src, p.splits, p.cs_stride, true, grads_w,
-                            p.passes, st);
+// The tower's fewer-tile-units rule would swap the DIN's q / k / v slices at h = 64 with two
+// heads, which changes their rounding: hence the direct orientation.
+int din_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ldz, int Nout, int M,
+                    int splits, float* partial, size_t pstride, const float* colsum,
+                    size_t cs_stride, float* grads_w, int passes, cudaStream_t st) {
+  return mlp_tc_weight_grad(A, lda, Kin, dZ, ldz, Nout, M, splits, partial, pstride, colsum,
+                            splits, cs_stride, true, grads_w, passes, st);
 }
 
-template <int KD>
-int attn_fwd(const DinPlan& p, const float* qkv, const uint8_t* lmask, float drop,
-             unsigned long long s, float* O, float* lse, cudaStream_t st) {
-  attn_fwd_kernel<KD><<<p.B * p.H, kThreads, 0, st>>>(qkv, lmask, p.N, p.H, p.h,
-                                                      1.f / sqrtf((float)p.h), drop, s, O, lse);
-  TFR_LAUNCH_OK();
-  return TFR_OK;
-}
-
-template <int KD>
-int attn_bwd(const DinPlan& p, const float* qkv, const uint8_t* lmask, float drop,
-             unsigned long long s, const float* O, const float* lse, const float* dO,
-             float* dsum, float* dqkv, cudaStream_t st) {
-  const float scale = 1.f / sqrtf((float)p.h);
-  attn_bwd_dq_kernel<KD><<<p.B * p.H, kThreads, 0, st>>>(qkv, lmask, p.N, p.H, p.h, scale, drop,
-                                                         s, O, lse, dO, dsum, dqkv);
-  TFR_LAUNCH_OK();
-  attn_bwd_dkv_kernel<KD><<<p.B * p.H, kThreads, 0, st>>>(qkv, lmask, p.N, p.H, p.h, scale,
-                                                          drop, s, lse, dsum, dO, dqkv);
-  TFR_LAUNCH_OK();
-  return TFR_OK;
-}
-
-#define TFR_DIN_DISPATCH(fn, ...)                                        \
-  (p.h <= 16 ? fn<4>(__VA_ARGS__) : p.h <= 32 ? fn<8>(__VA_ARGS__)       \
-   : p.h <= 64 ? fn<16>(__VA_ARGS__) : fn<32>(__VA_ARGS__))
+namespace {
 
 const float* layer_input(const DinPlan& p, const float* ws, int l) {
   if (l > 0) return ws + p.xo_off[l - 1];
@@ -611,8 +631,8 @@ int din_fwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
   const int h = p.h, HH = p.HH, M = p.M;
   pack_qkv_kernel<<<dim3(32, p.L), 256, 0, st>>>(params, p, ws);
   TFR_LAUNCH_OK();
-  int rc = gemm(X, p.D, 0, params, h, 1, ws + p.a0_off, h, M, h, p.D, params + (size_t)p.D * h,
-                TFR_ACT_RELU, p.passes, st);
+  int rc = din_gemm(X, p.D, 0, params, h, 1, ws + p.a0_off, h, M, h, p.D,
+                    params + (size_t)p.D * h, TFR_ACT_RELU, p.passes, st);
   if (rc) return rc;
   if (p.noisy()) {
     noise_kernel<<<blocks_for((size_t)M * h, 256), 256, 0, st>>>(
@@ -624,17 +644,17 @@ int din_fwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     const float* xl = layer_input(p, ws, l);
     const float* wqkv = ws + p.wqkv_off + l * p.wqkv_stride;
     float* qkv = ws + p.qkv_off[l];
-    rc = gemm(xl, h, 0, wqkv, 3 * HH, 1, qkv, 3 * HH, M, 3 * HH, h, wqkv + (size_t)h * 3 * HH,
-              TFR_ACT_NONE, p.passes, st);
+    rc = din_gemm(xl, h, 0, wqkv, 3 * HH, 1, qkv, 3 * HH, M, 3 * HH, h,
+                  wqkv + (size_t)h * 3 * HH, TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
     rc = p.tc ? din_tc_attn_fwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
                                 ws + p.o_off[l], ws + p.lse_off[l], st)
-              : TFR_DIN_DISPATCH(attn_fwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
-                                 ws + p.o_off[l], ws + p.lse_off[l], st);
+              : din_attn_fwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
+                             ws + p.o_off[l], ws + p.lse_off[l], st);
     if (rc) return rc;
     float* y = ws + p.xh_off[l];
-    rc = gemm(ws + p.o_off[l], HH, 0, params + p.wo(l), h, 1, y, h, M, h, HH, params + p.bo(l),
-              TFR_ACT_NONE, p.passes, st);
+    rc = din_gemm(ws + p.o_off[l], HH, 0, params + p.wo(l), h, 1, y, h, M, h, HH,
+                  params + p.bo(l), TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
     const bool last = l + 1 == p.L;
     ln_fwd_kernel<<<blocks_for(M, 8), 256, 0, st>>>(
@@ -672,16 +692,15 @@ int din_bwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     if (rc) return rc;
     rc = weight_grad(p, ws, ws + p.o_off[l], HH, HH, dy, h, h, cs, grads + p.wo(l), st);
     if (rc) return rc;
-    rc = gemm(dy, h, 0, params + p.wo(l), h, 0, dO, HH, M, HH, h, nullptr, TFR_ACT_NONE, p.passes,
-              st);
+    rc = din_gemm(dy, h, 0, params + p.wo(l), h, 0, dO, HH, M, HH, h, nullptr, TFR_ACT_NONE,
+                  p.passes, st);
     if (rc) return rc;
     const float* qkv = ws + p.qkv_off[l];
     rc = p.tc ? din_tc_attn_bwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
                                 ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv,
                                 st)
-              : TFR_DIN_DISPATCH(attn_bwd, p, qkv, lmask, drop, site_seed(p.seed, 2 + 2 * l),
-                                 ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv,
-                                 st);
+              : din_attn_bwd(qkv, lmask, p.B, p.N, p.H, h, drop, site_seed(p.seed, 2 + 2 * l),
+                             ws + p.o_off[l], ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv, st);
     if (rc) return rc;
     // Q / K / V projections: one dW GEMM each (the flat layout keeps them apart)
     const float* xl = layer_input(p, ws, l);
@@ -694,8 +713,8 @@ int din_bwd(const float* X, const uint8_t* lmask, const DinPlan& p, const float*
     }
     // dX_l = dQKV [Wq | Wk | Wv]^T + residual branch (+ ReLU mask of the input projection)
     const float* wqkv = ws + p.wqkv_off + l * p.wqkv_stride;
-    rc = gemm(dqkv, 3 * HH, 0, wqkv, 3 * HH, 0, tmp, h, M, h, 3 * HH, nullptr, TFR_ACT_NONE,
-              p.passes, st);
+    rc = din_gemm(dqkv, 3 * HH, 0, wqkv, 3 * HH, 0, tmp, h, M, h, 3 * HH, nullptr, TFR_ACT_NONE,
+                  p.passes, st);
     if (rc) return rc;
     add_mask_kernel<<<blocks_for((size_t)M * h, 256), 256, 0, st>>>(
         tmp, l == 0 ? ws + p.a0_off : nullptr, (size_t)M * h, dres);
@@ -729,8 +748,8 @@ int din_input_grad(const DinPlan& p, const float* params, float* ws, int col0, i
   for (int c0 = 0; c0 < ncols; c0 += chunk) {
     const int nc = ncols - c0 < chunk ? ncols - c0 : chunk;
     float* out = accumulate ? scratch : dX + c0;
-    int rc = gemm(dres, h, 0, params + (size_t)(col0 + c0) * h, h, 0, out, accumulate ? nc : ldx,
-                  p.M, nc, h, nullptr, TFR_ACT_NONE, p.passes, st);
+    int rc = din_gemm(dres, h, 0, params + (size_t)(col0 + c0) * h, h, 0, out,
+                      accumulate ? nc : ldx, p.M, nc, h, nullptr, TFR_ACT_NONE, p.passes, st);
     if (rc) return rc;
     if (accumulate) {
       add_cols_kernel<<<blocks_for((size_t)p.M * nc, 256), 256, 0, st>>>(scratch, (size_t)p.M,

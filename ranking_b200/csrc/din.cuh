@@ -18,13 +18,37 @@ __device__ __forceinline__ float din_uniform(unsigned long long s, unsigned long
   return (float)(z >> 40) * (1.0f / 16777216.0f);
 }
 
+// FP32 SIMT attention core (din.cu): qkv [B N, 3 H h] (q, k, v blocks of H heads of h
+// columns each); lmask uint8 [B N] (0 = key masked with kMaskAdder; NULL = all valid);
+// O [B N, H h]; lse [B N, H, 2] = {row max, 1 / sum}; dsum [B N, H]; dqkv [B N, 3 H h].
+// Dropout of P with rate `drop` draws din_uniform(dseed, ((b H + head) N + i) N + j).
+// h % 4 == 0, h <= 128.
+int din_attn_fwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+                 unsigned long long dseed, float* O, float* lse, cudaStream_t st);
+int din_attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h, float drop,
+                 unsigned long long dseed, const float* O, const float* lse, const float* dO,
+                 float* dsum, float* dqkv, cudaStream_t st);
+
 // TF32 tensor-core attention core (din_tc.cu), same operands, outputs and dropout draws as the
-// SIMT kernels: qkv [B N, 3 H h]; O [B N, H h]; lse [B N, H, 2] = {row max, 1 / sum};
-// dsum [B N, H]; dqkv [B N, 3 H h].
+// SIMT kernels.
 int din_tc_attn_fwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h,
                     float drop, unsigned long long dseed, float* O, float* lse, cudaStream_t st);
 int din_tc_attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h,
                     float drop, unsigned long long dseed, const float* O, const float* lse,
                     const float* dO, float* dsum, float* dqkv, cudaStream_t st);
+
+// C [GM, GN] (ldc) = A B (+ bias, act) on the scorer GEMM engine, 3xTF32 (passes 3) or TF32
+// (passes 1).  a_mn / b_mn: operand stored MN-major (A^T [GK, GM], B [GK, GN]) instead of
+// K-major (A [GM, GK], B [GN, GK]).
+int din_gemm(const float* A, int lda, int a_mn, const float* B, int ldb, int b_mn, float* C,
+             int ldc, int GM, int GN, int GK, const float* bias, int act, int passes,
+             cudaStream_t st);
+// grads_w[0 .. Kin Nout + Nout) = {A^T dZ, column sums of dZ}: A [M, Kin] (lda), dZ [M, Nout]
+// (ldz), split over M into `splits` row ranges of whole 32-row blocks (partials of pitch
+// pstride), reduced in fixed order; colsum holds mlp_colsum's per-split column sums of dZ
+// (pitch cs_stride).  Always in the direct orientation.
+int din_weight_grad(const float* A, int lda, int Kin, const float* dZ, int ldz, int Nout, int M,
+                    int splits, float* partial, size_t pstride, const float* colsum,
+                    size_t cs_stride, float* grads_w, int passes, cudaStream_t st);
 
 }  // namespace tfr

@@ -1,0 +1,349 @@
+"""TFR-BERT (extension/premade/tfrbert_task.py): a BERT cross-encoder scores every (query,
+document) token sequence of a list, trained end to end with a ranking loss and AdamW.
+
+    BertEncoderConfig, BertEncoder     the encoder's sizes and its flat parameters (K15)
+    TFRBertScorer                      Dropout(bert_output_dropout) + Dense(1) on the pooled
+                                       [CLS] output
+    TFRBertRankingTrainer              one fused step: tfr_bert_fwd, the fused loss kernel,
+                                       tfr_bert_bwd, tfr_adamw_step
+    TFRBertDataConfig, tfrbert_batches ELWC records with `input_ids` / `input_mask` /
+                                       `segment_ids` (int64, dim seq_length) and a label
+
+The encoder is tf-models-official's BertEncoder as TFRBertScorer uses it; its math and the
+flat parameter layout are written out in include/tfr_b200.h (K15).  There is no TF / HF
+checkpoint import: `set_weights` takes the tensors in the documented order (`weight_names`).
+"""
+import ctypes
+import dataclasses
+
+import torch
+
+from ranking_b200 import _C
+from ranking_b200 import data as data_lib
+from ranking_b200 import train as train_lib
+
+_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32}
+
+
+@dataclasses.dataclass
+class BertEncoderConfig:
+  """BERT-base by default (uncased_L-12_H-768_A-12)."""
+  vocab_size: int = 30522
+  hidden_size: int = 768
+  num_layers: int = 12
+  num_attention_heads: int = 12
+  intermediate_size: int = 3072
+  max_position_embeddings: int = 512
+  type_vocab_size: int = 2
+  hidden_dropout_prob: float = 0.1
+  attention_dropout_prob: float = 0.1
+  initializer_range: float = 0.02
+
+
+def weight_shapes(config):
+  """[(name, shape), ...] in the flat parameter order of tfr_bert_fwd (the scorer's w_s / b_s
+  included)."""
+  c = config
+  e, i = c.hidden_size, c.intermediate_size
+  out = [('word_embeddings', (c.vocab_size, e)),
+         ('position_embeddings', (c.max_position_embeddings, e)),
+         ('type_embeddings', (c.type_vocab_size, e)),
+         ('embeddings/layer_norm/gamma', (e,)), ('embeddings/layer_norm/beta', (e,))]
+  for l in range(c.num_layers):
+    p = 'transformer/layer_%d/' % l
+    out += [(p + 'attention/qkv/kernel', (e, 3 * e)), (p + 'attention/qkv/bias', (3 * e,)),
+            (p + 'attention/output/kernel', (e, e)), (p + 'attention/output/bias', (e,)),
+            (p + 'attention_layer_norm/gamma', (e,)), (p + 'attention_layer_norm/beta', (e,)),
+            (p + 'intermediate/kernel', (e, i)), (p + 'intermediate/bias', (i,)),
+            (p + 'output/kernel', (i, e)), (p + 'output/bias', (e,)),
+            (p + 'output_layer_norm/gamma', (e,)), (p + 'output_layer_norm/beta', (e,))]
+  out += [('pooler/kernel', (e, e)), ('pooler/bias', (e,)),
+          ('score/kernel', (e,)), ('score/bias', (1,))]
+  return out
+
+
+def _excluded_from_decay(name):
+  # tf-models' BERT optimizer: exclude_from_weight_decay=['LayerNorm', 'layer_norm', 'bias']
+  return 'layer_norm' in name or name.endswith('bias')
+
+
+def _truncated_normal(gen, shape, stddev):
+  """tf.keras TruncatedNormal: normal draws redrawn outside two standard deviations."""
+  t = torch.randn(shape, generator=gen, dtype=torch.float64)
+  while True:
+    bad = t.abs() > 2.0
+    if not bool(bad.any()):
+      break
+    t[bad] = torch.randn(int(bad.sum()), generator=gen, dtype=torch.float64)
+  return (t * stddev).float()
+
+
+class BertEncoder(object):
+  """The encoder's flat parameters and configuration (pooler and score head included, so the
+  scorer is one buffer: one gradient, one optimizer launch).  `precision` 'fp32' (default:
+  3xTF32 GEMMs, FP32 attention core) or 'tf32' (one TF32 pass, wgmma attention core); the
+  parameters are the same in both, so `set_precision` can switch a trained encoder.
+  Initialisation (host): truncated normal with stddev `initializer_range` for the tables and
+  kernels, zero biases, LayerNorm gamma 1 / beta 0."""
+
+  def __init__(self, config=None, seed=None, device='cuda', precision=None):
+    self.config = config or BertEncoderConfig()
+    self.set_precision(precision)
+    cfg = self._make_cfg(0.0)
+    n = _C.lib.tfr_bert_param_count(ctypes.byref(cfg))
+    if n == 0:
+      raise ValueError(_C.last_error())
+    gen = torch.Generator()
+    if seed is not None:
+      gen.manual_seed(seed)
+    self._base = int(seed if seed is not None else torch.seed()) & 0xFFFFFFFF
+    self._calls = 0
+    parts, mask = [], []
+    for name, shape in weight_shapes(self.config):
+      if 'layer_norm/gamma' in name:
+        t = torch.ones(shape)
+      elif _excluded_from_decay(name):
+        t = torch.zeros(shape)
+      else:
+        t = _truncated_normal(gen, shape, self.config.initializer_range)
+      parts.append(t.reshape(-1))
+      mask.append(torch.full((t.numel(),), 0 if _excluded_from_decay(name) else 1,
+                             dtype=torch.uint8))
+    flat = torch.cat(parts)
+    assert flat.numel() == n, (flat.numel(), n)
+    self.flat = torch.nn.Parameter(flat.to(device))
+    self.decay_mask = torch.cat(mask).to(device)
+    self.output_dropout = 0.0
+    self.dims = ['bert'] + list(dataclasses.astuple(self.config)[:7])
+    self.bn_state = torch.zeros(0, device=device)
+
+  def set_precision(self, precision):
+    precision = precision or 'fp32'
+    if precision not in _PRECISIONS:
+      raise ValueError('precision must be one of %s' % sorted(_PRECISIONS))
+    self.precision = precision
+    self._precision = _PRECISIONS[precision]
+
+  def _make_cfg(self, output_dropout, training=False, seed=0):
+    c = self.config
+    cfg = _C.BertCfg()
+    cfg.vocab_size = c.vocab_size
+    cfg.hidden_size = c.hidden_size
+    cfg.num_heads = c.num_attention_heads
+    cfg.intermediate_size = c.intermediate_size
+    cfg.num_layers = c.num_layers
+    cfg.max_position = c.max_position_embeddings
+    cfg.type_vocab_size = c.type_vocab_size
+    cfg.hidden_dropout = c.hidden_dropout_prob
+    cfg.attention_dropout = c.attention_dropout_prob
+    cfg.output_dropout = float(output_dropout)
+    cfg.training = int(bool(training))
+    cfg.seed = seed
+    cfg.precision = self._precision
+    return cfg
+
+  def _run_cfg(self, training):
+    """cfg of one call; training calls draw fresh dropout (seed = base << 32 | call)."""
+    if training:
+      self._calls += 1
+    return self._make_cfg(self.output_dropout, training,
+                          (self._base << 32) | (self._calls & 0xFFFFFFFF))
+
+  def weight_names(self):
+    return [n for n, _ in weight_shapes(self.config)]
+
+  def get_weights(self):
+    """CPU tensors in the documented order (`weight_names`)."""
+    out, off = [], 0
+    flat = self.flat.detach().cpu()
+    for _, shape in weight_shapes(self.config):
+      n = 1
+      for s in shape:
+        n *= s
+      out.append(flat[off:off + n].reshape(shape).clone())
+      off += n
+    return out
+
+  def set_weights(self, weights):
+    shapes = weight_shapes(self.config)
+    if len(weights) != len(shapes):
+      raise ValueError('expected %d weights, got %d' % (len(shapes), len(weights)))
+    parts = []
+    for (name, shape), w in zip(shapes, weights):
+      w = torch.as_tensor(w, dtype=torch.float32)
+      if tuple(w.shape) != tuple(shape):
+        raise ValueError('%s: expected shape %s, got %s' % (name, shape, tuple(w.shape)))
+      parts.append(w.reshape(-1))
+    with torch.no_grad():
+      self.flat.copy_(torch.cat(parts).to(self.flat.device))
+
+
+class TFRBertScorer(object):
+  """TFRBertScorer (tfrbert_task.py): Dropout(bert_output_dropout) on the encoder's pooled
+  output, then Dense(1).  Shares the encoder's flat buffer, whose last E + 1 floats are the
+  Dense(1) kernel and bias."""
+
+  def __init__(self, encoder, bert_output_dropout=0.1):
+    if not 0.0 <= bert_output_dropout < 1.0:
+      raise ValueError('bert_output_dropout must be in [0, 1)')
+    self.encoder = encoder
+    encoder.output_dropout = float(bert_output_dropout)
+    self.flat = encoder.flat
+    self.decay_mask = encoder.decay_mask
+    self.dims = encoder.dims
+    self.bn_state = encoder.bn_state
+
+
+class TFRBertRankingTrainer(train_lib.RankingTrainer):
+  """Fused step of the reference's TFR-BERT recipe:
+
+      scores [B, N] = scorer(ids, mask, type ids [B, N, L])   tfr_bert_fwd
+      loss, d loss / d scores                                  fused loss kernel
+      d loss / d params                                        tfr_bert_bwd
+      params update                                            tfr_adamw_step (default) or the
+                                                               base class's sgd / adagrad
+
+  AdamW defaults are BERT's: weight_decay_rate 0.01 on every kernel and table (LayerNorm and
+  biases excluded), beta_1 0.9, beta_2 0.999, epsilon 1e-6; `learning_rate` may be a float or
+  a schedule such as `train.PolynomialWarmUp`.  Padded items (label < 0) are encoded too, as in
+  the reference; the loss ignores them.  fit / evaluate / checkpoints are the base class's;
+  batches are ({'input_word_ids', 'input_mask', 'input_type_ids'}, y) pairs."""
+
+  def __init__(self, scorer, loss, optimizer='adamw', learning_rate=3e-5, epsilon=1e-6,
+               weight_decay_rate=0.01, **kw):
+    self.scorer = scorer
+    self.encoder = scorer.encoder
+    super().__init__(scorer, loss, optimizer=optimizer, learning_rate=learning_rate,
+                     epsilon=epsilon, weight_decay_rate=weight_decay_rate, **kw)
+    self.bad_ids = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+  def _ensure_bert(self, b, n, seq):
+    if self._shape == (b, n, seq):
+      return
+    dev = self.device
+    self.scores = torch.empty(b, n, dtype=torch.float32, device=dev)
+    self.dscores = torch.empty(b, n, dtype=torch.float32, device=dev)
+    self.per_list = torch.empty(2, b, dtype=torch.float32, device=dev)
+    self.total2 = torch.zeros(2, dtype=torch.float32, device=dev)
+    cfg = self.encoder._make_cfg(self.encoder.output_dropout)
+    nbytes = _C.lib.tfr_bert_workspace_bytes(ctypes.byref(cfg), b * n, seq)
+    if nbytes == 0:
+      raise ValueError(_C.last_error())
+    self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    self._shape = (b, n, seq)
+
+  def _inputs(self, input_word_ids, input_mask, input_type_ids):
+    if input_word_ids.dim() != 3:
+      raise ValueError('input_word_ids must be [B, N, L], got %s' %
+                       (tuple(input_word_ids.shape),))
+    shape = tuple(input_word_ids.shape)
+    for name, t in (('input_mask', input_mask), ('input_type_ids', input_type_ids)):
+      if tuple(t.shape) != shape:
+        raise ValueError('%s has shape %s, input_word_ids %s' % (name, tuple(t.shape), shape))
+    dev = self.device
+    wid = input_word_ids.to(dev, torch.int32, non_blocking=True).contiguous()
+    msk = input_mask.to(dev, non_blocking=True)
+    msk = (msk != 0).to(torch.uint8) if msk.dtype != torch.uint8 else msk.contiguous()
+    tid = input_type_ids.to(dev, torch.int32, non_blocking=True).contiguous()
+    b, n, seq = shape
+    self._ensure_bert(b, n, seq)
+    return wid, msk, tid, b * n, seq
+
+  def check_ids(self):
+    """Raises ValueError if a step has seen ids outside the tables (host sync)."""
+    n = int(self.bad_ids.item())
+    if n:
+      raise ValueError('%d word / type ids lay outside their tables and were skipped' % n)
+
+  def train_step(self, input_word_ids, input_mask, input_type_ids, y_true, sample_weight=None,
+                 mask=None):
+    """ids / mask / type ids [B, N, L] (device or host), y_true [B, N] (label < 0 = padded
+    item).  Returns the scalar loss as a 0-d device tensor (no host sync)."""
+    wid, msk, tid, s, seq = self._inputs(input_word_ids, input_mask, input_type_ids)
+    if mask is not None:
+      y_true = torch.where(mask.to(y_true.device), y_true, torch.full_like(y_true, -1.0))
+    cfg = ctypes.byref(self.encoder._run_cfg(True))
+    flat = self.scorer.flat.data
+    grads = self.grads
+    st = _C.stream()
+    _C.check(_C.lib.tfr_bert_fwd(_C.ptr(wid), _C.ptr(msk), _C.ptr(tid), s, seq, cfg,
+                                 _C.ptr(flat), _C.ptr(self.ws), _C.ptr(self.scores),
+                                 _C.ptr(self.bad_ids), st))
+    self.loss.fused_fwd_bwd(y_true, self.scores, sample_weight, self.dscores, self.per_list,
+                            self.total2)
+    _C.check(_C.lib.tfr_bert_bwd(_C.ptr(wid), _C.ptr(msk), _C.ptr(tid), s, seq, cfg,
+                                 _C.ptr(flat), _C.ptr(self.dscores), _C.ptr(self.ws),
+                                 _C.ptr(grads), st))
+    self._apply(grads)
+    return self.total2[0]
+
+  @torch.no_grad()
+  def predict(self, input_word_ids, input_mask, input_type_ids, mask=None, y_true=None):
+    """Scores [B, N] in inference mode (no dropout)."""
+    wid, msk, tid, s, seq = self._inputs(input_word_ids, input_mask, input_type_ids)
+    cfg = ctypes.byref(self.encoder._run_cfg(False))
+    _C.check(_C.lib.tfr_bert_fwd(_C.ptr(wid), _C.ptr(msk), _C.ptr(tid), s, seq, cfg,
+                                 _C.ptr(self.scorer.flat.data), _C.ptr(self.ws),
+                                 _C.ptr(self.scores), _C.ptr(self.bad_ids), _C.stream()))
+    return self.scores
+
+
+@dataclasses.dataclass
+class TFRBertDataConfig:
+  """TFRBertDataConfig (tfrbert_task.py): the reference's recipe reads lists of 10 sequences
+  of 64 tokens."""
+  input_path: str = ''
+  global_batch_size: int = 4
+  list_size: int = 10
+  seq_length: int = 128
+  is_training: bool = True
+  drop_remainder: bool = True
+  label_feature: str = 'label'
+
+
+_MAX_EXACT_ID = 1 << 24   # ids travel through the decoder's fp32 columns
+
+
+def tfrbert_batches(paths, batch_size, list_size, seq_length, vocab_size=None,
+                    type_vocab_size=None, label_feature='label', drop_remainder=True):
+  """Yields ({'input_word_ids': int32, 'input_mask': uint8, 'input_type_ids': int32}
+  [B, list_size, seq_length], y [B, list_size]) from TFRecord files of ELWC protos, as
+  TFRBertDataLoader decodes them: example features `input_ids`, `input_mask`, `segment_ids`
+  (int64, dim seq_length, default zeros) and the label (default -1).  Padded items and
+  missing features take the defaults: a padded item is an all-masked sequence of id 0.  Ids
+  must lie in [0, vocab_size) (and type ids in [0, type_vocab_size)) when those are given,
+  and below 2^24 always (the decoder carries them exactly in fp32); ValueError otherwise."""
+  seq = int(seq_length)
+  spec = {'input_ids': (seq, 0.0), 'input_mask': (seq, 0.0), 'segment_ids': (seq, 0.0),
+          label_feature: (1, -1.0)}
+  limits = {'input_ids': vocab_size, 'segment_ids': type_vocab_size}
+  buf = []
+
+  def flush():
+    out = data_lib.parse_from_example_list(buf, list_size, None, spec)
+    ex = out['examples']
+    feats = {}
+    for i, (name, key) in enumerate((('input_ids', 'input_word_ids'),
+                                     ('input_mask', 'input_mask'),
+                                     ('segment_ids', 'input_type_ids'))):
+      col = ex[:, :, i * seq:(i + 1) * seq]
+      if name == 'input_mask':
+        feats[key] = (col != 0).to(torch.uint8)
+        continue
+      lim = limits[name]
+      top = min(lim, _MAX_EXACT_ID) if lim is not None else _MAX_EXACT_ID
+      if bool(((col < 0) | (col >= top) | (col != col.round())).any()):
+        raise ValueError('%s holds ids outside [0, %d)' % (name, top))
+      feats[key] = col.to(torch.int32)
+    y = ex[:, :, 3 * seq].clone()
+    y = torch.where(out['mask'], y, torch.full_like(y, -1.0))
+    return feats, y
+
+  for path in ([paths] if isinstance(paths, str) else paths):
+    for rec in data_lib.read_tfrecords(path):
+      buf.append(rec)
+      if len(buf) == batch_size:
+        yield flush()
+        buf = []
+  if buf and not drop_remainder:
+    yield flush()

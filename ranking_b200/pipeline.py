@@ -12,15 +12,19 @@ from ranking_b200.keras import metrics as keras_metrics
 
 
 def save_checkpoint(trainer, path, step):
-  """Parameters, optimizer accumulator, BN moving statistics and the step counter.
+  """Parameters, optimizer accumulator, BN moving statistics and the step counter (and
+  AdamW's update count).
   Data parallel: rank 0 alone writes (replicas hold identical parameters; BN statistics
   are per replica and rank 0's are the ones kept), every rank waits for the file."""
   tower = trainer.tower
   if dp.rank(trainer.group) == 0:
     tmp = '%s.tmp.%d' % (path, os.getpid())
-    torch.save({'step': int(step), 'flat': tower.flat.detach().cpu(),
-                'accum': trainer.accum.cpu(), 'bn_state': tower.bn_state.cpu(),
-                'dims': list(tower.dims)}, tmp)
+    state = {'step': int(step), 'flat': tower.flat.detach().cpu(),
+             'accum': trainer.accum.cpu(), 'bn_state': tower.bn_state.cpu(),
+             'dims': list(tower.dims)}
+    if hasattr(trainer, 'adam_step'):   # AdamW's update count t
+      state['adam_step'] = int(trainer.adam_step)
+    torch.save(state, tmp)
     os.replace(tmp, path)      # atomic: a crash never leaves a torn file
   if dp.world_size(trainer.group) > 1:
     dist.barrier(group=trainer.group)
@@ -37,7 +41,13 @@ def load_checkpoint(trainer, path):
     trainer.accum.copy_(ckpt['accum'])
     if tower.bn_state.numel():
       tower.bn_state.copy_(ckpt['bn_state'])
+  if 'adam_step' in ckpt:
+    trainer.adam_step = int(ckpt['adam_step'])
   return int(ckpt['step'])
+
+
+def _to_device(features, dev):
+  return {k: v.to(dev, non_blocking=True) for k, v in features.items()}
 
 
 def evaluate(trainer, batches, metric_group=None):
@@ -47,7 +57,12 @@ def evaluate(trainer, batches, metric_group=None):
   group.reset_state()
   dev = trainer.device
   for batch in batches:
-    x, y = batch[0].to(dev, non_blocking=True), batch[1].to(dev, non_blocking=True)
+    y = batch[1].to(dev, non_blocking=True)
+    if isinstance(batch[0], dict):   # ({input_word_ids, ...}, y): TFRBertRankingTrainer
+      scores = trainer.predict(**_to_device(batch[0], dev), mask=(y >= 0))
+      group.update_state(y, scores)
+      continue
+    x = batch[0].to(dev, non_blocking=True)
     if len(batch) > 2:     # (x, y, tokens): token features for EmbeddingRankingTrainer
       scores = trainer.predict(x, mask=(y >= 0), tokens=batch[2])
     else:
@@ -76,11 +91,13 @@ def fit(trainer, train_batches, num_steps, checkpoint_dir=None,
   for batch in train_batches:
     if step >= num_steps:
       break
-    x, y = batch[0].to(dev, non_blocking=True), batch[1].to(dev, non_blocking=True)
-    if len(batch) > 2:
-      last = trainer.train_step(x, y, tokens=batch[2])
+    y = batch[1].to(dev, non_blocking=True)
+    if isinstance(batch[0], dict):   # id tensors of TFRBertRankingTrainer
+      last = trainer.train_step(**_to_device(batch[0], dev), y_true=y)
+    elif len(batch) > 2:
+      last = trainer.train_step(batch[0].to(dev, non_blocking=True), y, tokens=batch[2])
     else:
-      last = trainer.train_step(x, y)
+      last = trainer.train_step(batch[0].to(dev, non_blocking=True), y)
     step += 1
     if ckpt and step % steps_per_checkpoint == 0:
       save_checkpoint(trainer, ckpt, step)

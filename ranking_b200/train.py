@@ -19,7 +19,32 @@ import torch
 from ranking_b200 import _C
 from ranking_b200 import dp
 
-_OPT = {'sgd': 0, 'adagrad': 1}
+_OPT = {'sgd': 0, 'adagrad': 1, 'adamw': 2}
+
+
+class PolynomialWarmUp(object):
+  """Learning rate of BERT's recipe, evaluated on the host per optimizer step (0-based):
+  linear warmup to `initial_learning_rate` over `warmup_steps`, then polynomial decay with
+  power 1 to `end_learning_rate` at `decay_steps` (tf-models' PolynomialWarmUp over
+  PolynomialDecay, power 1):
+      lr(t) = initial * t / warmup_steps                                    t < warmup_steps
+      lr(t) = end + (initial - end) * (1 - min(t, decay_steps) / decay_steps)   otherwise"""
+
+  def __init__(self, initial_learning_rate, decay_steps, warmup_steps=0,
+               end_learning_rate=0.0):
+    if decay_steps < 1 or warmup_steps < 0:
+      raise ValueError('decay_steps must be >= 1 and warmup_steps >= 0')
+    self.initial_learning_rate = float(initial_learning_rate)
+    self.decay_steps = int(decay_steps)
+    self.warmup_steps = int(warmup_steps)
+    self.end_learning_rate = float(end_learning_rate)
+
+  def __call__(self, step):
+    step = int(step)
+    if step < self.warmup_steps:
+      return self.initial_learning_rate * step / self.warmup_steps
+    frac = 1.0 - min(step, self.decay_steps) / self.decay_steps
+    return self.end_learning_rate + (self.initial_learning_rate - self.end_learning_rate) * frac
 
 
 class RankingTrainer(object):
@@ -29,11 +54,17 @@ class RankingTrainer(object):
     'fused' (default on CUDA ranks of one node): the all-reduce is part of the optimizer
             kernel — peer loads over NVLink, one flag round (csrc/dp_fused.cu, K7);
     'nccl'  one ncclAllReduce of the flat gradient, then the optimizer kernel.
+
+  optimizer 'adamw' (tfr_adamw_step): accum holds [m | v]; `adam_step` counts the updates
+  and checkpoints keep it; `learning_rate` may be a float or a schedule called with the
+  0-based update index (PolynomialWarmUp); tower.decay_mask (uint8 per parameter, if the
+  tower has one) picks the weights that decay.  Needs world size 1 or collective 'nccl'.
   """
 
   def __init__(self, tower, loss, optimizer='adagrad', learning_rate=0.001,
                epsilon=1e-7, initial_accumulator_value=0.1, process_group=None,
-               collective='fused', keep_summed_grads=False):
+               collective='fused', keep_summed_grads=False, beta_1=0.9, beta_2=0.999,
+               weight_decay_rate=0.0):
     if optimizer not in _OPT:
       raise ValueError('optimizer must be one of %s' % sorted(_OPT))
     if not hasattr(loss, 'fused_fwd_bwd'):
@@ -43,13 +74,22 @@ class RankingTrainer(object):
     self.tower = tower
     self.loss = loss
     self.opt_kind = _OPT[optimizer]
-    self.lr = float(learning_rate)
+    self.lr = learning_rate if callable(learning_rate) else float(learning_rate)
     self.eps = float(epsilon)
     dev = tower.flat.device
     self.device = dev
-    self.accum = torch.full_like(tower.flat.data, initial_accumulator_value)
     self.group = process_group
     self.world = dp.world_size(process_group)
+    if optimizer == 'adamw':
+      if self.world > 1 and collective == 'fused':
+        raise ValueError("optimizer 'adamw' with more than one rank needs collective='nccl'")
+      self.accum = torch.zeros(2 * tower.flat.numel(), dtype=torch.float32, device=dev)
+      self.adam_step = 0
+      self.beta_1, self.beta_2 = float(beta_1), float(beta_2)
+      self.weight_decay_rate = float(weight_decay_rate)
+      self.decay_mask = getattr(tower, 'decay_mask', None)
+    else:
+      self.accum = torch.full_like(tower.flat.data, initial_accumulator_value)
     self.reducer = None
     if self.world > 1 and collective == 'fused':
       self.reducer = dp.FusedGradReducer(tower.flat.numel(), dev, process_group)
@@ -128,6 +168,16 @@ class RankingTrainer(object):
                         summed_out=self.summed)
       return
     dp.all_reduce_sum_(grads, self.group)   # 'nccl': the one collective of the step
+    if self.opt_kind == _OPT['adamw']:
+      lr = self.lr(self.adam_step) if callable(self.lr) else self.lr
+      self.adam_step += 1
+      n = grads.numel()
+      _C.check(_C.lib.tfr_adamw_step(
+          _C.ptr(t.flat.data), _C.ptr(grads), _C.ptr(self.accum[:n]), _C.ptr(self.accum[n:]),
+          _C.ptr(self.decay_mask), n, lr, self.beta_1, self.beta_2, self.eps,
+          self.weight_decay_rate, self.adam_step, dp.replica_grad_scale(self.group),
+          _C.stream()))
+      return
     _C.check(_C.lib.tfr_optimizer_step(
         _C.ptr(t.flat.data), _C.ptr(grads), _C.ptr(self.accum), grads.numel(),
         self.opt_kind, self.lr, self.eps, dp.replica_grad_scale(self.group), _C.stream()))
