@@ -6,6 +6,13 @@ per-task loss weights (the reference's MultiTaskPipeline, keras/pipeline.py:733-
       --losses relevance=softmax_loss,click=sigmoid_cross_entropy_loss --loss_weights click=0.5
 
   python examples/multitask_train.py --synthetic     # seeded data, no files needed
+  python examples/multitask_train.py --synthetic --scorer din      # listwise context
+  python examples/multitask_train.py --synthetic --scorer dasalc
+
+--scorer picks the model that carries a score plane per task: `dnn` (default) a create_tower
+tower (MultiTaskRankingTrainer), `din` a DocumentInteractionAttention embedding feeding that
+tower (MultiTaskDINRankingTrainer), `dasalc` the DIN and a DASALCScorer
+(MultiTaskDASALCRankingTrainer; features go through log1p_cutoff first).
 
 --synthetic writes TFRecords whose two labels come from two different linear utilities of
 the same features (a graded relevance and a binary click), trains both tasks and prints each
@@ -61,7 +68,12 @@ def main():
   ap.add_argument('--loss_weights', default='')
   ap.add_argument('--list_size', type=int, default=20)
   ap.add_argument('--batch_size', type=int, default=32)
-  ap.add_argument('--hidden', default='64,32')
+  ap.add_argument('--hidden', default='64,32', help='tower widths of --scorer dnn / din')
+  ap.add_argument('--scorer', default='dnn', choices=['dnn', 'din', 'dasalc'])
+  ap.add_argument('--din_heads', type=int, default=2)
+  ap.add_argument('--din_head_size', type=int, default=16, help='also DASALC context_dim')
+  ap.add_argument('--din_layers', type=int, default=1)
+  ap.add_argument('--dasalc_hidden', type=int, default=64, help='DASALC hidden_dim W')
   ap.add_argument('--epochs', type=int, default=6)
   ap.add_argument('--steps_per_epoch', type=int, default=24)
   ap.add_argument('--learning_rate', type=float, default=0.1)
@@ -101,13 +113,30 @@ def main():
       model_dir=args.model_dir or os.path.join(tmp, 'model'), num_epochs=args.epochs,
       steps_per_epoch=args.steps_per_epoch, validation_steps=8,
       learning_rate=args.learning_rate, loss=losses, loss_weights=weights)
-  p = pipeline.MultiTaskPipeline(
-      lambda: tfr.keras.layers.create_tower(hidden, len(labels), activation='relu',
-                                            input_dim=input_dim, seed=1, precision='tf32x3'),
-      batches(train), batches(valid), hp)
+  def model():
+    t = len(labels)
+    if args.scorer == 'dnn':
+      return tfr.keras.layers.create_tower(hidden, t, activation='relu', input_dim=input_dim,
+                                           seed=1, precision='tf32x3')
+    din = tfr.keras.layers.DocumentInteractionAttention(args.din_heads, args.din_head_size,
+                                                        args.din_layers, dropout=0.0, seed=2)
+    din.build(input_dim)
+    if args.scorer == 'din':
+      return din, tfr.keras.layers.create_tower(hidden, t, activation='relu',
+                                                input_dim=input_dim + args.din_head_size,
+                                                seed=1, precision='tf32x3')
+    from ranking_b200.research import dasalc
+    return din, dasalc.DASALCScorer(input_dim, args.dasalc_hidden, args.din_head_size,
+                                    dropout=0.0, input_noise_stddev=0.0, seed=1,
+                                    output_units=t)
+
+  trainer_cls = {'dnn': None, 'din': tfr.train.MultiTaskDINRankingTrainer,
+                 'dasalc': tfr.train.MultiTaskDASALCRankingTrainer}[args.scorer]
+  p = pipeline.MultiTaskPipeline(model, batches(train), batches(valid), hp,
+                                 trainer_cls=trainer_cls)
   hist = p.train_and_validate()
   last = hist[-1]
-  print('epochs %d, validation loss %.5f' % (len(hist), last['loss']))
+  print('scorer %s, epochs %d, validation loss %.5f' % (args.scorer, len(hist), last['loss']))
   for t in labels:
     print('%-12s loss %.5f  NDCG@1 %.4f  NDCG@5 %.4f  NDCG@10 %.4f  NDCG %.4f' % (
         t, last[t + '_loss'], last[t + '_metric/ndcg_1'], last[t + '_metric/ndcg_5'],

@@ -602,6 +602,31 @@ int tfr_dasalc_fwd(const float* X, const float* E, int lde, int M, const tfr_das
 int tfr_dasalc_bwd(const float* X, int M, const tfr_dasalc_cfg* cfg, const float* params,
                    const float* dscores, const uint8_t* mask, void* workspace, float* grads,
                    float* dE, int ldde, int precision, void* stream);
+/* Multi-task DASALC: the same scorer with T = num_tasks output units, one per ranking task.
+ * The parameter layout is tfr_dasalc_param_count's up to b_c, then w_o [W, T] (Keras kernel
+ * layout) and b_o [T], then the BN gamma / beta as above; with T = 1 it is exactly that layout.
+ *   score_planes [T, M]: score_planes[o * M + m] = Dropout(relu(t * c + t))[m] w_o[:, o] + b_o[o],
+ *   so plane o is task o's [B, N] score matrix; masked rows are ln(1e-10) on every plane.
+ * The random draws and the moving-statistics update are tfr_dasalc_fwd's (they do not depend
+ * on T).  The backward takes dscore_planes [T, M] and task_weights_host (T host floats, NULL =
+ * all 1) and forms the gradients of sum_o w_o L_o: the cross backward consumes the combined
+ * signal sum_o w_o ds_o[m] w_o[:, o], rows the mask clears contribute 0 for every task, and
+ * dw_o / db_o are reduced in a fixed order (two identical calls give identical bits).
+ * Limits: tfr_dasalc_fwd's, plus 1 <= num_tasks <= 8, precision TFR_PREC_TF32X3 or
+ * TFR_PREC_TF32, every weight finite and score_planes / dscore_planes / grads not NULL
+ * (TFR_INVALID_ARGUMENT before any CUDA call; the size queries return 0).
+ * With T = 1 and weight 1 the scores, grads, dE and bn_state are tfr_dasalc_fwd / _bwd's bits.
+ * The workspace is tfr_dasalc_workspace_bytes_tasks(cfg, M, T). */
+size_t tfr_dasalc_param_count_tasks(const tfr_dasalc_cfg* cfg, int num_tasks);
+size_t tfr_dasalc_workspace_bytes_tasks(const tfr_dasalc_cfg* cfg, int M, int num_tasks);
+int tfr_dasalc_fwd_tasks(const float* X, const float* E, int lde, int M,
+                         const tfr_dasalc_cfg* cfg, const float* params, const uint8_t* mask,
+                         void* workspace, float* score_planes, int num_tasks, int precision,
+                         void* stream);
+int tfr_dasalc_bwd_tasks(const float* X, int M, const tfr_dasalc_cfg* cfg, const float* params,
+                         const float* dscore_planes, const float* task_weights_host,
+                         const uint8_t* mask, void* workspace, float* grads, float* dE, int ldde,
+                         int num_tasks, int precision, void* stream);
 /* DASALC's feature transform (research/dasalc.py:127-129), elementwise over n floats:
  *   out = clip(sign(x) log1p(|x|), -cutoff, cutoff),  cutoff > 0; out may alias X. */
 int tfr_symmetric_log1p_clip(const float* X, size_t n, float cutoff, float* out, void* stream);

@@ -177,6 +177,12 @@ _SIGNATURES = {
     'tfr_dasalc_workspace_bytes': (C.c_size_t, [C.POINTER(DasalcCfg), _I]),
     'tfr_dasalc_fwd': (_I, [_P, _P, _I, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _I, _P]),
     'tfr_dasalc_bwd': (_I, [_P, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _P, _P, _I, _I, _P]),
+    'tfr_dasalc_param_count_tasks': (C.c_size_t, [C.POINTER(DasalcCfg), _I]),
+    'tfr_dasalc_workspace_bytes_tasks': (C.c_size_t, [C.POINTER(DasalcCfg), _I, _I]),
+    'tfr_dasalc_fwd_tasks': (_I, [_P, _P, _I, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _I, _I,
+                                  _P]),
+    'tfr_dasalc_bwd_tasks': (_I, [_P, _I, C.POINTER(DasalcCfg), _P, _P, _P, _P, _P, _P, _P, _I,
+                                  _I, _I, _P]),
     'tfr_symmetric_log1p_clip': (_I, [_P, C.c_size_t, _F, _P, _P]),
     'tfr_bilinear_param_count': (C.c_size_t, [_I, _I]),
     'tfr_bilinear_workspace_bytes': (C.c_size_t, [_I, _I, _I]),

@@ -282,8 +282,10 @@ class ModelFitPipeline(object):
 
 
 class MultiTaskPipeline(ModelFitPipeline):
-  """`MultiTaskPipeline` (keras/pipeline.py:733-824) over `MultiTaskRankingTrainer`:
-  `hparams.loss` maps each task to a loss key (dict order = the tower's output units) and
+  """`MultiTaskPipeline` (keras/pipeline.py:733-824) over `MultiTaskRankingTrainer`, or over
+  `trainer_cls` (`MultiTaskDINRankingTrainer`, `MultiTaskDASALCRankingTrainer`), which is
+  called as trainer_cls(*parts, losses, ...) with `parts` what `tower_fn()` returns: a tower,
+  or a tuple of model parts such as (din, tower) or (din, scorer).  `hparams.loss` maps each task to a loss key (dict order = the tower's output units) and
   `hparams.loss_weights` is None or a dict over those tasks.  The epoch loop, checkpoints,
   best checkpoint, early stopping and ReduceLROnPlateau are `ModelFitPipeline`'s.
 
@@ -297,10 +299,11 @@ class MultiTaskPipeline(ModelFitPipeline):
   TOPNS = (1, 5, 10, None)
 
   def __init__(self, tower_fn, train_batches_fn, valid_batches_fn, hparams,
-               process_group=None, log_fn=print):
+               process_group=None, log_fn=print, trainer_cls=None):
     super().__init__(tower_fn, train_batches_fn, valid_batches_fn, hparams,
                      process_group=process_group, log_fn=log_fn)
     self.tasks = list(hparams.loss)
+    self._trainer_cls = trainer_cls
 
   @staticmethod
   def _validate_hparams(hparams):
@@ -329,11 +332,10 @@ class MultiTaskPipeline(ModelFitPipeline):
   def _make_trainer(self, tower):
     from ranking_b200 import train as train_lib
     hp = self._hparams
-    return train_lib.MultiTaskRankingTrainer(tower, self.build_loss(),
-                                             loss_weights=hp.loss_weights,
-                                             optimizer=hp.optimizer,
-                                             learning_rate=hp.learning_rate,
-                                             process_group=self._group)
+    cls = self._trainer_cls or train_lib.MultiTaskRankingTrainer
+    parts = tower if isinstance(tower, tuple) else (tower,)
+    return cls(*parts, self.build_loss(), loss_weights=hp.loss_weights, optimizer=hp.optimizer,
+               learning_rate=hp.learning_rate, process_group=self._group)
 
   @staticmethod
   def _unpack(batch, dev, non_blocking=False):

@@ -6,7 +6,7 @@ ICLR 2021; research/dasalc.py of the reference): the scorer and its feature tran
     a0 = BN_in(x) + GaussianNoise            x: log1p_cutoff-transformed features [.., D]
     a_l = Dropout(BN_l(relu(Dense_W(a_l-1))))  two hidden layers of width W
     t = Dense_W(a_2),  c = Dense_W(BN_c(e))   e: the DocumentInteractionAttention output [.., h]
-    s = Dense_1(Dropout(relu(t * c + t)))     the latent cross
+    s = Dense_T(Dropout(relu(t * c + t)))     the latent cross, T = output_units tasks
 
 All parameters live in ONE flat fp32 buffer (`flat`) in the layout of include/tfr_b200.h
 (W_1, b_1, W_2, b_2, W_t, b_t, W_c, b_c, w_o, b_o, then gamma / beta of BN_in, BN_1, BN_2, BN_c);
@@ -37,13 +37,13 @@ class _DASALCFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, x, e, flat, m8, scorer):
-    m = x.shape[0]
-    scores = torch.empty(m, dtype=torch.float32, device=x.device)
+    m, t = x.shape[0], scorer.output_units
+    scores = torch.empty(t, m, dtype=torch.float32, device=x.device)
     ws = scorer._new_workspace(m)
     cfg = scorer._run_cfg()
-    _C.check(_C.lib.tfr_dasalc_fwd(_C.ptr(x), _C.ptr(e), e.shape[1], m, ctypes.byref(cfg),
-                                   _C.ptr(flat), _C.ptr(m8), _C.ptr(ws), _C.ptr(scores),
-                                   scorer._precision, _C.stream()))
+    _C.check(_C.lib.tfr_dasalc_fwd_tasks(_C.ptr(x), _C.ptr(e), e.shape[1], m, ctypes.byref(cfg),
+                                         _C.ptr(flat), _C.ptr(m8), _C.ptr(ws), _C.ptr(scores), t,
+                                         scorer._precision, _C.stream()))
     ctx.cfg, ctx.ws, ctx.scorer = cfg, ws, scorer
     ctx.save_for_backward(x, flat, m8)
     return scores
@@ -56,9 +56,10 @@ class _DASALCFn(torch.autograd.Function):
     grads = torch.empty_like(flat)
     de = torch.empty(m, h, dtype=torch.float32, device=x.device)
     g = g.float().contiguous()
-    _C.check(_C.lib.tfr_dasalc_bwd(_C.ptr(x), m, ctypes.byref(ctx.cfg), _C.ptr(flat), _C.ptr(g),
-                                   _C.ptr(m8), _C.ptr(ctx.ws), _C.ptr(grads), _C.ptr(de), h,
-                                   ctx.scorer._precision, _C.stream()))
+    _C.check(_C.lib.tfr_dasalc_bwd_tasks(_C.ptr(x), m, ctypes.byref(ctx.cfg), _C.ptr(flat),
+                                         _C.ptr(g), None, _C.ptr(m8), _C.ptr(ctx.ws),
+                                         _C.ptr(grads), _C.ptr(de), h, ctx.scorer.output_units,
+                                         ctx.scorer._precision, _C.stream()))
     return None, de, grads, None, None
 
 
@@ -73,7 +74,9 @@ class DASALCScorer(torch.nn.Module):
   through `log1p_cutoff` and the DIN embedding of every item.
 
   Called as `scorer((x, e), mask)` with x [B, N, D] (or [M, D]) and e [B, N, h] (or [M, h]);
-  returns scores of the same leading shape, ln(1e-10) where `mask` is False.  Gradients flow
+  returns scores of the same leading shape, ln(1e-10) where `mask` is False.  With
+  `output_units` T > 1 (one unit per ranking task, MultiTaskDASALCRankingTrainer) the output
+  layer is [W, T] and the result is [T, *leading shape], one score plane per task.  Gradients flow
   to `flat` and to `e` (not to x).  Keras initialisers: glorot-uniform kernels, zero biases,
   BN gamma ones / beta zeros, moving mean zeros / variance ones; BN epsilon 1e-3 as
   tf.compat.v1.layers.batch_normalization.  Limits: D, hidden_dim, context_dim multiples of 4,
@@ -84,13 +87,14 @@ class DASALCScorer(torch.nn.Module):
 
   def __init__(self, input_dim, hidden_dim=512, context_dim=100, dropout=0.4,
                input_noise_stddev=1.5, batch_norm_moment=0.9, precision='tf32x3', seed=None,
-               device='cuda'):
+               device='cuda', output_units=1):
     super().__init__()
     if precision not in _PRECISIONS:
       raise ValueError('precision must be one of %s' % sorted(_PRECISIONS))
     self.input_dim = int(input_dim)
     self.hidden_dim = int(hidden_dim)
     self.context_dim = int(context_dim)
+    self.output_units = int(output_units)
     self.dropout = float(dropout or 0.0)
     self.input_noise_stddev = float(input_noise_stddev or 0.0)
     self.batch_norm_moment = float(batch_norm_moment)
@@ -105,7 +109,7 @@ class DASALCScorer(torch.nn.Module):
     cfg.bn_epsilon = self.bn_epsilon
     cfg.bn_momentum = self.batch_norm_moment
     cfg.training = 1
-    n = _C.lib.tfr_dasalc_param_count(ctypes.byref(cfg))
+    n = _C.lib.tfr_dasalc_param_count_tasks(ctypes.byref(cfg), self.output_units)
     if n == 0:
       raise ValueError(_C.last_error())
     ns = _C.lib.tfr_dasalc_bn_state_count(ctypes.byref(cfg))
@@ -113,7 +117,7 @@ class DASALCScorer(torch.nn.Module):
     d, w, h = self.input_dim, self.hidden_dim, self.context_dim
     # (name, rows, cols) of the kernels; every kernel is followed by its bias [cols]
     shapes = [('hidden1', d, w), ('hidden2', w, w), ('tower', w, w), ('context', h, w),
-              ('output', w, 1)]
+              ('output', w, self.output_units)]
     gen = torch.Generator()
     if seed is not None:
       gen.manual_seed(int(seed))
@@ -134,6 +138,8 @@ class DASALCScorer(torch.nn.Module):
     flat = torch.cat(parts)
     assert flat.numel() == n and soff == ns, (flat.numel(), n, soff, ns)
     self.dims = ['dasalc', d, w, h]
+    if self.output_units > 1:
+      self.dims.append(self.output_units)
     self.flat = torch.nn.Parameter(flat.to(device))
     self.register_buffer('bn_state', torch.cat(state).to(device))
     self._base = int(seed if seed is not None else torch.seed()) & 0xFFFFFFFF
@@ -171,7 +177,8 @@ class DASALCScorer(torch.nn.Module):
     return cfg
 
   def _new_workspace(self, m):
-    nbytes = _C.lib.tfr_dasalc_workspace_bytes(ctypes.byref(self._cfg), int(m))
+    nbytes = _C.lib.tfr_dasalc_workspace_bytes_tasks(ctypes.byref(self._cfg), int(m),
+                                                     self.output_units)
     if nbytes == 0:
       raise ValueError(_C.last_error())
     return torch.empty(nbytes, dtype=torch.uint8, device=self.flat.device)
@@ -193,10 +200,14 @@ class DASALCScorer(torch.nn.Module):
     m8 = None
     if mask is not None:
       m8 = torch.as_tensor(mask, device=x.device).reshape(-1).to(torch.uint8).contiguous()
-    return _DASALCFn.apply(x, e, self.flat, m8, self).reshape(lead)
+    scores = _DASALCFn.apply(x, e, self.flat, m8, self)
+    if self.output_units == 1:
+      return scores.reshape(lead)
+    return scores.reshape((self.output_units,) + tuple(lead))
 
   def get_config(self):
     return {'input_dim': self.input_dim, 'hidden_dim': self.hidden_dim,
             'context_dim': self.context_dim, 'dropout': self.dropout,
             'input_noise_stddev': self.input_noise_stddev,
-            'batch_norm_moment': self.batch_norm_moment, 'precision': self.precision}
+            'batch_norm_moment': self.batch_norm_moment, 'precision': self.precision,
+            'output_units': self.output_units}

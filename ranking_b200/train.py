@@ -221,25 +221,24 @@ class RankingTrainer(object):
 _MAX_TASKS = 8
 
 
-class MultiTaskRankingTrainer(RankingTrainer):
-  """Fused step for several ranking tasks on one tower (the reference's multi-task
-  `UnivariateScorer` with `MultiTaskPipeline`'s per-task losses and `loss_weights`,
-  keras/model.py:755-777 and keras/pipeline.py:733-824).
+class _TaskPlanes(object):
+  """The task handling every multi-task trainer shares; mixed in before a single-task
+  trainer, whose scorer then writes task-major score planes [T, B, N] and reads T dscore
+  planes.  `losses` is an ordered dict task -> `ranking_b200.keras.losses` object; dict order
+  is the order of the scorer's output units.  `loss_weights` maps tasks to weights (missing:
+  1.0).  One step is
 
-  `losses` is an ordered dict task -> `ranking_b200.keras.losses` object; dict order is the
-  order of the tower's output units, so `tower.output_units == len(losses)`.  `loss_weights`
-  maps tasks to weights (missing: 1.0).  One step is
-
-      tfr_mlp_fwd_tasks          task-major score planes [T, B, N], RestoreList on each
+      scorer forward             task-major score planes, RestoreList on each
       loss_t.fused_fwd_bwd       one per task, on plane t, into dscore plane t
-      tfr_mlp_bwd_tasks          output-layer backward applies w_t as it reads plane t
+      scorer backward            applies w_t as it reads dscore plane t
       optimizer / all-reduce     as RankingTrainer
 
   and returns sum_t w_t L_t (each L_t reduced by its own loss's reduction), the Keras
   compile-time `loss_weights` semantics, as a 0-d device tensor; `task_losses` holds the
   [T] per-task values of the last step."""
 
-  def __init__(self, tower, losses, loss_weights=None, **kw):
+  def _set_tasks(self, losses, loss_weights, output_units):
+    """Checks the tasks against the scorer's output units; returns the first task's loss."""
     losses = dict(losses)
     if not losses:
       raise ValueError('losses must name at least one task')
@@ -254,17 +253,18 @@ class MultiTaskRankingTrainer(RankingTrainer):
     if unknown:
       raise ValueError('loss_weights name unknown tasks %s (tasks: %s)' %
                        (unknown, list(losses)))
-    if tower.output_units != len(losses):
+    if output_units != len(losses):
       raise ValueError('the tower has %d output units for %d tasks' %
-                       (tower.output_units, len(losses)))
-    if tower._precision not in (_C.PREC_FP32, _C.PREC_TF32X3, _C.PREC_TF32):
-      raise ValueError('multi-task towers need precision fp32, tf32x3 or tf32')
+                       (output_units, len(losses)))
     self.tasks = list(losses)
     self.losses = losses
     self.loss_weights = [float(weights.get(t, 1.0)) for t in self.tasks]
     if not all(w == w and abs(w) != float('inf') for w in self.loss_weights):
       raise ValueError('loss weights must be finite: %s' % self.loss_weights)
-    super().__init__(tower, losses[self.tasks[0]], **kw)
+    return losses[self.tasks[0]]
+
+  def _set_task_weights(self):
+    """After RankingTrainer.__init__: the weights as the backward and the loss sum take them."""
     t = len(self.tasks)
     self._w_host = (ctypes.c_float * t)(*self.loss_weights)
     # tfr_weighted_sum over the [T, 2] task totals {L_t, sum of weights}: (w_t, 0) pairs
@@ -284,27 +284,19 @@ class MultiTaskRankingTrainer(RankingTrainer):
     self.ws = self._new_workspace(b, n)
     self._shape = (b, n)
 
-  def _forward(self, x, y_true, m8, cfg, training):
-    b, n, _ = x.shape
-    t = self.tower
-    _C.check(_C.lib.tfr_mlp_fwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data), _C.ptr(m8),
-                                      _C.ptr(self.ws), _C.ptr(self.scores), t._precision,
-                                      _C.stream()))
-
-  def _backward(self, x, m8, cfg, grads):
-    b, n, _ = x.shape
-    t = self.tower
-    _C.check(_C.lib.tfr_mlp_bwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data),
-                                      _C.ptr(self.dscores), self._w_host, _C.ptr(m8),
-                                      _C.ptr(self.ws), _C.ptr(grads), t._precision,
-                                      _C.stream()))
-
   def _labels(self, labels):
     missing = [t for t in self.tasks if t not in labels]
     if missing or len(labels) != len(self.tasks):
       raise ValueError('labels must map exactly the tasks %s (got %s)' %
                        (self.tasks, sorted(labels)))
     return [labels[t] for t in self.tasks]
+
+  @staticmethod
+  def _any_label(ys):
+    mask = ys[0] >= 0
+    for y in ys[1:]:
+      mask = mask | (y >= 0)
+    return mask
 
   def train_step(self, x, labels, sample_weight=None, mask=None):
     """x [B, N, D] (device), labels {task: [B, N]} (label < 0: no label for that task),
@@ -315,9 +307,7 @@ class MultiTaskRankingTrainer(RankingTrainer):
     self._ensure(b, n)
     x = self._prep_x(x)
     if mask is None:
-      mask = ys[0] >= 0
-      for y in ys[1:]:
-        mask = mask | (y >= 0)
+      mask = self._any_label(ys)
     m8 = mask.reshape(-1).to(torch.uint8).contiguous()
     cfg = ctypes.byref(self.tower._run_cfg(training=True))
     grads = self.reducer.grads() if self.reducer is not None else self.grads
@@ -339,12 +329,39 @@ class MultiTaskRankingTrainer(RankingTrainer):
     """{task: [B, N] score view}; masked items (`mask`, else items without any label >= 0
     when `labels` is given) hold ln(1e-10) in every task's plane."""
     if mask is None and labels is not None:
-      ys = self._labels(labels)
-      mask = ys[0] >= 0
-      for y in ys[1:]:
-        mask = mask | (y >= 0)
+      mask = self._any_label(self._labels(labels))
     scores = super().predict(x, mask=mask)
     return {t: scores[i] for i, t in enumerate(self.tasks)}
+
+
+class MultiTaskRankingTrainer(_TaskPlanes, RankingTrainer):
+  """Fused step for several ranking tasks on one tower (the reference's multi-task
+  `UnivariateScorer` with `MultiTaskPipeline`'s per-task losses and `loss_weights`,
+  keras/model.py:755-777 and keras/pipeline.py:733-824): `tower.output_units ==
+  len(losses)`, the scorer forward / backward are tfr_mlp_fwd_tasks / tfr_mlp_bwd_tasks, and
+  the rest of the step is _TaskPlanes'."""
+
+  def __init__(self, tower, losses, loss_weights=None, **kw):
+    first = self._set_tasks(losses, loss_weights, tower.output_units)
+    if tower._precision not in (_C.PREC_FP32, _C.PREC_TF32X3, _C.PREC_TF32):
+      raise ValueError('multi-task towers need precision fp32, tf32x3 or tf32')
+    super().__init__(tower, first, **kw)
+    self._set_task_weights()
+
+  def _forward(self, x, y_true, m8, cfg, training):
+    b, n, _ = x.shape
+    t = self.tower
+    _C.check(_C.lib.tfr_mlp_fwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data), _C.ptr(m8),
+                                      _C.ptr(self.ws), _C.ptr(self.scores), t._precision,
+                                      _C.stream()))
+
+  def _backward(self, x, m8, cfg, grads):
+    b, n, _ = x.shape
+    t = self.tower
+    _C.check(_C.lib.tfr_mlp_bwd_tasks(_C.ptr(x), b * n, cfg, _C.ptr(t.flat.data),
+                                      _C.ptr(self.dscores), self._w_host, _C.ptr(m8),
+                                      _C.ptr(self.ws), _C.ptr(grads), t._precision,
+                                      _C.stream()))
 
 
 class GroupwiseRankingTrainer(RankingTrainer):
@@ -514,8 +531,16 @@ class DINRankingTrainer(RankingTrainer):
     _C.check(_C.lib.tfr_din_fwd(_C.ptr(x), _C.ptr(lm), b, n, ctypes.byref(self._din_cfg),
                                 _C.ptr(din.flat.data), _C.ptr(self.din_ws),
                                 ctypes.c_void_p(self.xe.data_ptr() + 4 * d), width, st))
-    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(self.mlp.flat.data),
+    self._tower_fwd(b * n, m8, cfg, st)
+
+  def _tower_fwd(self, m, m8, cfg, st):
+    _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(self.xe), m, cfg, _C.ptr(self.mlp.flat.data),
                                 _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores),
+                                self.mlp._precision, st))
+
+  def _tower_bwd(self, m, m8, cfg, tower_grads, st):
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(self.xe), m, cfg, _C.ptr(self.mlp.flat.data),
+                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws), tower_grads,
                                 self.mlp._precision, st))
 
   def _backward(self, x, m8, cfg, grads):
@@ -523,10 +548,7 @@ class DINRankingTrainer(RankingTrainer):
     din, mlp = self.din, self.mlp
     n_din = self.tower.n_din
     st = _C.stream()
-    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(self.xe), b * n, cfg, _C.ptr(mlp.flat.data),
-                                _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
-                                ctypes.c_void_p(grads.data_ptr() + 4 * n_din), mlp._precision,
-                                st))
+    self._tower_bwd(b * n, m8, cfg, ctypes.c_void_p(grads.data_ptr() + 4 * n_din), st)
     _C.check(_C.lib.tfr_mlp_input_grad(cfg, b * n, _C.ptr(mlp.flat.data), _C.ptr(self.ws), d,
                                        din.head_size, _C.ptr(self.d_emb), din.head_size,
                                        mlp._precision, st))
@@ -581,6 +603,9 @@ class DASALCRankingTrainer(RankingTrainer):
                        (din.head_size, scorer.context_dim))
     if not float(cutoff) > 0:
       raise ValueError('cutoff must be > 0')
+    if scorer.output_units != self._scorer_units():
+      raise ValueError('the scorer has %d output units, the trainer scores %d task(s)' %
+                       (scorer.output_units, self._scorer_units()))
     self.din = din
     self.scorer = scorer
     self.cutoff = float(cutoff)
@@ -607,7 +632,7 @@ class DASALCRankingTrainer(RankingTrainer):
 
   def _forward(self, x, y_true, m8, cfg, training):
     b, n, _ = x.shape
-    din, sc = self.din, self.scorer
+    din = self.din
     lm = m8
     if lm is None and y_true is not None:
       lm = (y_true >= 0).reshape(-1).to(torch.uint8).contiguous()
@@ -617,22 +642,96 @@ class DASALCRankingTrainer(RankingTrainer):
     _C.check(_C.lib.tfr_din_fwd(_C.ptr(x), _C.ptr(lm), b, n, ctypes.byref(self._din_cfg),
                                 _C.ptr(din.flat.data), _C.ptr(self.din_ws), _C.ptr(self.emb),
                                 din.head_size, st))
-    _C.check(_C.lib.tfr_dasalc_fwd(_C.ptr(x), _C.ptr(self.emb), din.head_size, b * n, cfg,
+    self._scorer_fwd(x, b * n, m8, cfg, st)
+
+  def _scorer_units(self):
+    return 1
+
+  def _scorer_fwd(self, x, m, m8, cfg, st):
+    sc = self.scorer
+    _C.check(_C.lib.tfr_dasalc_fwd(_C.ptr(x), _C.ptr(self.emb), sc.context_dim, m, cfg,
                                    _C.ptr(sc.flat.data), _C.ptr(m8), _C.ptr(self.ws),
                                    _C.ptr(self.scores), sc._precision, st))
 
+  def _scorer_bwd(self, x, m, m8, cfg, scorer_grads, st):
+    sc = self.scorer
+    _C.check(_C.lib.tfr_dasalc_bwd(_C.ptr(x), m, cfg, _C.ptr(sc.flat.data),
+                                   _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
+                                   scorer_grads, _C.ptr(self.d_emb), sc.context_dim,
+                                   sc._precision, st))
+
   def _backward(self, x, m8, cfg, grads):
     b, n, _ = x.shape
-    din, sc = self.din, self.scorer
+    din = self.din
     h = din.head_size
     st = _C.stream()
-    _C.check(_C.lib.tfr_dasalc_bwd(_C.ptr(x), b * n, cfg, _C.ptr(sc.flat.data),
-                                   _C.ptr(self.dscores), _C.ptr(m8), _C.ptr(self.ws),
-                                   ctypes.c_void_p(grads.data_ptr() + 4 * self.tower.n_din),
-                                   _C.ptr(self.d_emb), h, sc._precision, st))
+    scorer_grads = ctypes.c_void_p(grads.data_ptr() + 4 * self.tower.n_din)
+    self._scorer_bwd(x, b * n, m8, cfg, scorer_grads, st)
     _C.check(_C.lib.tfr_din_bwd(_C.ptr(x), _C.ptr(self._lm), b, n, ctypes.byref(self._din_cfg),
                                 _C.ptr(din.flat.data), _C.ptr(self.d_emb), h,
                                 _C.ptr(self.din_ws), _C.ptr(grads), st))
+
+
+class MultiTaskDINRankingTrainer(_TaskPlanes, DINRankingTrainer):
+  """DINRankingTrainer with a score plane per task: the DocumentInteractionAttention
+  embedding feeds one create_tower tower with `tower.output_units == len(losses)` output
+  units, one per task.  One step is
+
+      [X | E] with E = din((X, list_mask))    tfr_din_fwd
+      score planes = tower([X | E])           tfr_mlp_fwd_tasks
+      per-task losses                         one fused loss kernel per task
+      tower gradients, d loss / d E           tfr_mlp_bwd_tasks (loss weights), tfr_mlp_input_grad
+      DIN gradients                           tfr_din_bwd
+      optimizer                               one launch over the shared flat buffer
+
+  The tower constraints are DINRankingTrainer's; labels, masks, the returned loss and
+  predict are MultiTaskRankingTrainer's."""
+
+  def __init__(self, din, tower, losses, loss_weights=None, **kw):
+    first = self._set_tasks(losses, loss_weights, tower.output_units)
+    super().__init__(din, tower, first, **kw)
+    self._set_task_weights()
+
+  def _tower_fwd(self, m, m8, cfg, st):
+    _C.check(_C.lib.tfr_mlp_fwd_tasks(_C.ptr(self.xe), m, cfg, _C.ptr(self.mlp.flat.data),
+                                      _C.ptr(m8), _C.ptr(self.ws), _C.ptr(self.scores),
+                                      self.mlp._precision, st))
+
+  def _tower_bwd(self, m, m8, cfg, tower_grads, st):
+    _C.check(_C.lib.tfr_mlp_bwd_tasks(_C.ptr(self.xe), m, cfg, _C.ptr(self.mlp.flat.data),
+                                      _C.ptr(self.dscores), self._w_host, _C.ptr(m8),
+                                      _C.ptr(self.ws), tower_grads, self.mlp._precision, st))
+
+
+class MultiTaskDASALCRankingTrainer(_TaskPlanes, DASALCRankingTrainer):
+  """DASALCRankingTrainer with a score plane per task: `scorer` is a DASALCScorer with
+  `output_units == len(losses)`, run by tfr_dasalc_fwd_tasks / tfr_dasalc_bwd_tasks (K13
+  with a [W, T] output layer; the loss weights are applied as the backward reads the dscore
+  planes).  The log1p transform, circular padding, DIN and optimizer are
+  DASALCRankingTrainer's; labels, masks, the returned loss and predict are
+  MultiTaskRankingTrainer's."""
+
+  def __init__(self, din, scorer, losses, loss_weights=None, cutoff=30.0, **kw):
+    first = self._set_tasks(losses, loss_weights, scorer.output_units)
+    super().__init__(din, scorer, first, cutoff=cutoff, **kw)
+    self._set_task_weights()
+
+  def _scorer_units(self):
+    return len(self.tasks)
+
+  def _scorer_fwd(self, x, m, m8, cfg, st):
+    sc = self.scorer
+    _C.check(_C.lib.tfr_dasalc_fwd_tasks(_C.ptr(x), _C.ptr(self.emb), sc.context_dim, m, cfg,
+                                         _C.ptr(sc.flat.data), _C.ptr(m8), _C.ptr(self.ws),
+                                         _C.ptr(self.scores), len(self.tasks), sc._precision,
+                                         st))
+
+  def _scorer_bwd(self, x, m, m8, cfg, scorer_grads, st):
+    sc = self.scorer
+    _C.check(_C.lib.tfr_dasalc_bwd_tasks(_C.ptr(x), m, cfg, _C.ptr(sc.flat.data),
+                                         _C.ptr(self.dscores), self._w_host, _C.ptr(m8),
+                                         _C.ptr(self.ws), scorer_grads, _C.ptr(self.d_emb),
+                                         sc.context_dim, len(self.tasks), sc._precision, st))
 
 
 class HostBatchPipeline(object):
