@@ -44,7 +44,9 @@ def main():
   ap.add_argument('--num_layers', type=int, default=12)
   ap.add_argument('--num_heads', type=int, default=12)
   ap.add_argument('--intermediate_size', type=int, default=3072)
-  ap.add_argument('--precision', choices=('fp32', 'tf32'), default='fp32')
+  # bf16: the reference's runtime.mixed_precision_dtype 'mixed_bfloat16' (fp32 variables, bf16
+  # compute).  'mixed_float16' (fp16 with loss scaling) is not offered.
+  ap.add_argument('--precision', choices=('fp32', 'tf32', 'bf16'), default='fp32')
   ap.add_argument('--seed', type=int, default=1234)
   args = ap.parse_args()
 

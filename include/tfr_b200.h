@@ -670,6 +670,30 @@ int tfr_symmetric_log1p_clip(const float* X, size_t n, float cutoff, float* out,
  * 3xTF32 and the attention core in FP32 CUDA-core FMA; TFR_PREC_TF32 runs the GEMMs in one
  * TF32 pass and the attention core on wgmma TF32 (as tfr_din_cfg).  LayerNorm, GELU, softmax,
  * masking, dropout and the head are fp32 in both.
+ * TFR_PREC_BF16 (mixed precision, Keras' 'mixed_bfloat16' policy): parameters, optimizer state
+ * and gradients stay fp32 in the same flat layout (a checkpoint does not depend on precision);
+ * the layers compute on bf16 values, rounded to nearest even at these points only:
+ *   GEMM operands     bf16 shadows of Wqkv, Wo, W1, W2, Wp, refreshed from params by every
+ *                     forward (the backward reuses them); the activations x_l, o, x', a and
+ *                     the [CLS] rows; the backward signals dy, du, dqkv, dpre
+ *   GEMM outputs      fp32 accumulation plus the fp32 bias, then rounded: qkv, y = o Wo + bo,
+ *                     u, y2 = a W2 + b2, pre = x_L[CLS] Wp + bp, and every input-side
+ *                     gradient (dO = dy Wo^T, da = dy W2^T, d x' = du W1^T, dx = dqkv Wqkv^T,
+ *                     dCLS = dpre Wp^T)
+ *   elementwise       computed in fp32, stored rounded: the LayerNorm outputs x_0, x', x''
+ *                     and a = gelu(u); du = bf16(da gelu'(u)); dy = bf16(LN backward's dz,
+ *                     dropout applied); dpre = bf16(head backward)
+ *   attention         S = q k^T (fp32 accumulation) times 1 / sqrt(dh), masking, softmax
+ *                     and dropout in fp32; P~ = bf16(dropout(P)) with P normalised;
+ *                     o = bf16(P~ v).  Backward: dP = dO v^T in fp32, D_i = dO_i . o_i over
+ *                     the stored bf16 values, dS = bf16(P (dP keep - D_i)) (the gradient of
+ *                     the scaled logits), dq = bf16((dS k) / sqrt(dh)),
+ *                     dk = bf16((dS^T q) / sqrt(dh)), dv = bf16(P~^T dO)
+ * and stay fp32: the embedding tables and their gather, LayerNorm statistics and arithmetic
+ * (xhat, rstd), the residual gradient, dgamma / dbeta, the dW partials and their fixed-order
+ * reduction, the bias gradients (fp32 column sums of the bf16 dy / du / dqkv / dpre), the
+ * embedding LayerNorm's gradient, the pooler tanh, the score head and the scores.  Dropout
+ * draws are those of the other modes.  Extra limits: E, I and dh multiples of 8.
  * Limits (TFR_INVALID_ARGUMENT before any CUDA call, and 0 from the size queries): dh = E / H
  * a multiple of 4 in [4, 128], E <= 1024, I a multiple of 4 in [4, 4096], 1 <= layers <= 24,
  * 1 <= L <= max_position <= 512, 1 <= T_v <= 16, 1 <= V < 2^30, dropout rates in [0, 1),
@@ -696,7 +720,7 @@ typedef struct {
   float output_dropout;         /* dropout_s (TFRBertScorer's bert_output_dropout) */
   int32_t training;             /* 1: dropout active; 0: inference */
   uint64_t seed;                /* vary per step; same value -> same draws */
-  int32_t precision;            /* TFR_PREC_FP32 (default) or TFR_PREC_TF32 */
+  int32_t precision;            /* TFR_PREC_FP32 (default), TFR_PREC_TF32 or TFR_PREC_BF16 */
 } tfr_bert_cfg;
 
 size_t tfr_bert_param_count(const tfr_bert_cfg* cfg);

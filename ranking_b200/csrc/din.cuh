@@ -3,6 +3,7 @@
 #pragma once
 #include <cstdint>
 
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 namespace tfr {
@@ -36,6 +37,18 @@ int din_tc_attn_fwd(const float* qkv, const uint8_t* lmask, int B, int N, int H,
 int din_tc_attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H, int h,
                     float drop, unsigned long long dseed, const float* O, const float* lse,
                     const float* dO, float* dsum, float* dqkv, cudaStream_t st);
+
+// bf16 tensor-core attention core (din_bf16.cu): qkv, O, dO and dqkv bf16, lse and dsum fp32,
+// same layouts and dropout draws.  P~ is rounded to bf16 after normalisation, before P~ v; dS
+// is rounded to bf16 before dS K and dS^T Q, and dQ / dK are scaled by 1 / sqrt(h) after
+// those products.  dsum = dO . O over the stored bf16 values.  h % 8 == 0, h <= 128.
+int din_bf16_attn_fwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                      float drop, unsigned long long dseed, __nv_bfloat16* O, float* lse,
+                      cudaStream_t st);
+int din_bf16_attn_bwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                      float drop, unsigned long long dseed, const __nv_bfloat16* O,
+                      const float* lse, const __nv_bfloat16* dO, float* dsum,
+                      __nv_bfloat16* dqkv, cudaStream_t st);
 
 // C [GM, GN] (ldc) = A B (+ bias, act) on the scorer GEMM engine, 3xTF32 (passes 3) or TF32
 // (passes 1).  a_mn / b_mn: operand stored MN-major (A^T [GK, GM], B [GK, GN]) instead of

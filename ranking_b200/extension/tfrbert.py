@@ -12,6 +12,8 @@ document) token sequence of a list, trained end to end with a ranking loss and A
 The encoder is tf-models-official's BertEncoder as TFRBertScorer uses it; its math and the
 flat parameter layout are written out in include/tfr_b200.h (K15).  There is no TF / HF
 checkpoint import: `set_weights` takes the tensors in the documented order (`weight_names`).
+Precision: 'fp32', 'tf32' or 'bf16' (the reference's 'mixed_bfloat16' policy: fp32 parameters
+and optimizer, bf16 activations, GEMMs and attention core; sizes in multiples of 8).
 """
 import ctypes
 import dataclasses
@@ -22,7 +24,7 @@ from ranking_b200 import _C
 from ranking_b200 import data as data_lib
 from ranking_b200 import train as train_lib
 
-_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32}
+_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32, 'bf16': _C.PREC_BF16}
 
 
 @dataclasses.dataclass
@@ -81,8 +83,10 @@ def _truncated_normal(gen, shape, stddev):
 class BertEncoder(object):
   """The encoder's flat parameters and configuration (pooler and score head included, so the
   scorer is one buffer: one gradient, one optimizer launch).  `precision` 'fp32' (default:
-  3xTF32 GEMMs, FP32 attention core) or 'tf32' (one TF32 pass, wgmma attention core); the
-  parameters are the same in both, so `set_precision` can switch a trained encoder.
+  3xTF32 GEMMs, FP32 attention core), 'tf32' (one TF32 pass, wgmma attention core) or 'bf16'
+  (mixed precision: bf16 activations, GEMMs and attention core on fp32 master weights, as
+  Keras' 'mixed_bfloat16' policy; hidden, intermediate and head sizes must be multiples of 8).
+  The parameters are the same in all three, so `set_precision` can switch a trained encoder.
   Initialisation (host): truncated normal with stddev `initializer_range` for the tables and
   kernels, zero biases, LayerNorm gamma 1 / beta 0."""
 
@@ -121,8 +125,12 @@ class BertEncoder(object):
     precision = precision or 'fp32'
     if precision not in _PRECISIONS:
       raise ValueError('precision must be one of %s' % sorted(_PRECISIONS))
-    self.precision = precision
+    old = getattr(self, '_precision', None)
     self._precision = _PRECISIONS[precision]
+    if _C.lib.tfr_bert_param_count(ctypes.byref(self._make_cfg(0.0))) == 0:
+      self._precision = old
+      raise ValueError(_C.last_error())
+    self.precision = precision
 
   def _make_cfg(self, output_dropout, training=False, seed=0):
     c = self.config

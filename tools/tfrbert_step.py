@@ -4,8 +4,11 @@ arms within one run:
 
   ours-fp32    3xTF32 GEMMs, FP32 attention core          (precision 'fp32')
   ours-tf32    TF32 GEMMs, wgmma TF32 attention core      (precision 'tf32')
+  ours-bf16    bf16 GEMMs and wgmma attention core on fp32 master weights (precision 'bf16')
   torch-fp32   torch autograd + torch.optim.AdamW, TF32 matmul off
   torch-tf32   the same with TF32 matmul on
+  torch-bf16   the same under torch.autocast('cuda', dtype=torch.bfloat16): ours-bf16's
+               like-for-like competitor (fp32 parameters and optimizer, bf16 compute)
 
 BERT-base (12 layers, E 768, H 12, I 3072), seq 64, lists of 10, at 4 lists (the reference
 yaml) and 32.  Dropout 0.1 everywhere in both.  Then one profiled step of each of our arms,
@@ -89,7 +92,7 @@ def _ours(precision):
   return lambda wid, mask, tid, y: tr.train_step(wid, mask, tid, y)
 
 
-def _torch(tf32):
+def _torch(tf32, bf16=False):
   torch.manual_seed(1)
   model = TorchBert().cuda().train()
   decay = [p for n, p in model.named_parameters()
@@ -102,9 +105,10 @@ def _torch(tf32):
     torch.backends.cuda.matmul.allow_tf32 = tf32
     torch.backends.cudnn.allow_tf32 = tf32
     b = wid.shape[0]
-    s = model(wid.reshape(b * N, SEQ), mask.reshape(b * N, SEQ),
-              tid.reshape(b * N, SEQ)).reshape(b, N)
-    loss = _softmax_loss(y, s)
+    with torch.autocast('cuda', dtype=torch.bfloat16, enabled=bf16):
+      s = model(wid.reshape(b * N, SEQ), mask.reshape(b * N, SEQ),
+                tid.reshape(b * N, SEQ)).reshape(b, N)
+    loss = _softmax_loss(y, s.float())
     opt.zero_grad(set_to_none=True)
     loss.backward()
     opt.step()
@@ -116,9 +120,9 @@ _FAMILIES = [('embedding', ('emb_ln', 'embedding', 'radix', 'segment', 'scatter_
              ('attention', ('attn_',)),
              ('ffn_gelu', ('gelu',)),
              ('layernorm', ('ln_fwd', 'ln_bwd', 'reduce_partials')),
-             ('pooler_loss', ('head_', 'loss', 'softmax')),
+             ('pooler_loss', ('head_', 'loss', 'softmax', 'cls_scatter')),
              ('optimizer', ('adamw',)),
-             ('gemm', ('gemm', 'wgmma', 'colsum', 'tc_', 'weight_grad', 'split'))]
+             ('gemm', ('gemm', 'wgmma', 'colsum', 'tc_', 'weight_grad', 'split', 'shadow'))]
 
 
 def _family(name):
@@ -149,8 +153,9 @@ def main():
   lines = []
   for b in args.lists:
     batch = _batch(b)
-    arms = {'ours-fp32': _ours('fp32'), 'ours-tf32': _ours('tf32'),
-            'torch-fp32': _torch(False), 'torch-tf32': _torch(True)}
+    arms = {'ours-fp32': _ours('fp32'), 'ours-tf32': _ours('tf32'), 'ours-bf16': _ours('bf16'),
+            'torch-fp32': _torch(False), 'torch-tf32': _torch(True),
+            'torch-bf16': _torch(True, bf16=True)}
     for fn in arms.values():
       for _ in range(args.warmup):
         fn(*batch)
@@ -171,7 +176,7 @@ def main():
              'ms_rounds': ts, 'gpu': gpu, 'power_limit_and_max_sm_clock': power}
       lines.append(rec)
       print(json.dumps(rec), flush=True)
-    for name in ('ours-fp32', 'ours-tf32'):
+    for name in ('ours-fp32', 'ours-tf32', 'ours-bf16'):
       fn = arms[name]
       with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         fn(*batch)
