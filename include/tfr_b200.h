@@ -940,6 +940,24 @@ int tfr_tc_gemm_bf16(const void* A, int lda, const void* B, int ldb, void* C, in
                      float* colsum, int colsum_stride, int* colsum_slots_out,
                      int splits, size_t split_stride, void* stream);
 
+/* Parity helpers for TFR-BERT's bf16 attention core (csrc/din_bf16.cu; the rounding points
+ * are K15's TFR_PREC_BF16 "attention" row).  Layouts as the DIN's attention core (K11):
+ * qkv bf16 [B N, 3 H h] (q, k, v blocks of H heads of h columns), lmask uint8 [B N] (0 = key
+ * masked with the -1e9 adder; NULL = all valid), O bf16 [B N, H h], lse fp32 [B N, H, 2] =
+ * {row max, 1 / sum} (exact for a list with no valid item: 1 / sum = float(1 / N)),
+ * dsum fp32 [B N, H] = dO . O over the stored bf16 values, dO bf16 [B N, H h], dqkv bf16
+ * [B N, 3 H h].  Dropout of P with rate `drop` keeps element ((b H + head) N + i) N + j iff
+ * u(dseed, e) >= drop, with dseed the combined site seed (seed * 0x100000001B3 + site).
+ * Limits (TFR_INVALID_ARGUMENT before any CUDA call): NULL qkv / O / lse (and dO / dsum /
+ * dqkv), h a multiple of 8 in [8, 128], 1 <= N <= TFR_DIN_MAX_LIST, H >= 1,
+ * H h <= TFR_BERT_MAX_HIDDEN, drop in [0, 1), every buffer but lmask 16-byte aligned.
+ * B = 0 launches nothing. */
+int tfr_attn_bf16_fwd(const void* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                      float drop, unsigned long long dseed, void* O, float* lse, void* stream);
+int tfr_attn_bf16_bwd(const void* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                      float drop, unsigned long long dseed, const void* O, const float* lse,
+                      const void* dO, float* dsum, void* dqkv, void* stream);
+
 /* ---------------------------------------------------------------------------
  * Input side (host code, no device work): a batch of serialized
  * `ExampleListWithContext` protos -> dense float buffers, with the padding /

@@ -566,4 +566,57 @@ int din_bf16_attn_bwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int
                                dqkv, st);
 }
 
+namespace {
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// The parity entries' limits: those of TFR-BERT's bf16 mode (tfr_bert_*), checked before any
+// CUDA call.
+int check_attn(const void* qkv, int B, int N, int H, int h, float drop) {
+  TFR_REQUIRE(qkv, "bf16 attention: NULL qkv");
+  TFR_REQUIRE(h >= 8 && h <= 128 && h % 8 == 0,
+              "bf16 attention: head size %d must be a multiple of 8 in [8, 128]", h);
+  TFR_REQUIRE(N >= 1 && N <= TFR_DIN_MAX_LIST, "bf16 attention: N %d must be in [1, %d]", N,
+              TFR_DIN_MAX_LIST);
+  TFR_REQUIRE(H >= 1 && (long long)H * h <= TFR_BERT_MAX_HIDDEN,
+              "bf16 attention: %d heads of %d exceed %d columns", H, h, TFR_BERT_MAX_HIDDEN);
+  TFR_REQUIRE(B >= 0 && (long long)B * H * ((N + kT - 1) / kT) <= 0x7fffffffLL,
+              "bf16 attention: batch %d out of range", B);
+  TFR_REQUIRE(drop >= 0.f && drop < 1.f, "bf16 attention: dropout rate must be in [0, 1)");
+  return TFR_OK;
+}
+
+}  // namespace
 }  // namespace tfr
+
+// Parity entries: the bf16 attention core alone (see include/tfr_b200.h).
+extern "C" int tfr_attn_bf16_fwd(const void* qkv, const uint8_t* lmask, int B, int N, int H,
+                                 int h, float drop, unsigned long long dseed, void* O, float* lse,
+                                 void* stream) {
+  using namespace tfr;
+  int rc = check_attn(qkv, B, N, H, h, drop);
+  if (rc) return rc;
+  TFR_REQUIRE(O && lse, "bf16 attention: NULL output");
+  TFR_REQUIRE(aligned16(qkv) && aligned16(O) && aligned16(lse),
+              "bf16 attention: operands must be 16-byte aligned");
+  if (B == 0) return TFR_OK;
+  return din_bf16_attn_fwd(static_cast<const bf16*>(qkv), lmask, B, N, H, h, drop, dseed,
+                           static_cast<bf16*>(O), lse, (cudaStream_t)stream);
+}
+
+extern "C" int tfr_attn_bf16_bwd(const void* qkv, const uint8_t* lmask, int B, int N, int H,
+                                 int h, float drop, unsigned long long dseed, const void* O,
+                                 const float* lse, const void* dO, float* dsum, void* dqkv,
+                                 void* stream) {
+  using namespace tfr;
+  int rc = check_attn(qkv, B, N, H, h, drop);
+  if (rc) return rc;
+  TFR_REQUIRE(O && lse && dO && dsum && dqkv, "bf16 attention: NULL operand");
+  TFR_REQUIRE(aligned16(qkv) && aligned16(O) && aligned16(lse) && aligned16(dO) &&
+                  aligned16(dsum) && aligned16(dqkv),
+              "bf16 attention: operands must be 16-byte aligned");
+  if (B == 0) return TFR_OK;
+  return din_bf16_attn_bwd(static_cast<const bf16*>(qkv), lmask, B, N, H, h, drop, dseed,
+                           static_cast<const bf16*>(O), lse, static_cast<const bf16*>(dO), dsum,
+                           static_cast<bf16*>(dqkv), (cudaStream_t)stream);
+}

@@ -15,6 +15,7 @@ import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
+SENTINEL = 7.0
 
 
 def _pack_bits(keep):
@@ -27,12 +28,19 @@ def _pack_bits(keep):
   return words.t().contiguous().to(torch.int32)
 
 
-def run_kmajor(gm, gn, gk, epi=0, act=0, want_bits=False, want_colsum=False, seed=0):
-  """mn = 0: C[gm, gn] (bf16) = A[gm, gk] B[gn, gk]^T."""
+def run_kmajor(gm, gn, gk, epi=0, act=0, want_bits=False, want_colsum=False, seed=0, lda=None,
+               ldc=None):
+  """mn = 0: C[gm, gn] (bf16, row pitch ldc) = A[gm, gk] (row pitch lda) B[gn, gk]^T.  The
+  columns [gk, lda) of A hold values that must not be read, the columns [gn, ldc) of C a
+  sentinel that must stay."""
   import ranking_b200  # noqa: F401
   from ranking_b200 import _C
   g = torch.Generator().manual_seed(seed)
-  A = torch.randn(gm, gk, generator=g).bfloat16()
+  lda = lda or gk
+  ldc = ldc or gn
+  A_full = torch.randn(gm, lda, generator=g).bfloat16()
+  A_full[:, gk:] = 1e4
+  A = A_full[:, :gk]
   B = torch.randn(gn, gk, generator=g).bfloat16()
   bias = torch.randn(gn, generator=g)
   keep = torch.rand(gm, gn, generator=g) > 0.4
@@ -44,8 +52,9 @@ def run_kmajor(gm, gn, gk, epi=0, act=0, want_bits=False, want_colsum=False, see
       ref = torch.relu(ref)
   elif epi == 3:
     ref = torch.where(keep, ref, torch.zeros_like(ref))
-  a_d, b_d, bias_d = A.cuda(), B.cuda(), bias.cuda()
-  C = torch.full((gm, gn), float('nan'), dtype=torch.bfloat16, device='cuda')
+  a_d, b_d, bias_d = A_full.cuda(), B.cuda(), bias.cuda()
+  C = torch.full((gm, ldc), SENTINEL, dtype=torch.bfloat16, device='cuda')
+  C[:, :gn] = float('nan')
   bits_out = bits_in = colsum = None
   slots = (torch.zeros(1, dtype=torch.int32))
   import ctypes
@@ -58,11 +67,13 @@ def run_kmajor(gm, gn, gk, epi=0, act=0, want_bits=False, want_colsum=False, see
   if want_colsum:
     colsum = torch.full((148 * 8, stride), float('nan'), device='cuda')
   rc = _C.lib.tfr_tc_gemm_bf16(
-      _C.ptr(a_d), gk, _C.ptr(b_d), gk, _C.ptr(C), gn, gm, gn, gk, 0, epi, _C.ptr(bias_d),
+      _C.ptr(a_d), lda, _C.ptr(b_d), gk, _C.ptr(C), ldc, gm, gn, gk, 0, epi, _C.ptr(bias_d),
       act, _C.ptr(bits_out), _C.ptr(bits_in), _C.ptr(colsum), stride,
       ctypes.cast(ctypes.byref(nslots), ctypes.c_void_p), 1, 0, _C.stream())
   _C.check(rc)
   torch.cuda.synchronize()
+  assert (C[:, gn:].float() == SENTINEL).all(), 'columns past GN written'
+  C = C[:, :gn]
   out = C.double().cpu()
   err = float(((out - ref).abs() - 2.0 ** -8 * ref.abs()).clamp(min=0).div(scale + 1e-30).max())
   if want_bits:
@@ -76,24 +87,32 @@ def run_kmajor(gm, gn, gk, epi=0, act=0, want_bits=False, want_colsum=False, see
   return err, out, ref
 
 
-def run_mnmajor(gm, gn, gk, splits, seed=0):
-  """mn = 1: C[gm, gn] (fp32, summed over the split partials) = A[gk, gm]^T B[gk, gn]."""
+def run_mnmajor(gm, gn, gk, splits, seed=0, lda=None, ldc=None):
+  """mn = 1: C[gm, gn] (fp32, summed over the split partials; row pitch ldc) = A[gk, gm]^T
+  (row pitch lda) B[gk, gn].  Columns [gm, lda) of A must not be read, columns [gn, ldc) of
+  every partial keep their sentinel."""
   import ranking_b200  # noqa: F401
   from ranking_b200 import _C
   g = torch.Generator().manual_seed(seed)
-  A = torch.randn(gk, gm, generator=g).bfloat16()
+  lda = lda or gm
+  ldc = ldc or gn
+  A_full = torch.randn(gk, lda, generator=g).bfloat16()
+  A_full[:, gm:] = 1e4
+  A = A_full[:, :gm]
   B = torch.randn(gk, gn, generator=g).bfloat16()
   ref = A.double().t() @ B.double()
   scale = A.double().abs().t() @ B.double().abs()
-  a_d, b_d = A.cuda(), B.cuda()
+  a_d, b_d = A_full.cuda(), B.cuda()
   rows = (gm + 127) // 128 * 128
-  C = torch.full((splits, rows, gn), float('nan'), device='cuda')
+  C = torch.full((splits, rows, ldc), SENTINEL, device='cuda')
+  C[:, :gm, :gn] = float('nan')
   rc = _C.lib.tfr_tc_gemm_bf16(
-      _C.ptr(a_d), gm, _C.ptr(b_d), gn, _C.ptr(C), gn, gm, gn, gk, 1, 0, None, 0, None, None,
-      None, 0, None, splits, rows * gn, _C.stream())
+      _C.ptr(a_d), lda, _C.ptr(b_d), gn, _C.ptr(C), ldc, gm, gn, gk, 1, 0, None, 0, None, None,
+      None, 0, None, splits, rows * ldc, _C.stream())
   _C.check(rc)
   torch.cuda.synchronize()
-  out = C[:, :gm].double().sum(0).cpu()
+  assert (C[:, :, gn:] == SENTINEL).all(), 'columns past GN written'
+  out = C[:, :gm, :gn].double().sum(0).cpu()
   err = float(((out - ref).abs() / (scale + 1e-30)).max())
   return err, out, ref
 
@@ -124,6 +143,75 @@ def test_bf16_gemm_kmajor_epilogues(shape):
 def test_bf16_gemm_mnmajor(shape):
   err, _, _ = run_mnmajor(*shape, seed=sum(shape))
   assert err <= 2e-6, err
+
+
+def dw_splits(sms, kin, nout, rows):
+  """csrc/bert.cu dw_splits: the split count TFR-BERT's bf16 dW GEMMs launch."""
+  tiles = ((kin + 127) // 128) * ((nout + 127) // 128)
+  nkb = (rows + 63) // 64
+  best, best_t = 1, 0.0
+  for s in range(1, min(16, nkb) + 1):
+    per = (nkb + s - 1) // s
+    if (nkb + per - 1) // per != s:
+      continue
+    t = ((tiles * s + sms - 1) // sms) * per * 0.46e-6 + s * kin * nout * 8.0 / 3e12
+    if s == 1 or t < best_t:
+      best, best_t = s, t
+  return best
+
+
+# TFR-BERT's calls (csrc/bert.cu bgemm / dense_grad_bf16), (GM, GN, GK, lda, ldc, bias):
+# the pooler on the [CLS] rows (GM = S, lda = L E), GN = 3E or I up to 4096, GK = I up to 4096.
+BERT_KM = [(5, 768, 768, 64 * 768, 768, True),       # pooler, BERT-base
+           (1, 1024, 1024, 512 * 1024, 1032, True),  # pooler, one sequence, ldc > GN
+           (130, 600, 200, 200, 608, True),          # qkv at E 200
+           (256, 2304, 768, 768, 2304, True),        # qkv, BERT-base
+           (200, 3072, 768, 768, 3072, True),        # u = x' W1
+           (136, 4096, 1024, 1024, 4104, False),     # u at I 4096, ldc > GN
+           (70, 240, 1032, 1032, 240, True),         # y2 = a W2 at I 1032
+           (256, 768, 3072, 3072, 768, True),        # y2, BERT-base
+           (130, 1024, 4096, 4096, 1024, False)]     # d x' = du W1^T at I 4096
+# dW (mn = 1), (GM = Kin, GN = Nout, GK = rows, lda, ldc, splits): the pooler's dW over S
+# [CLS] rows (A strided by L E) and the dW of the layers, split as dw_splits picks.
+BERT_MN = [(768, 768, gk, 64 * 768, 768, 1) for gk in (1, 2, 5, 63, 64, 65)] + [
+    (64, 64, 5, 7 * 64, 72, 1),                        # ldc > GN
+    (4096, 1024, 520, 4096, 1024, None),              # dW2 at I 4096 (Kin = 4096)
+    (4096, 64, 1937, 4096, 64, None),
+    (64, 192, 1937, 64, 200, None),                   # 16 splits, the last one block short
+    (136, 408, 3000, 136, 408, None)]
+
+
+def _bert_id(c):
+  return 'x'.join(str(v) for v in c)
+
+
+@pytest.mark.parametrize('shape', BERT_KM, ids=_bert_id)
+def test_bf16_gemm_kmajor_bert_calls(shape):
+  gm, gn, gk, lda, ldc, bias = shape
+  err, _, _ = run_kmajor(gm, gn, gk, epi=1 if bias else 0, act=0, seed=gm + gn + gk, lda=lda,
+                         ldc=ldc)
+  print('[bf16 gemm bert mn=0 %s] err %.2e (bar 1e-5)' % (_bert_id(shape), err))
+  assert err <= 1e-5, err
+
+
+@pytest.mark.parametrize('shape', BERT_MN, ids=_bert_id)
+def test_bf16_gemm_mnmajor_bert_calls(shape):
+  gm, gn, gk, lda, ldc, splits = shape
+  splits = splits or dw_splits(132, gm, gn, gk)
+  err, _, _ = run_mnmajor(gm, gn, gk, splits, seed=gm + gn + gk, lda=lda, ldc=ldc)
+  print('[bf16 gemm bert mn=1 %s] splits %d, err %.2e (bar 2e-6)' %
+        (_bert_id(shape), splits, err))
+  assert err <= 2e-6, err
+
+
+def test_bert_dw_split_counts():
+  """The dW shapes above reach dw_splits' 16 with a shorter last split, and more than one."""
+  counts = {c[:3]: dw_splits(132, *c[:3]) for c in BERT_MN if c[5] is None}
+  assert counts[(64, 192, 1937)] == 16
+  nkb = (1937 + 63) // 64
+  per = (nkb + 15) // 16
+  assert nkb - 15 * per < per   # the last split is shorter
+  assert any(1 < s < 16 for s in counts.values()), counts
 
 
 if __name__ == '__main__':

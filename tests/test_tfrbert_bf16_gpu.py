@@ -20,7 +20,9 @@ pytestmark = pytest.mark.gpu
 
 V, P, TV = T.V, T.P, T.TV
 
-#        S, L,   E,    H,  I,    NL    (dh = E / H); every case has an all-padded item
+#        S, L,   E,    H,  I,    NL    (dh = E / H); every case has an all-padded item.  The
+# head sizes cover every bucket of the bf16 attention core (16 / 32 / 64 / 128) and a padded one
+# in each.
 CASES = [(6, 7, 64, 4, 520, 1),        # dh 16, I not a multiple of 64
          (4, 65, 200, 5, 520, 2),      # dh 40 (bucket 64), E 200, L past one 64-row tile
          (3, 64, 128, 2, 1032, 3),     # dh 64, three layers
@@ -28,7 +30,11 @@ CASES = [(6, 7, 64, 4, 520, 1),        # dh 16, I not a multiple of 64
          (2, 128, 256, 2, 520, 1),     # dh 128, L 128
          (2, 16, 768, 12, 3072, 1),    # BERT-base widths
          (2, 8, 1024, 16, 1032, 1),    # E 1024
-         (2, 512, 64, 4, 136, 1)]      # L 512
+         (2, 512, 64, 4, 136, 1),      # L 512
+         (4, 33, 64, 8, 64, 1),        # dh 8 (half of bucket 16 is padding)
+         (3, 130, 96, 4, 136, 1),      # dh 24 (bucket 32), L past two 64-row tiles
+         (3, 130, 64, 2, 136, 1),      # dh 32
+         (2, 70, 240, 2, 248, 1)]      # dh 120 (a partly padded bucket 128)
 # RMS check: the kernels against the replay, at most 1/8 of the rounding's own effect (the
 # replay against the unrounded reference).  What separates the kernels from the replay are
 # roundings that flip between fp32 and fp64 accumulation, one bf16 unit each, and their RMS
