@@ -9,7 +9,9 @@ first tenth of the steps and linear decay to 0, and the best checkpoint by MAP.
 
 Input is ELWC with example features `input_ids`, `input_mask`, `segment_ids` (int64,
 seq_length each) and an int `relevance` label (--label).  The encoder starts from its
-initialisation: no TF / HF checkpoint is read.
+initialisation, or, as the recipe fine-tunes, from a pretrained BERT (--init_checkpoint: a TF2
+BertEncoder checkpoint or a Hugging Face model; sizes from --bert_config_file or the
+config.json beside it).  --gradient_clip_norm 1.0 is the recipe's AdamWeightDecay clipping.
 """
 import argparse
 import os
@@ -39,30 +41,59 @@ def main():
   ap.add_argument('--learning_rate', type=float, default=3e-5)
   ap.add_argument('--weight_decay_rate', type=float, default=0.01)
   ap.add_argument('--dropout_rate', type=float, default=0.1)
-  ap.add_argument('--vocab_size', type=int, default=30522)
-  ap.add_argument('--hidden_size', type=int, default=768)
-  ap.add_argument('--num_layers', type=int, default=12)
-  ap.add_argument('--num_heads', type=int, default=12)
-  ap.add_argument('--intermediate_size', type=int, default=3072)
+  # encoder sizes: default BERT-base; with --bert_config_file / --init_checkpoint they come
+  # from the config, and a size flag that disagrees with it is an error
+  ap.add_argument('--vocab_size', type=int, default=None, help='default 30522')
+  ap.add_argument('--hidden_size', type=int, default=None, help='default 768')
+  ap.add_argument('--num_layers', type=int, default=None, help='default 12')
+  ap.add_argument('--num_heads', type=int, default=None, help='default 12')
+  ap.add_argument('--intermediate_size', type=int, default=None, help='default 3072')
+  ap.add_argument('--init_checkpoint', default=None,
+                  help='pretrained encoder: TF2 BertEncoder checkpoint prefix, Hugging Face '
+                       'model.safetensors / pytorch_model.bin, or a directory holding one')
+  ap.add_argument('--bert_config_file', default=None,
+                  help='BERT / Hugging Face config.json (default: the one beside '
+                       '--init_checkpoint)')
+  ap.add_argument('--gradient_clip_norm', type=float, default=0.0,
+                  help='clip gradients to this global norm before AdamW; 0 = off (the '
+                       "reference recipe's AdamWeightDecay uses 1.0)")
   # bf16: the reference's runtime.mixed_precision_dtype 'mixed_bfloat16' (fp32 variables, bf16
   # compute).  'mixed_float16' (fp16 with loss scaling) is not offered.
   ap.add_argument('--precision', choices=('fp32', 'tf32', 'bf16'), default='fp32')
   ap.add_argument('--seed', type=int, default=1234)
   args = ap.parse_args()
+  if args.gradient_clip_norm < 0:
+    ap.error('--gradient_clip_norm must be >= 0')
 
-  cfg = tfrbert.BertEncoderConfig(vocab_size=args.vocab_size, hidden_size=args.hidden_size,
-                                  num_layers=args.num_layers,
-                                  num_attention_heads=args.num_heads,
-                                  intermediate_size=args.intermediate_size,
-                                  hidden_dropout_prob=args.dropout_rate,
-                                  attention_dropout_prob=args.dropout_rate)
+  sizes = {'vocab_size': args.vocab_size, 'hidden_size': args.hidden_size,
+           'num_layers': args.num_layers, 'num_attention_heads': args.num_heads,
+           'intermediate_size': args.intermediate_size}
+  config_file = args.bert_config_file
+  if config_file is None and args.init_checkpoint is not None:
+    config_file = tfrbert.config_beside(args.init_checkpoint)
+    if config_file is None:
+      ap.error('no config.json beside --init_checkpoint; pass --bert_config_file')
+  if config_file is not None:
+    cfg = tfrbert.BertEncoderConfig.from_json(config_file)
+    for field, value in sizes.items():
+      if value is not None and value != getattr(cfg, field):
+        ap.error('--%s %d disagrees with %s (%s %d)' %
+                 (field if field != 'num_attention_heads' else 'num_heads', value,
+                  config_file, field, getattr(cfg, field)))
+  else:
+    cfg = tfrbert.BertEncoderConfig(**{k: v for k, v in sizes.items() if v is not None})
+  # the recipe's dropout rates (BERT's 0.1 by default) replace the config file's
+  cfg.hidden_dropout_prob = cfg.attention_dropout_prob = args.dropout_rate
   encoder = tfrbert.BertEncoder(cfg, seed=args.seed, precision=args.precision)
+  if args.init_checkpoint is not None:
+    encoder.load_checkpoint(args.init_checkpoint)
   scorer = tfrbert.TFRBertScorer(encoder, bert_output_dropout=args.dropout_rate)
   warmup = args.train_steps // 10 if args.warmup_steps is None else args.warmup_steps
   schedule = train.PolynomialWarmUp(args.learning_rate, args.train_steps, warmup)
   trainer = tfrbert.TFRBertRankingTrainer(scorer, losses.get('softmax_loss'),
                                           learning_rate=schedule,
-                                          weight_decay_rate=args.weight_decay_rate)
+                                          weight_decay_rate=args.weight_decay_rate,
+                                          gradient_clip_norm=args.gradient_clip_norm or None)
 
   def batches(paths, drop_remainder=True):
     return tfrbert.tfrbert_batches(paths, args.batch_size, args.list_size, args.seq_length,

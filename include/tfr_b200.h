@@ -1067,6 +1067,36 @@ int tfr_adamw_step(float* params, const float* grads, float* m, float* v,
                    const uint8_t* decay_mask, size_t n, float lr, float beta1, float beta2,
                    float eps, float weight_decay, int64_t step, float grad_scale, void* stream);
 
+/* Global-norm gradient clipping, as tf-models' AdamWeightDecay applies it before the update
+ * (gradient_clip_norm, 1.0 in BERT's fine-tuning recipe; tf.clip_by_global_norm).
+ *
+ * tfr_global_norm writes ||x||_2 = sqrt(sum_i x_i^2) of n floats to *norm_out (device).  The
+ * squares are summed in double in a fixed order: per-block partials over fixed grid-stride
+ * positions (of float4s when x is 16-byte aligned), then one ordered final sum, so two
+ * identical calls give identical bits.  inf or NaN inputs give an inf or NaN norm; so does,
+ * once rounded to float, a finite norm above FLT_MAX (~3.4e38).  The workspace (device, >= the bytes
+ * tfr_global_norm_workspace_bytes(n) returns, 8 per block) holds the partials; n = 0 writes
+ * 0.  No host synchronisation.  TFR_INVALID_ARGUMENT for NULL norm_out / workspace, NULL x
+ * with n > 0, or a short workspace.
+ *
+ * tfr_adamw_step_clipped is tfr_adamw_step with every gradient multiplied, after grad_scale,
+ * by s read from `norm` (device, the global norm of grads * grad_scale):
+ *   s = 1                     norm <= clip_norm   (exactly tfr_adamw_step's bits)
+ *   s = clip_norm / norm      norm >  clip_norm
+ *   s = NaN                   norm inf or NaN     (every clipped gradient is NaN; with
+ *                                                  tfr_global_norm's norm that includes a
+ *                                                  gradient whose norm exceeds FLT_MAX)
+ * The weight-decay term is not scaled.  The scale is applied inside the update kernel: no
+ * extra pass over the gradient and no host synchronisation.  TFR_INVALID_ARGUMENT as
+ * tfr_adamw_step, and for NULL norm or clip_norm not finite and > 0. */
+size_t tfr_global_norm_workspace_bytes(size_t n);
+int tfr_global_norm(const float* x, size_t n, float* norm_out, void* workspace,
+                    size_t workspace_bytes, void* stream);
+int tfr_adamw_step_clipped(float* params, const float* grads, float* m, float* v,
+                           const uint8_t* decay_mask, size_t n, float lr, float beta1,
+                           float beta2, float eps, float weight_decay, int64_t step,
+                           float grad_scale, float clip_norm, const float* norm, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K7  data-parallel step: all-reduce(SUM) of the flat gradient fused with the optimizer,
  * over NVLink peer memory (one process per GPU on one node).  Replaces the reference's

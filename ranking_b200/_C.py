@@ -217,6 +217,10 @@ _SIGNATURES = {
     'tfr_optimizer_step': (_I, [_P, _P, _P, C.c_size_t, _I, _F, _F, _F, _P]),
     'tfr_adamw_step': (_I, [_P, _P, _P, _P, _P, C.c_size_t, _F, _F, _F, _F, _F, C.c_int64, _F,
                             _P]),
+    'tfr_global_norm_workspace_bytes': (C.c_size_t, [C.c_size_t]),
+    'tfr_global_norm': (_I, [_P, C.c_size_t, _P, _P, C.c_size_t, _P]),
+    'tfr_adamw_step_clipped': (_I, [_P, _P, _P, _P, _P, C.c_size_t, _F, _F, _F, _F, _F,
+                                    C.c_int64, _F, _F, _P, _P]),
     'tfr_bert_param_count': (C.c_size_t, [C.POINTER(BertCfg)]),
     'tfr_bert_workspace_bytes': (C.c_size_t, [C.POINTER(BertCfg), _I, _I]),
     'tfr_bert_fwd': (_I, [_P, _P, _P, _I, _I, C.POINTER(BertCfg), _P, _P, _P, _P, _P]),

@@ -1,6 +1,7 @@
 // C-ABI glue: error string, scorer-tower dispatch, fused optimizer.
 #include <atomic>
 #include <cmath>
+#include <cstdint>
 #include <cstring>
 
 #include "common.cuh"
@@ -204,13 +205,24 @@ optimizer_kernel(float* __restrict__ params, const float* __restrict__ grads,
 
 
 // AdamWeightDecay; step_size = lr sqrt(1 - beta2^t) / (1 - beta1^t) (host, double).
+// Clip: g is scaled by the global-norm factor read from *norm (the header's contract); the
+// factor is exactly 1 when the norm is within clip_norm, so those steps keep the unclipped bits.
+template <bool Clip>
 __global__ void __launch_bounds__(256)
 adamw_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ m,
              float* __restrict__ v, const uint8_t* __restrict__ decay_mask, size_t n, float lr,
-             float beta1, float beta2, float eps, float wd, float step_size, float grad_scale) {
+             float beta1, float beta2, float eps, float wd, float step_size, float grad_scale,
+             float clip_norm, const float* __restrict__ norm) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float g = grads[i] * grad_scale;
+  float g = grads[i] * grad_scale;
+  if (Clip) {
+    const float nrm = *norm;
+    // tf.clip_by_global_norm: an inf or NaN norm makes every clipped gradient NaN
+    const float s = !isfinite(nrm) ? __int_as_float(0x7fc00000)
+                                   : (nrm <= clip_norm ? 1.f : clip_norm / nrm);
+    g *= s;
+  }
   const float mi = beta1 * m[i] + (1.f - beta1) * g;
   const float vi = beta2 * v[i] + (1.f - beta2) * g * g;
   m[i] = mi;
@@ -218,6 +230,77 @@ adamw_kernel(float* __restrict__ params, const float* __restrict__ grads, float*
   float p = params[i];
   if (!decay_mask || decay_mask[i]) p -= lr * wd * p;
   params[i] = p - step_size * mi / (sqrtf(vi) + eps);
+}
+
+// Global L2 norm, in two fixed-order passes.  Pass 1: thread t of block b sums squares (in
+// double) over fixed positions p = b * 256 + t + k * norm_blocks(n) * 256 -- float4 number p
+// when x is 16-byte aligned (the n % 4 tail elements then go to the first threads of block 0),
+// float number p otherwise -- and the block reduces them in a fixed tree.  Pass 2: one block
+// sums the per-block partials the same way and writes sqrt as float.
+constexpr int kNormThreads = 256;
+constexpr int kNormPerThread = 16;   // elements per thread before the grid saturates
+constexpr int kNormMaxBlocks = 2048;
+
+static unsigned norm_blocks(size_t n) {
+  const size_t per_block = (size_t)kNormThreads * kNormPerThread;
+  const size_t b = (n + per_block - 1) / per_block;
+  return (unsigned)(b < 1 ? 1 : (b > kNormMaxBlocks ? kNormMaxBlocks : b));
+}
+
+__device__ __forceinline__ double block_sum_fixed(double x, double* sh) {
+  // fixed shuffle tree inside each warp, then warp 0 over the warp sums in warp order
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) sh[warp] = x;
+  __syncthreads();
+  x = 0.0;
+  if (warp == 0) {
+    const int nw = blockDim.x >> 5;
+    x = lane < nw ? sh[lane] : 0.0;
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  }
+  return x;   // valid in thread 0
+}
+
+__global__ void __launch_bounds__(kNormThreads)
+sumsq_partials_kernel(const float* __restrict__ x, size_t n, double* __restrict__ partials) {
+  __shared__ double sh[kNormThreads / 32];
+  const size_t stride = (size_t)gridDim.x * kNormThreads;
+  const size_t first = (size_t)blockIdx.x * kNormThreads + threadIdx.x;
+  double a0 = 0.0, a1 = 0.0;   // two chains, so the FMA latency does not throttle the loads
+  if ((reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const float4* __restrict__ x4 = reinterpret_cast<const float4*>(x);
+    const size_t n4 = n >> 2;
+#pragma unroll 2
+    for (size_t i = first; i < n4; i += stride) {
+      const float4 v = __ldg(x4 + i);
+      a0 = fma((double)v.x, (double)v.x, a0);
+      a1 = fma((double)v.y, (double)v.y, a1);
+      a0 = fma((double)v.z, (double)v.z, a0);
+      a1 = fma((double)v.w, (double)v.w, a1);
+    }
+    if (first < (n & 3)) {
+      const double v = (double)__ldg(x + (n4 << 2) + first);
+      a0 = fma(v, v, a0);
+    }
+  } else {
+#pragma unroll 4
+    for (size_t i = first; i < n; i += stride) {
+      const double v = (double)__ldg(x + i);
+      a0 = fma(v, v, a0);
+    }
+  }
+  const double acc = block_sum_fixed(a0 + a1, sh);
+  if (threadIdx.x == 0) partials[blockIdx.x] = acc;
+}
+
+__global__ void __launch_bounds__(1024)
+norm_final_kernel(const double* __restrict__ partials, int nparts, float* __restrict__ norm) {
+  __shared__ double sh[32];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < nparts; i += blockDim.x) acc += partials[i];
+  acc = block_sum_fixed(acc, sh);
+  if (threadIdx.x == 0) *norm = (float)sqrt(acc);
 }
 }  // namespace tfr
 
@@ -422,9 +505,56 @@ extern "C" int tfr_adamw_step(float* params, const float* grads, float* m, float
   const float step_size =
       (float)((double)lr * std::sqrt(1.0 - std::pow((double)beta2, t)) /
               (1.0 - std::pow((double)beta1, t)));
-  adamw_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+  adamw_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       params, grads, m, v, decay_mask, n, lr, beta1, beta2, eps, weight_decay, step_size,
-      grad_scale);
+      grad_scale, 0.f, nullptr);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" size_t tfr_global_norm_workspace_bytes(size_t n) {
+  return (size_t)norm_blocks(n) * sizeof(double);
+}
+
+extern "C" int tfr_global_norm(const float* x, size_t n, float* norm_out, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  TFR_REQUIRE(norm_out && workspace && (x || n == 0), "NULL argument");
+  const unsigned blocks = norm_blocks(n);
+  TFR_REQUIRE(workspace_bytes >= (size_t)blocks * sizeof(double),
+              "global norm of %zu floats needs a %zu-byte workspace, got %zu", n,
+              (size_t)blocks * sizeof(double), workspace_bytes);
+  const cudaStream_t st = (cudaStream_t)stream;
+  double* partials = (double*)workspace;
+  if (n == 0) {
+    TFR_CUDA_OK(cudaMemsetAsync(norm_out, 0, sizeof(float), st));
+    return TFR_OK;
+  }
+  sumsq_partials_kernel<<<blocks, kNormThreads, 0, st>>>(x, n, partials);
+  TFR_LAUNCH_OK();
+  norm_final_kernel<<<1, 1024, 0, st>>>(partials, (int)blocks, norm_out);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" int tfr_adamw_step_clipped(float* params, const float* grads, float* m, float* v,
+                                      const uint8_t* decay_mask, size_t n, float lr,
+                                      float beta1, float beta2, float eps, float weight_decay,
+                                      int64_t step, float grad_scale, float clip_norm,
+                                      const float* norm, void* stream) {
+  TFR_REQUIRE(params && grads && m && v && norm, "NULL argument");
+  TFR_REQUIRE(step >= 1, "AdamW step %lld must be >= 1", (long long)step);
+  TFR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f,
+              "beta1 %g and beta2 %g must be in [0, 1)", (double)beta1, (double)beta2);
+  TFR_REQUIRE(clip_norm > 0.f && std::isfinite(clip_norm),
+              "clip_norm %g must be finite and > 0", (double)clip_norm);
+  if (n == 0) return TFR_OK;
+  const double t = (double)step;
+  const float step_size =
+      (float)((double)lr * std::sqrt(1.0 - std::pow((double)beta2, t)) /
+              (1.0 - std::pow((double)beta1, t)));
+  adamw_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      params, grads, m, v, decay_mask, n, lr, beta1, beta2, eps, weight_decay, step_size,
+      grad_scale, clip_norm, norm);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

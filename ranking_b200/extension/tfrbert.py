@@ -10,19 +10,24 @@ document) token sequence of a list, trained end to end with a ranking loss and A
                                        `segment_ids` (int64, dim seq_length) and a label
 
 The encoder is tf-models-official's BertEncoder as TFRBertScorer uses it; its math and the
-flat parameter layout are written out in include/tfr_b200.h (K15).  There is no TF / HF
-checkpoint import: `set_weights` takes the tensors in the documented order (`weight_names`).
+flat parameter layout are written out in include/tfr_b200.h (K15).  `set_weights` takes the
+tensors in the documented order (`weight_names`); `BertEncoder.from_pretrained` and
+`load_checkpoint` import a pretrained TF2 BertEncoder or Hugging Face BERT checkpoint
+(bert_checkpoint.py), and `BertEncoderConfig.from_json` reads its `config.json`.
 Precision: 'fp32', 'tf32' or 'bf16' (the reference's 'mixed_bfloat16' policy: fp32 parameters
 and optimizer, bf16 activations, GEMMs and attention core; sizes in multiples of 8).
 """
 import ctypes
 import dataclasses
+import json
+import os
 
 import torch
 
 from ranking_b200 import _C
 from ranking_b200 import data as data_lib
 from ranking_b200 import train as train_lib
+from ranking_b200.extension import bert_checkpoint
 
 _PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32, 'bf16': _C.PREC_BF16}
 
@@ -40,6 +45,64 @@ class BertEncoderConfig:
   hidden_dropout_prob: float = 0.1
   attention_dropout_prob: float = 0.1
   initializer_range: float = 0.02
+
+  # the encoder's GELU is the tanh form; 'gelu' is the erf form in Hugging Face (and the
+  # tanh form in Google's BERT code), so an HF 'gelu' model imported here differs from HF's
+  # own outputs by the GELU approximation
+  _HIDDEN_ACTS = ('gelu', 'gelu_new', 'gelu_pytorch_tanh')
+  _JSON_KEYS = {'vocab_size': 'vocab_size', 'hidden_size': 'hidden_size',
+                'num_hidden_layers': 'num_layers',
+                'num_attention_heads': 'num_attention_heads',
+                'intermediate_size': 'intermediate_size',
+                'max_position_embeddings': 'max_position_embeddings',
+                'type_vocab_size': 'type_vocab_size',
+                'hidden_dropout_prob': 'hidden_dropout_prob',
+                'attention_probs_dropout_prob': 'attention_dropout_prob',
+                'initializer_range': 'initializer_range'}
+
+  @classmethod
+  def from_json(cls, path):
+    """The config of a Google BERT `bert_config.json` or Hugging Face `config.json`
+    (missing keys keep their defaults).  `hidden_act` must be 'gelu_new',
+    'gelu_pytorch_tanh' or 'gelu' (see above), `layer_norm_eps` (if given) 1e-12 and
+    `position_embedding_type` (if given) 'absolute'; ValueError otherwise, and for a head
+    count that does not divide the hidden size."""
+    with open(path) as f:
+      d = json.load(f)
+    act = d.get('hidden_act', 'gelu')
+    if act not in cls._HIDDEN_ACTS:
+      raise ValueError('%s: hidden_act %r unsupported (the encoder computes the tanh GELU: '
+                       'one of %s)' % (path, act, list(cls._HIDDEN_ACTS)))
+    # the encoder's LayerNorm epsilon is BERT's 1e-12 and its positions are absolute
+    # (include/tfr_b200.h, K15); other values would import into a different model
+    eps = float(d.get('layer_norm_eps', 1e-12))
+    if eps != 1e-12:
+      raise ValueError('%s: layer_norm_eps %g unsupported (the encoder uses 1e-12)' %
+                       (path, eps))
+    pos = d.get('position_embedding_type', 'absolute')
+    if pos != 'absolute':
+      raise ValueError('%s: position_embedding_type %r unsupported (absolute only)' %
+                       (path, pos))
+    kw = {}
+    for key, field in cls._JSON_KEYS.items():
+      if key in d:
+        kw[field] = (float if field.endswith(('_prob', '_range')) else int)(d[key])
+    c = cls(**kw)
+    if c.num_attention_heads < 1 or c.hidden_size % c.num_attention_heads:
+      raise ValueError('%s: hidden_size %d is not a multiple of num_attention_heads %d' %
+                       (path, c.hidden_size, c.num_attention_heads))
+    return c
+
+
+def config_beside(checkpoint):
+  """The `config.json` or `bert_config.json` in a checkpoint's directory (or in the
+  directory itself), else None."""
+  folder = checkpoint if os.path.isdir(checkpoint) else \
+      os.path.dirname(os.path.abspath(checkpoint))
+  for name in ('config.json', 'bert_config.json'):
+    if os.path.isfile(os.path.join(folder, name)):
+      return os.path.join(folder, name)
+  return None
 
 
 def weight_shapes(config):
@@ -185,6 +248,30 @@ class BertEncoder(object):
     with torch.no_grad():
       self.flat.copy_(torch.cat(parts).to(self.flat.device))
 
+  def load_checkpoint(self, path):
+    """Overwrites every encoder weight with a pretrained checkpoint's (a TF2 BertEncoder
+    checkpoint prefix, a Hugging Face `model.safetensors` / `pytorch_model.bin`, or a
+    directory holding one); the score head keeps its values, as the reference restores only
+    the `encoder` object.  ValueError for a checkpoint that disagrees with the config."""
+    loaded = bert_checkpoint.read_bert_weights(path, self.config)
+    head = self.get_weights()[-2:]
+    self.set_weights(list(loaded.values()) + head)
+
+  @classmethod
+  def from_pretrained(cls, path, config=None, seed=None, device='cuda', precision=None):
+    """An encoder initialised from a pretrained checkpoint (see `load_checkpoint`).  The
+    config is `config`, else the `config.json` or `bert_config.json` beside the checkpoint.
+    The parameters are fp32 in every `precision`."""
+    if config is None:
+      config_file = config_beside(path)
+      if config_file is None:
+        raise ValueError('%s: no config.json or bert_config.json beside the checkpoint; '
+                         'pass config=' % path)
+      config = BertEncoderConfig.from_json(config_file)
+    enc = cls(config, seed=seed, device=device, precision=precision)
+    enc.load_checkpoint(path)
+    return enc
+
 
 class TFRBertScorer(object):
   """TFRBertScorer (tfrbert_task.py): Dropout(bert_output_dropout) on the encoder's pooled
@@ -213,9 +300,11 @@ class TFRBertRankingTrainer(train_lib.RankingTrainer):
 
   AdamW defaults are BERT's: weight_decay_rate 0.01 on every kernel and table (LayerNorm and
   biases excluded), beta_1 0.9, beta_2 0.999, epsilon 1e-6; `learning_rate` may be a float or
-  a schedule such as `train.PolynomialWarmUp`.  Padded items (label < 0) are encoded too, as in
-  the reference; the loss ignores them.  fit / evaluate / checkpoints are the base class's;
-  batches are ({'input_word_ids', 'input_mask', 'input_type_ids'}, y) pairs."""
+  a schedule such as `train.PolynomialWarmUp`; `gradient_clip_norm` (the base class's, off by
+  default; the recipe's AdamWeightDecay uses 1.0) clips to a global norm first.  Padded items
+  (label < 0) are encoded too, as in the reference; the loss ignores them.  fit / evaluate /
+  checkpoints are the base class's; batches are ({'input_word_ids', 'input_mask',
+  'input_type_ids'}, y) pairs."""
 
   def __init__(self, scorer, loss, optimizer='adamw', learning_rate=3e-5, epsilon=1e-6,
                weight_decay_rate=0.01, **kw):

@@ -59,12 +59,17 @@ class RankingTrainer(object):
   and checkpoints keep it; `learning_rate` may be a float or a schedule called with the
   0-based update index (PolynomialWarmUp); tower.decay_mask (uint8 per parameter, if the
   tower has one) picks the weights that decay.  Needs world size 1 or collective 'nccl'.
+
+  gradient_clip_norm (adamw only, world size 1; default None = off): tf-models'
+  AdamWeightDecay clipping, g *= clip / max(||g||, clip) over the whole flat gradient
+  (tfr_global_norm, then tfr_adamw_step_clipped, which scales g inside the update).
+  `grad_norm` is then a 0-d device tensor holding the last step's pre-clip norm.
   """
 
   def __init__(self, tower, loss, optimizer='adagrad', learning_rate=0.001,
                epsilon=1e-7, initial_accumulator_value=0.1, process_group=None,
                collective='fused', keep_summed_grads=False, beta_1=0.9, beta_2=0.999,
-               weight_decay_rate=0.0):
+               weight_decay_rate=0.0, gradient_clip_norm=None):
     if optimizer not in _OPT:
       raise ValueError('optimizer must be one of %s' % sorted(_OPT))
     if not hasattr(loss, 'fused_fwd_bwd'):
@@ -80,6 +85,24 @@ class RankingTrainer(object):
     self.device = dev
     self.group = process_group
     self.world = dp.world_size(process_group)
+    self.gradient_clip_norm = None
+    if gradient_clip_norm is not None:
+      clip = float(gradient_clip_norm)
+      if optimizer != 'adamw':
+        raise ValueError("gradient_clip_norm needs optimizer 'adamw', got %r" % optimizer)
+      if self.world > 1:
+        # tf-models clips each replica's gradient before the all-reduce; this trainer only
+        # sees the sum
+        raise ValueError('gradient_clip_norm supports one rank only, got world size %d' %
+                         self.world)
+      if not (clip > 0.0 and clip != float('inf')):
+        raise ValueError('gradient_clip_norm must be finite and > 0, got %r' %
+                         (gradient_clip_norm,))
+      self.gradient_clip_norm = clip
+      n = tower.flat.numel()
+      self.grad_norm = torch.zeros((), dtype=torch.float32, device=dev)
+      self._norm_ws = torch.empty(_C.lib.tfr_global_norm_workspace_bytes(n),
+                                  dtype=torch.uint8, device=dev)
     if optimizer == 'adamw':
       if self.world > 1 and collective == 'fused':
         raise ValueError("optimizer 'adamw' with more than one rank needs collective='nccl'")
@@ -172,6 +195,16 @@ class RankingTrainer(object):
       lr = self.lr(self.adam_step) if callable(self.lr) else self.lr
       self.adam_step += 1
       n = grads.numel()
+      if self.gradient_clip_norm is not None:
+        _C.check(_C.lib.tfr_global_norm(_C.ptr(grads), n, _C.ptr(self.grad_norm),
+                                         _C.ptr(self._norm_ws), self._norm_ws.numel(),
+                                         _C.stream()))
+        _C.check(_C.lib.tfr_adamw_step_clipped(
+            _C.ptr(t.flat.data), _C.ptr(grads), _C.ptr(self.accum[:n]),
+            _C.ptr(self.accum[n:]), _C.ptr(self.decay_mask), n, lr, self.beta_1, self.beta_2,
+            self.eps, self.weight_decay_rate, self.adam_step, dp.replica_grad_scale(self.group),
+            self.gradient_clip_norm, _C.ptr(self.grad_norm), _C.stream()))
+        return
       _C.check(_C.lib.tfr_adamw_step(
           _C.ptr(t.flat.data), _C.ptr(grads), _C.ptr(self.accum[:n]), _C.ptr(self.accum[n:]),
           _C.ptr(self.decay_mask), n, lr, self.beta_1, self.beta_2, self.eps,

@@ -5,6 +5,8 @@ arms within one run:
   ours-fp32    3xTF32 GEMMs, FP32 attention core          (precision 'fp32')
   ours-tf32    TF32 GEMMs, wgmma TF32 attention core      (precision 'tf32')
   ours-bf16    bf16 GEMMs and wgmma attention core on fp32 master weights (precision 'bf16')
+  ours-*-clip  the same with gradient_clip_norm 1.0 (the recipe's AdamWeightDecay clipping:
+               tfr_global_norm + tfr_adamw_step_clipped), for tf32 and bf16
   torch-fp32   torch autograd + torch.optim.AdamW, TF32 matmul off
   torch-tf32   the same with TF32 matmul on
   torch-bf16   the same under torch.autocast('cuda', dtype=torch.bfloat16): ours-bf16's
@@ -14,9 +16,11 @@ BERT-base (12 layers, E 768, H 12, I 3072), seq 64, lists of 10, at 4 lists (the
 yaml) and 32.  Dropout 0.1 everywhere in both.  Then one profiled step of each of our arms,
 kernel time summed by family (embedding, attention, FFN, LayerNorm, GEMM, pooler and loss,
 optimizer).  Prints one JSON line per (shape, arm) and one per profile; writes them to
---out too.
+--out too.  --arms picks a subset (the profiles cover the chosen ours-* arms).
 
   python tools/tfrbert_step.py --steps 20 --warmup 5 --out /tmp/tfrbert_step.jsonl
+  python tools/tfrbert_step.py --lists 32 --arms ours-tf32 ours-tf32-clip ours-bf16 \
+      ours-bf16-clip
 """
 import argparse
 import json
@@ -85,10 +89,11 @@ def _softmax_loss(y, s):
   return -(p * torch.log_softmax(s, 1)).sum(1)[keep].sum() / max(int(keep.sum()), 1)
 
 
-def _ours(precision):
+def _ours(precision, clip=None):
   enc = tfrbert.BertEncoder(seed=1, precision=precision)
   tr = tfrbert.TFRBertRankingTrainer(tfrbert.TFRBertScorer(enc, 0.1), losses.get('softmax_loss'),
-                                     learning_rate=train.PolynomialWarmUp(3e-5, 10000, 1000))
+                                     learning_rate=train.PolynomialWarmUp(3e-5, 10000, 1000),
+                                     gradient_clip_norm=clip)
   return lambda wid, mask, tid, y: tr.train_step(wid, mask, tid, y)
 
 
@@ -121,7 +126,7 @@ _FAMILIES = [('embedding', ('emb_ln', 'embedding', 'radix', 'segment', 'scatter_
              ('ffn_gelu', ('gelu',)),
              ('layernorm', ('ln_fwd', 'ln_bwd', 'reduce_partials')),
              ('pooler_loss', ('head_', 'loss', 'softmax', 'cls_scatter')),
-             ('optimizer', ('adamw',)),
+             ('optimizer', ('adamw', 'sumsq_partials', 'norm_final')),
              ('gemm', ('gemm', 'wgmma', 'colsum', 'tc_', 'weight_grad', 'split', 'shadow'))]
 
 
@@ -133,6 +138,12 @@ def _family(name):
   return 'other'
 
 
+_ARMS = {'ours-fp32': lambda: _ours('fp32'), 'ours-tf32': lambda: _ours('tf32'),
+         'ours-tf32-clip': lambda: _ours('tf32', 1.0), 'ours-bf16': lambda: _ours('bf16'),
+         'ours-bf16-clip': lambda: _ours('bf16', 1.0), 'torch-fp32': lambda: _torch(False),
+         'torch-tf32': lambda: _torch(True), 'torch-bf16': lambda: _torch(True, bf16=True)}
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--steps', type=int, default=20)
@@ -140,6 +151,8 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--lists', type=int, nargs='+', default=[4, 32])
   ap.add_argument('--out')
+  ap.add_argument('--arms', nargs='+', choices=sorted(_ARMS), default=None,
+                  help='default: every arm')
   args = ap.parse_args()
   if not torch.cuda.is_available():
     raise SystemExit('tfrbert_step: no CUDA device')
@@ -153,9 +166,8 @@ def main():
   lines = []
   for b in args.lists:
     batch = _batch(b)
-    arms = {'ours-fp32': _ours('fp32'), 'ours-tf32': _ours('tf32'), 'ours-bf16': _ours('bf16'),
-            'torch-fp32': _torch(False), 'torch-tf32': _torch(True),
-            'torch-bf16': _torch(True, bf16=True)}
+    arms = {name: make() for name, make in _ARMS.items()
+            if args.arms is None or name in args.arms}
     for fn in arms.values():
       for _ in range(args.warmup):
         fn(*batch)
@@ -176,7 +188,7 @@ def main():
              'ms_rounds': ts, 'gpu': gpu, 'power_limit_and_max_sm_clock': power}
       lines.append(rec)
       print(json.dumps(rec), flush=True)
-    for name in ('ours-fp32', 'ours-tf32', 'ours-bf16'):
+    for name in [a for a in arms if a.startswith('ours-')]:
       fn = arms[name]
       with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         fn(*batch)
