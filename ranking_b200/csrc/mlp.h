@@ -116,7 +116,9 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
                      float* ws, float* grads, int passes, cudaStream_t st,
                      const TaskWeights* tw = nullptr);
 // Tower input gradient for columns [col0, col0 + ncols) after mlp_tc_bwd (no input BN,
-// at least one hidden layer): tfr_mlp_input_grad.
+// at least one hidden layer): tfr_mlp_input_grad.  After a backward that took the fused dW_0
+// kernel (mlp_tc_fused_bwd_ok) it first recomputes dZ_0 into the workspace's dZ_0 region;
+// nothing mlp_tc_bwd returns depends on that region.
 int mlp_tc_input_grad(int M, const MlpPlan& p, const float* params, float* ws, int col0,
                       int ncols, float* dX, int ldx, int passes, cudaStream_t st);
 // The three roles of Dense d's GEMMs on the TF32 engine.  Apart from the split kernel and
@@ -153,6 +155,16 @@ bool mlp_tc_fused_fwd_ok(int first_layer, const float* X, int M, const MlpPlan& 
 int mlp_tc_fused_fwd(int first_layer, const float* X, int M, const MlpPlan& p,
                      const float* params, const uint8_t* mask, float* ws, float* scores,
                      cudaStream_t st, bool planar = false);
+// Fused 3xTF32 backward of Dense 0 (mlp_tc_fused_bwd.cu): from dZ_1, dZ_0 = (dZ_1 W_1^T) *
+// relu'(H_0) and dW_0 in one kernel, into dW_0's split-K partial slots (ws + partial_off) and
+// one db_0 column-sum slot per split (ws + tile_off), for mlp_reduce2; dZ_0 is not stored.
+// dW_0 is bit-identical to mlp_tc_dense_dgrad(d = 1) then mlp_tc_weight_grad(d = 0).  _ok
+// says whether mlp_tc_bwd takes it: 3xTF32, no BN / dropout / input BN, ReLU or no
+// activation, at least two hidden layers, dims[0] <= 136 in dW_0's swapped orientation,
+// dims[1] and dims[2] <= 256, a 16-byte aligned workspace.  Expects the parameters split.
+bool mlp_tc_fused_bwd_ok(const MlpPlan& p, int passes, const float* ws);
+int mlp_tc_fused_dw0(const float* X, const float* dz1, int M, const MlpPlan& p, float* ws,
+                     cudaStream_t st);
 
 // pieces of the CUDA-core path reused by the tensor-core path
 int mlp_out_layer_fwd(const float* H, int M, int K, int O, const float* W, const float* bias,

@@ -205,6 +205,17 @@ int mlp_tc_fwd_from(int first_layer, const float* X, int M, const MlpPlan& p,
                            params + p.b_off[L], mask, scores, st, planar);
 }
 
+bool mlp_tc_fused_bwd_ok(const MlpPlan& p, int passes, const float* ws) {
+  const int L = p.n_dense - 1;
+  if (passes != 3 || p.post() || p.input_bn || L < 2) return false;
+  if (p.activation != TFR_ACT_RELU && p.activation != TFR_ACT_NONE) return false;
+  if (p.dims[0] > 136 || p.dims[1] > 256 || p.dims[2] > 256) return false;
+  // dW_0 in the swapped orientation mlp_tc_weight_grad picks (dZ_0 the A operand), whose one
+  // column tile of dims[0] <= 136 the kernel keeps in registers
+  if (tc::tile_units(p.dims[1], p.dims[0]) >= tc::tile_units(p.dims[0], p.dims[1])) return false;
+  return (reinterpret_cast<uintptr_t>(ws) & 15) == 0;
+}
+
 int mlp_tc_bwd(const float* X, int M, const MlpPlan& p, const float* params,
                const float* dscores, const uint8_t* mask, float* ws, float* grads,
                int passes, cudaStream_t st, const TaskWeights* tw) {
@@ -254,6 +265,7 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
   const float* bsrc = oslots + (((size_t)p.dims[L] * p.dims[L + 1] + p.dims[L + 1] + 3) & ~(size_t)3);
   int bslots = p.out_slots;
   size_t bstride = p.oslot_stride;
+  const bool fused0 = stop_layer == 0 && mlp_tc_fused_bwd_ok(p, passes, ws);
   for (int d = L - 1; d >= stop_layer; --d) {
     const int Kin = p.dims[d], Nout = p.dims[d + 1];
     const float* A = d > 0 ? ws + p.act_off[d - 1] : X0;
@@ -269,6 +281,14 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
     rc = mlp_tc_weight_grad(A, Kin, Kin, dz_cur, Nout, Nout, M, splits, partial, pstride, bsrc,
                             bslots, bstride, false, grads + p.w_off[d], passes, st);
     if (rc) return rc;
+    if (d == 1 && fused0) {
+      // dZ_0 and dW_0's partials in one kernel (dZ_0 is not stored), db_0 from its per-split
+      // column sums
+      rc = mlp_tc_fused_dw0(X0, dz_cur, M, p, ws, st);
+      if (rc) return rc;
+      return mlp_reduce2(partial, splits, pstride, (size_t)p.dims[0] * Kin, tiles, splits,
+                         p.tile_stride, (size_t)Kin, grads + p.w_off[0], st);
+    }
     if (d > 0 || p.input_bn) {   // d == 0 with input BN: dL/dXin for its gamma / beta
       const bool masked = d > 0 && mact != TFR_ACT_NONE;
       const bool sums = d > 0 && !p.post();
@@ -297,12 +317,21 @@ int mlp_tc_bwd_until(int stop_layer, MlpBwdTail* tail, const float* X, int M, co
 }
 
 // dX[:, 0:ncols] = dZ_0 W_0[col0:col0 + ncols, :]^T.  Without input BN, mlp_tc_bwd leaves dZ_0
-// in the ping-pong buffer it started from after L - 1 swaps.
+// in the ping-pong buffer it started from after L - 1 swaps.  A backward that took the fused
+// dW_0 kernel left dZ_1 in the other buffer and no dZ_0: it is recomputed first by the same
+// GEMM the per-layer walk runs, so it has the same bits.
 int mlp_tc_input_grad(int M, const MlpPlan& p, const float* params, float* ws, int col0,
                       int ncols, float* dX, int ldx, int passes, cudaStream_t st) {
   int rc = check_dims(p);
   if (rc) return rc;
   const int L = p.n_dense - 1;
+  if (mlp_tc_fused_bwd_ok(p, passes, ws)) {
+    rc = mlp_tc_dense_dgrad(
+        p, 1, 0, p.dims[1], ws + p.dz_off[L & 1], M, params, ws,
+        p.activation == TFR_ACT_RELU ? reinterpret_cast<const uint32_t*>(ws + p.bits_off[0]) : nullptr,
+        nullptr, 0, nullptr, ws + p.dz_off[(L - 1) & 1], p.dims[1], passes, st);
+    if (rc) return rc;
+  }
   return mlp_tc_dense_dgrad(p, 0, col0, ncols, ws + p.dz_off[(L - 1) & 1], M, params, ws,
                             nullptr, nullptr, 0, nullptr, dX, ldx, passes, st);
 }

@@ -634,6 +634,64 @@ __device__ __forceinline__ void producer_ring(const Args& args, unsigned char* s
   }
 }
 
+// producer_ring's slab copy and in-place transpose, for a kernel that runs its own ring
+// (mlp_tc_fused_bwd.cu).  copy_slab: producer thread pt (0..127) copies k rows k0 .. k0 + 31 of B
+// [GK][GN] (row pitch ldb) raw into the B tile at `dst`, columns n0 .. n0 + 127 as 32 rows of
+// BN * 4 bytes, then (FOLD) the `tail` folded columns past them as 32 rows of 32 bytes at
+// kTileBytes; zero past GK and GN.  One cp.async group's worth; the caller commits it.
+template <bool FOLD>
+__device__ __forceinline__ void copy_slab(const float* src, int ldb, int GK, int GN, uint32_t dst,
+                                          int n0, int k0, int tail, int pt) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = pt + i * kEpiThreads;
+    const int k = c >> 5, nc = c & 31, n = n0 + nc * 4;
+    const int cnt = k0 + k < GK ? min(max(GN - n, 0), 4) : 0;
+    const float* p = cnt > 0 ? src + static_cast<size_t>(k0 + k) * ldb + n : src;
+    cp_async16(dst + k * (BN * 4) + nc * 16, p, cnt * 4);
+  }
+  if (FOLD && pt < 64) {   // [32 k][8 columns], two chunks per k row
+    const int k = pt >> 1, h = pt & 1;
+    const int cnt = k0 + k < GK ? min(max(tail - 4 * h, 0), 4) : 0;
+    const float* p = cnt > 0 ? src + static_cast<size_t>(k0 + k) * ldb + n0 + BN + 4 * h : src;
+    cp_async16(dst + kTileBytes + k * 32 + h * 16, p, cnt * 4);
+  }
+}
+// Producer thread pt: the landed slab in tile `t` transposed in place into the swizzled K-major
+// tile (and, SPLIT, split into t = hi and lo).  Every producer thread takes part: it holds a
+// barrier over the 128 between its reads and its writes.
+template <bool SPLIT, bool FOLD>
+__device__ __forceinline__ void transpose_slab(unsigned char* t, unsigned char* lo, int pt) {
+  const int lane = pt & 31, pw = pt >> 5;
+  // opaque per call: keeps ptxas from holding every store offset in registers across blocks
+  int qw = pw * 4 + (lane >> 3), q = pt;
+  asm volatile("" : "+r"(qw), "+r"(q));
+  float4 v[2][4];
+  float tv[2];
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const int slot = qw + 16 * b, kc = slot >> 2, r = 4 * (8 * (slot & 3) + (lane & 7));
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      v[b][i] = *reinterpret_cast<const float4*>(t + (4 * kc + i) * (BN * 4) + r * 4);
+  }
+  if (FOLD) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      tv[e] = *reinterpret_cast<const float*>(t + kTileBytes + ((q >> 3) + 16 * e) * 32 + (q & 7) * 4);
+  }
+  bar_sync(kBarProd, kEpiThreads);   // the whole slab is read before any of it is overwritten
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const int slot = qw + 16 * b;
+    store_mn_block<SPLIT>(t, lo, v[b], slot >> 2, 4 * (8 * (slot & 3) + (lane & 7)));
+  }
+  if (FOLD) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) store_mn_tail<SPLIT>(t, lo, tv[e], (q >> 3) + 16 * e, q & 7);
+  }
+}
+
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));

@@ -9,7 +9,9 @@ shapes and split-K count as dw1-dw3.  The last line times the
 whole 3xTF32 forward of the config-2 tower (136-256-128-64-1, the fused kernel) through
 tfr_mlp_fwd: X read once; H1, H2, H3, their sign words and the scores written once.  It
 also prints fwd1 + fwd2 + fwd3 from the same run, the per-layer forward's GEMMs, to compare
-against.
+against.  The line after it times the fused dW_0 backward kernel (tower_fused_dw0_kernel, which
+replaces dz1 + dw1 with the same splits) at the config-2 shapes: its device time from
+torch.profiler over a tfr_mlp_bwd loop of the config-2 tower, against dz1 + dw1 from this run.
 usage: gemm_only.py [--reps R] [--warmup W] [--out FILE.json]"""
 import argparse
 import json
@@ -133,12 +135,18 @@ def main():
         '(fwd1 + fwd2 + fwd3 %.1f us, %+.1f %%)' % (
             M, fwd['us'], fwd['tflops'], fwd['gbps'], per_layer,
             100.0 * (fwd['us'] / per_layer - 1.0)), flush=True)
+  fused = time_fused_dw0(dev, g, args.reps, args.warmup, sms)
+  pair = sum(r['us'] for r in step if r['gemm'] in ('dz1', 'dw1'))
+  print('fused dW_0 (tower_fused_dw0_kernel, M %d, %d units)  %8.1f us  %6.2f us/tile-half  '
+        '(dz1 + dw1 %.1f us, %+.1f %%)' % (
+            M, fused['units'], fused['us'], fused['us_per_tile_half'], pair,
+            100.0 * (fused['us'] / pair - 1.0)), flush=True)
   if args.out:
     with open(args.out, 'w') as f:
       json.dump(dict(device=torch.cuda.get_device_name(dev), sms=sms, reps=args.reps,
                      gemms=rows, total_us=round(total, 2), dw_us=round(dw, 2),
                      dwt_us=round(dwt, 2), fwd_per_layer_us=round(per_layer, 2),
-                     tower_fwd=fwd), f, indent=1)
+                     tower_fwd=fwd, fused_dw0=fused, dz1_dw1_us=round(pair, 2)), f, indent=1)
 
 
 def time_tower_fwd(dev, g, reps, warmup):
@@ -171,6 +179,48 @@ def time_tower_fwd(dev, g, reps, warmup):
   nbytes = 4 * M * (DIMS[0] + sum(DIMS[1:]) + words + 1)
   return dict(m=M, us=round(us, 2), tflops=round(flop / us * 1e-6, 2),
               gbps=round(nbytes / us * 1e-3, 1), bytes=nbytes, flop=flop)
+
+
+def time_fused_dw0(dev, g, reps, warmup, sms):
+  """Device time of tower_fused_dw0_kernel per call, from torch.profiler over `reps` backward
+  calls of the config-2 tower (the kernel runs once per call).  A work unit is one row split
+  times one 128-column half of dZ_0; a tile-half is one 128-row tile of a unit."""
+  import ctypes
+  from ranking_b200.keras import layers
+  tower = layers.create_tower(DIMS[1:], 1, activation='relu', use_batch_norm=False, dropout=0,
+                              input_dim=DIMS[0], seed=0, precision='tf32x3')
+  x = torch.randn(M, DIMS[0], device=dev, generator=g)
+  ds = torch.randn(M, device=dev, generator=g)
+  ws = tower._new_workspace(M)
+  out = torch.empty(M, 1, device=dev)
+  grads = torch.empty_like(tower.flat.data)
+  cfg = tower._run_cfg()
+  _C.check(_C.lib.tfr_mlp_fwd(_C.ptr(x), M, ctypes.byref(cfg), _C.ptr(tower.flat.data), None,
+                              _C.ptr(ws), _C.ptr(out), _C.PREC_TF32X3, _C.stream()))
+
+  def call():
+    _C.check(_C.lib.tfr_mlp_bwd(_C.ptr(x), M, ctypes.byref(cfg), _C.ptr(tower.flat.data),
+                                _C.ptr(ds), None, _C.ptr(ws), _C.ptr(grads), _C.PREC_TF32X3,
+                                _C.stream()))
+  for _ in range(warmup):
+    call()
+  torch.cuda.synchronize()
+  from torch.profiler import ProfilerActivity, profile
+  with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(reps):
+      call()
+    torch.cuda.synchronize()
+  ev = [e for e in prof.key_averages() if 'tower_fused_dw0_kernel' in e.key]
+  if len(ev) != 1 or ev[0].count != reps:
+    raise RuntimeError('expected %d tower_fused_dw0_kernel launches, profiled %s' % (
+        reps, [(e.key, e.count) for e in ev]))
+  us = ev[0].device_time_total / reps
+  splits = splits_for(M, sms)
+  units = 2 * splits
+  rows = ((M + 31) // 32 + splits - 1) // splits * 32
+  tiles = sum((min(M, (s + 1) * rows) - s * rows + 127) // 128 for s in range(splits)) * 2
+  return dict(us=round(us, 2), units=units, tile_halves=tiles,
+              us_per_tile_half=round(us * min(units, sms) / tiles, 3))
 
 
 if __name__ == '__main__':
