@@ -67,7 +67,8 @@ group_count_kernel(const int* __restrict__ inv, int S, int B, int N, int gs,
 }
 
 // H1[r, :] = act(b1 + sum_j P_j[b * N + idx[r, j], :]), r = b * G + g; sign bits as in the
-// GEMM epilogue: word [(col / 32) * M + r].  One thread per 4 columns.
+// GEMM epilogue: word [(col / 32) * M + r].  One thread per 4 columns.  A member index
+// outside [0, N) adds nothing: it is never dereferenced (tfr_group_mlp_check reports it).
 __global__ void __launch_bounds__(256)
 group_gather_fwd_kernel(const float* __restrict__ P, size_t p_stride, const int32_t* __restrict__ idx,
                         int M, int N, int G, int gs, int H, const float* __restrict__ bias, int act,
@@ -84,6 +85,7 @@ group_gather_fwd_kernel(const float* __restrict__ P, size_t p_stride, const int3
     acc = __ldg(reinterpret_cast<const float4*>(bias) + c4);
     for (int j = 0; j < gs; ++j) {
       const int i = idx[r * gs + j];
+      if ((unsigned)i >= (unsigned)N) continue;
       const float4 v = __ldg(reinterpret_cast<const float4*>(P + (size_t)j * p_stride +
                                                              ((size_t)b * N + i) * H) + c4);
       acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
@@ -146,6 +148,8 @@ group_scatter_mean_fwd_kernel(const float* __restrict__ gscore, const int* __res
   logits[bi] = c > 0.f ? acc / c : 0.f;
 }
 
+// dgscore[b, g, j] = dlogits[b, idx[b, g, j]] / cnt for valid groups; 0 for invalid groups and
+// for a member index outside [0, N), which is never dereferenced.
 __global__ void __launch_bounds__(256)
 group_scatter_mean_bwd_kernel(const float* __restrict__ dlogits, const int32_t* __restrict__ idx,
                               const uint8_t* __restrict__ gmask, const float* __restrict__ cnt,
@@ -155,8 +159,9 @@ group_scatter_mean_bwd_kernel(const float* __restrict__ dlogits, const int32_t* 
   const size_t bg = t / gs;
   const int b = (int)(bg / G);
   float v = 0.f;
-  if (gmask[bg]) {
-    const size_t bi = (size_t)b * N + idx[t];
+  const int i = idx[t];
+  if (gmask[bg] && (unsigned)i < (unsigned)N) {
+    const size_t bi = (size_t)b * N + i;
     const float c = cnt[bi];
     v = c > 0.f ? dlogits[bi] / c : 0.f;
   }
