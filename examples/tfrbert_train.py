@@ -12,6 +12,8 @@ seq_length each) and an int `relevance` label (--label).  The encoder starts fro
 initialisation, or, as the recipe fine-tunes, from a pretrained BERT (--init_checkpoint: a TF2
 BertEncoder checkpoint or a Hugging Face model; sizes from --bert_config_file or the
 config.json beside it).  --gradient_clip_norm 1.0 is the recipe's AdamWeightDecay clipping.
+--precision fp16 is the recipe's mixed_float16, the policy it names for GPUs, with dynamic
+loss scaling (--loss_scale).
 """
 import argparse
 import os
@@ -57,13 +59,23 @@ def main():
   ap.add_argument('--gradient_clip_norm', type=float, default=0.0,
                   help='clip gradients to this global norm before AdamW; 0 = off (the '
                        "reference recipe's AdamWeightDecay uses 1.0)")
-  # bf16: the reference's runtime.mixed_precision_dtype 'mixed_bfloat16' (fp32 variables, bf16
-  # compute).  'mixed_float16' (fp16 with loss scaling) is not offered.
-  ap.add_argument('--precision', choices=('fp32', 'tf32', 'bf16'), default='fp32')
+  # the reference's runtime.mixed_precision_dtype: bf16 is 'mixed_bfloat16' (fp32 variables,
+  # bf16 compute), fp16 is 'mixed_float16' (fp32 variables, fp16 compute, loss scaling)
+  ap.add_argument('--precision', choices=('fp32', 'tf32', 'bf16', 'fp16'), default='fp32',
+                  help="fp16 = the reference's mixed_float16, bf16 = its mixed_bfloat16")
+  ap.add_argument('--loss_scale', default='dynamic',
+                  help="fp16 only: 'dynamic' (Keras' dynamic loss scale, from 2^15) or a "
+                       'fixed scale')
   ap.add_argument('--seed', type=int, default=1234)
   args = ap.parse_args()
   if args.gradient_clip_norm < 0:
     ap.error('--gradient_clip_norm must be >= 0')
+  loss_scale = args.loss_scale
+  if loss_scale != 'dynamic':
+    try:
+      loss_scale = float(loss_scale)
+    except ValueError:
+      ap.error("--loss_scale must be 'dynamic' or a number")
 
   sizes = {'vocab_size': args.vocab_size, 'hidden_size': args.hidden_size,
            'num_layers': args.num_layers, 'num_attention_heads': args.num_heads,
@@ -93,7 +105,8 @@ def main():
   trainer = tfrbert.TFRBertRankingTrainer(scorer, losses.get('softmax_loss'),
                                           learning_rate=schedule,
                                           weight_decay_rate=args.weight_decay_rate,
-                                          gradient_clip_norm=args.gradient_clip_norm or None)
+                                          gradient_clip_norm=args.gradient_clip_norm or None,
+                                          loss_scale=loss_scale)
 
   def batches(paths, drop_remainder=True):
     return tfrbert.tfrbert_batches(paths, args.batch_size, args.list_size, args.seq_length,

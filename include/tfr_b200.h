@@ -371,12 +371,15 @@ int tfr_weighted_sum(const float* v, const float* w, int n, float scale,
  *   TFR_PREC_TF32X3 wgmma tf32, 3-pass error-compensated split (~fp32)
  *   TFR_PREC_TF32   wgmma tf32, 1 pass
  *   TFR_PREC_BF16   wgmma bf16 (bf16 operands, fp32 accumulate)
+ *   TFR_PREC_FP16   wgmma fp16 (fp16 operands, fp32 accumulate): TFR-BERT only (K15); every
+ *                   other entry point refuses it as it refuses an unknown value
  * ------------------------------------------------------------------------- */
 typedef enum {
   TFR_PREC_FP32 = 0,
   TFR_PREC_TF32X3 = 1,
   TFR_PREC_TF32 = 2,
-  TFR_PREC_BF16 = 3
+  TFR_PREC_BF16 = 3,
+  TFR_PREC_FP16 = 4
 } tfr_precision;
 
 typedef enum { TFR_ACT_NONE = 0, TFR_ACT_RELU = 1 } tfr_activation;
@@ -694,6 +697,18 @@ int tfr_symmetric_log1p_clip(const float* X, size_t n, float cutoff, float* out,
  * reduction, the bias gradients (fp32 column sums of the bf16 dy / du / dqkv / dpre), the
  * embedding LayerNorm's gradient, the pooler tanh, the score head and the scores.  Dropout
  * draws are those of the other modes.  Extra limits: E, I and dh multiples of 8.
+ * TFR_PREC_FP16 (mixed precision, Keras' 'mixed_float16' policy, the one the reference's recipe
+ * names for GPUs): TFR_PREC_BF16's contract word for word with IEEE binary16 (fp16: 11
+ * significant bits, round to nearest even, subnormals kept) in place of bf16 at every rounding
+ * point above; the same fp32 values, dropout draws and extra limits.  Out of range: a value
+ * whose magnitude rounds past 65504 is stored as +-inf, and every kernel passes inf and NaN on
+ * as IEEE arithmetic gives them (nothing is clamped), so an overflow anywhere in the backward
+ * reaches the gradient as inf or NaN.  Dynamic loss scaling (below, after AdamW) relies on
+ * that.
+ * Loss scaling: tfr_bert_bwd is linear in dscores in every mode.  A caller that passes
+ * S * dscores (tfr_loss_scale_mul) gets every backward signal, and the fp32 gradient, scaled
+ * by S: that is the whole interface between the encoder and the loss scale.  In fp16 it lifts
+ * small backward signals out of fp16's subnormal range (below 2^-14, and 0 below 2^-25).
  * Limits (TFR_INVALID_ARGUMENT before any CUDA call, and 0 from the size queries): dh = E / H
  * a multiple of 4 in [4, 128], E <= 1024, I a multiple of 4 in [4, 4096], 1 <= layers <= 24,
  * 1 <= L <= max_position <= 512, 1 <= T_v <= 16, 1 <= V < 2^30, dropout rates in [0, 1),
@@ -720,7 +735,8 @@ typedef struct {
   float output_dropout;         /* dropout_s (TFRBertScorer's bert_output_dropout) */
   int32_t training;             /* 1: dropout active; 0: inference */
   uint64_t seed;                /* vary per step; same value -> same draws */
-  int32_t precision;            /* TFR_PREC_FP32 (default), TFR_PREC_TF32 or TFR_PREC_BF16 */
+  int32_t precision;            /* TFR_PREC_FP32 (default), TFR_PREC_TF32, TFR_PREC_BF16 or
+                                   TFR_PREC_FP16 */
 } tfr_bert_cfg;
 
 size_t tfr_bert_param_count(const tfr_bert_cfg* cfg);
@@ -939,6 +955,14 @@ int tfr_tc_gemm_bf16(const void* A, int lda, const void* B, int ldb, void* C, in
                      uint32_t* mask_bits_out, const uint32_t* mask_bits_in,
                      float* colsum, int colsum_stride, int* colsum_slots_out,
                      int splits, size_t split_stride, void* stream);
+/* The same engine on fp16 operands (TFR-BERT's TFR_PREC_FP16): every argument and layout as
+ * tfr_tc_gemm_bf16, with fp16 in place of bf16 (a 16-bit C is fp16, rounded to nearest even;
+ * magnitudes past 65504 are stored as inf). */
+int tfr_tc_gemm_f16(const void* A, int lda, const void* B, int ldb, void* C, int ldc,
+                    int GM, int GN, int GK, int mn, int epi, const float* bias, int act,
+                    uint32_t* mask_bits_out, const uint32_t* mask_bits_in,
+                    float* colsum, int colsum_stride, int* colsum_slots_out,
+                    int splits, size_t split_stride, void* stream);
 
 /* Parity helpers for TFR-BERT's bf16 attention core (csrc/din_bf16.cu; the rounding points
  * are K15's TFR_PREC_BF16 "attention" row).  Layouts as the DIN's attention core (K11):
@@ -957,6 +981,13 @@ int tfr_attn_bf16_fwd(const void* qkv, const uint8_t* lmask, int B, int N, int H
 int tfr_attn_bf16_bwd(const void* qkv, const uint8_t* lmask, int B, int N, int H, int h,
                       float drop, unsigned long long dseed, const void* O, const float* lse,
                       const void* dO, float* dsum, void* dqkv, void* stream);
+/* The same core on fp16 (K15's TFR_PREC_FP16): arguments, layouts, limits and rounding points
+ * as tfr_attn_bf16_*, with fp16 in place of bf16. */
+int tfr_attn_f16_fwd(const void* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                     float drop, unsigned long long dseed, void* O, float* lse, void* stream);
+int tfr_attn_f16_bwd(const void* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                     float drop, unsigned long long dseed, const void* O, const float* lse,
+                     const void* dO, float* dsum, void* dqkv, void* stream);
 
 /* ---------------------------------------------------------------------------
  * Input side (host code, no device work): a batch of serialized
@@ -1096,6 +1127,40 @@ int tfr_adamw_step_clipped(float* params, const float* grads, float* m, float* v
                            const uint8_t* decay_mask, size_t n, float lr, float beta1,
                            float beta2, float eps, float weight_decay, int64_t step,
                            float grad_scale, float clip_norm, const float* norm, void* stream);
+
+/* Dynamic loss scaling, the rule of Keras' LossScaleOptimizer(dynamic=True) (Keras is not part
+ * of the reference, so this is the contract).  State: the scale S (float, device; initial 2^15)
+ * and a good-step counter c (int64, device; initial 0); growth_steps (Keras'
+ * dynamic_growth_steps) 2000 by default.  One step, with g_s = the gradient of S * loss
+ * (tfr_loss_scale_mul on dscores, then the backward) and N = tfr_global_norm(g_s):
+ *   N finite       g = g_s * (1 / S)  (Keras' unscale); with clipping, the factor of
+ *                  tfr_adamw_step_clipped on the unscaled norm N_u = float((double) N / S);
+ *                  then the AdamW update of tfr_adamw_step.  c += 1; when c reaches
+ *                  growth_steps, S = 2 S (kept only if finite) and c = 0
+ *   N inf or NaN   (any inf or NaN element; also a finite gradient whose norm exceeds FLT_MAX,
+ *                  which Keras would apply) params, m and v are left bit for bit as they are;
+ *                  S = max(S / 2, 1), c = 0
+ * The update count t (bias correction, learning-rate schedule) advances on a skipped step too:
+ * Keras' skip branch increments the inner optimizer's `iterations`.  With a fixed scale S never
+ * changes and c is not kept; a non-finite step is still skipped (Keras would apply it).
+ * Everything runs on the device, in stream order, with no host synchronisation:
+ *   tfr_loss_scale_mul     out[i] = x[i] * *scale over n floats (out may alias x)
+ *   tfr_adamw_step_scaled  the update above, reading N from *norm and S from *scale; clip_norm
+ *                          0 disables clipping, else it must be finite and > 0 (the
+ *                          TFR_INVALID_ARGUMENT rules of tfr_adamw_step otherwise; no
+ *                          grad_scale: one replica)
+ *   tfr_loss_scale_update  one thread, launched after tfr_adamw_step_scaled (which must read
+ *                          the old S): *unscaled_norm = float((double) N / S) (optional),
+ *                          then S and c by the rule above; growth_steps 0 (a fixed scale)
+ *                          leaves S and c (c may then be NULL).  TFR_INVALID_ARGUMENT for NULL
+ *                          scale / norm or growth_steps < 0. */
+int tfr_loss_scale_mul(const float* x, size_t n, const float* scale, float* out, void* stream);
+int tfr_adamw_step_scaled(float* params, const float* grads, float* m, float* v,
+                          const uint8_t* decay_mask, size_t n, float lr, float beta1,
+                          float beta2, float eps, float weight_decay, int64_t step,
+                          float clip_norm, const float* norm, const float* scale, void* stream);
+int tfr_loss_scale_update(float* scale, int64_t* good_steps, const float* norm,
+                          float* unscaled_norm, int64_t growth_steps, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K7  data-parallel step: all-reduce(SUM) of the flat gradient fused with the optimizer,

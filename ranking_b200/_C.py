@@ -25,7 +25,7 @@ PHI_LOGISTIC, PHI_HINGE, PHI_SOFT_ZERO_ONE, PHI_MSE = 0, 1, 2, 3
  LAMBDA_PRECISION) = range(6)
 GAIN_IDENTITY, GAIN_POW2_MINUS_1, GAIN_TABLE = 0, 1, 2
 DISC_INVERSE, DISC_LOG2_INVERSE, DISC_LOG1P_INVERSE, DISC_TABLE = 0, 1, 2, 3
-PREC_FP32, PREC_TF32X3, PREC_TF32, PREC_BF16 = 0, 1, 2, 3
+PREC_FP32, PREC_TF32X3, PREC_TF32, PREC_BF16, PREC_FP16 = 0, 1, 2, 3, 4
 ACT_NONE, ACT_RELU = 0, 1
 MLP_MAX_LAYERS = 8
 GAM_MAX_FEATURES, GAM_MAX_HIDDEN, GAM_MAX_CONTEXT = 512, 4, 16
@@ -205,6 +205,11 @@ _SIGNATURES = {
                          _P, _P, _I, _I, _I, C.c_size_t, _P, _P, _P]),
     'tfr_tc_gemm_bf16': (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P,
                               _I, _P, _I, C.c_size_t, _P]),
+    'tfr_tc_gemm_f16': (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P,
+                             _I, _P, _I, C.c_size_t, _P]),
+    'tfr_attn_f16_fwd': (_I, [_P, _P, _I, _I, _I, _I, _F, C.c_uint64, _P, _P, _P]),
+    'tfr_attn_f16_bwd': (_I, [_P, _P, _I, _I, _I, _I, _F, C.c_uint64, _P, _P, _P, _P, _P,
+                              _P]),
     'tfr_attn_bf16_fwd': (_I, [_P, _P, _I, _I, _I, _I, _F, C.c_uint64, _P, _P, _P]),
     'tfr_attn_bf16_bwd': (_I, [_P, _P, _I, _I, _I, _I, _F, C.c_uint64, _P, _P, _P, _P, _P,
                                _P]),
@@ -221,6 +226,10 @@ _SIGNATURES = {
     'tfr_global_norm': (_I, [_P, C.c_size_t, _P, _P, C.c_size_t, _P]),
     'tfr_adamw_step_clipped': (_I, [_P, _P, _P, _P, _P, C.c_size_t, _F, _F, _F, _F, _F,
                                     C.c_int64, _F, _F, _P, _P]),
+    'tfr_loss_scale_mul': (_I, [_P, C.c_size_t, _P, _P, _P]),
+    'tfr_adamw_step_scaled': (_I, [_P, _P, _P, _P, _P, C.c_size_t, _F, _F, _F, _F, _F,
+                                   C.c_int64, _F, _P, _P, _P]),
+    'tfr_loss_scale_update': (_I, [_P, _P, _P, _P, C.c_int64, _P]),
     'tfr_bert_param_count': (C.c_size_t, [C.POINTER(BertCfg)]),
     'tfr_bert_workspace_bytes': (C.c_size_t, [C.POINTER(BertCfg), _I, _I]),
     'tfr_bert_fwd': (_I, [_P, _P, _P, _I, _I, C.POINTER(BertCfg), _P, _P, _P, _P, _P]),

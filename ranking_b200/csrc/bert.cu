@@ -18,8 +18,10 @@
 // the embedding tables' gradients are tfr_embedding_bwd's radix-sorted segment sums, so two
 // identical calls give identical bits.
 #include <cstring>
+#include <type_traits>
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "din.cuh"
@@ -38,7 +40,9 @@ struct BertPlan {
   float hdrop, adrop, sdrop;
   int passes;
   bool tc;
-  bool bf16;    // TFR_PREC_BF16: bf16 activations and GEMM operands (see the bf16 path below)
+  bool h16;     // TFR_PREC_BF16 / TFR_PREC_FP16: 16-bit activations and GEMM operands (see the
+                // 16-bit path below)
+  bool f16;     // TFR_PREC_FP16: the 16-bit type is fp16, else bf16
   int sms;
   unsigned long long seed;
   // parameters (floats)
@@ -56,9 +60,9 @@ struct BertPlan {
   size_t part_off, part_stride, cs_off, cs_stride;
   size_t emb_ws_off, emb_ws_floats;
   int rows_per_split, splits, s_rows_per_split, s_splits;
-  // bf16 mode: the GEMM outputs y / y2 (consumed by the next LayerNorm), the [CLS] rows'
+  // 16-bit modes: the GEMM outputs y / y2 (consumed by the next LayerNorm), the [CLS] rows'
   // gradient, and the weight shadows W [in, out] (wb) and W^T [out, in] (wbt) of Wqkv, Wo, W1,
-  // W2 per layer, then Wp, at the same bf16 offsets in both
+  // W2 per layer, then Wp, at the same 16-bit offsets in both
   size_t ytmp_off, dcls_off, wb_off, wbt_off, sh_layer, sh_total;
   size_t ws_floats;
 
@@ -124,15 +128,17 @@ int check_bert_cfg(const tfr_bert_cfg* c) {
                   c->output_dropout >= 0.f && c->output_dropout < 1.f,
               "dropout rates must be in [0, 1)");
   TFR_REQUIRE(c->precision == TFR_PREC_FP32 || c->precision == TFR_PREC_TF32 ||
-                  c->precision == TFR_PREC_BF16,
-              "precision %d must be TFR_PREC_FP32 (%d), TFR_PREC_TF32 (%d) or TFR_PREC_BF16 (%d)",
-              c->precision, TFR_PREC_FP32, TFR_PREC_TF32, TFR_PREC_BF16);
-  // the bf16 GEMM engine reads 16-byte rows: hidden, intermediate and head sizes in whole
+                  c->precision == TFR_PREC_BF16 || c->precision == TFR_PREC_FP16,
+              "precision %d must be TFR_PREC_FP32 (%d), TFR_PREC_TF32 (%d), TFR_PREC_BF16 (%d) "
+              "or TFR_PREC_FP16 (%d)",
+              c->precision, TFR_PREC_FP32, TFR_PREC_TF32, TFR_PREC_BF16, TFR_PREC_FP16);
+  // the 16-bit GEMM engine reads 16-byte rows: hidden, intermediate and head sizes in whole
   // 8-element chunks
-  TFR_REQUIRE(c->precision != TFR_PREC_BF16 ||
-                  (c->hidden_size % 8 == 0 && c->intermediate_size % 8 == 0 && dh % 8 == 0),
-              "TFR_PREC_BF16 needs hidden_size %d, intermediate_size %d and head size %d to be "
-              "multiples of 8", c->hidden_size, c->intermediate_size, dh);
+  const bool h16 = c->precision == TFR_PREC_BF16 || c->precision == TFR_PREC_FP16;
+  TFR_REQUIRE(!h16 || (c->hidden_size % 8 == 0 && c->intermediate_size % 8 == 0 && dh % 8 == 0),
+              "%s needs hidden_size %d, intermediate_size %d and head size %d to be "
+              "multiples of 8", c->precision == TFR_PREC_FP16 ? "TFR_PREC_FP16" : "TFR_PREC_BF16",
+              c->hidden_size, c->intermediate_size, dh);
   return TFR_OK;
 }
 
@@ -170,9 +176,9 @@ void row_splits(size_t M, int target, int* rows_per, int* splits) {
   *splits = kb > 0 ? (kb + kb_per - 1) / kb_per : 1;
 }
 
-size_t bf16_floats(size_t n) { return al64((n + 1) / 2); }   // floats that hold n bf16
+size_t h16_floats(size_t n) { return al64((n + 1) / 2); }   // floats that hold n 16-bit values
 
-// Split count of a bf16 dW GEMM (mn = 1: Kin x Nout output tiles of 128 x 128, `rows` of k in
+// Split count of a 16-bit dW GEMM (mn = 1: Kin x Nout output tiles of 128 x 128, `rows` of k in
 // blocks of 64), from a cost model of the persistent grid: whole waves of tiles x splits work
 // items over the SMs, each split's k blocks at about 0.5 us (a 128 x 128 x 64 bf16 block on
 // one SM), plus writing and reading back one fp32 partial per split at about 3 TB/s.  Every
@@ -194,40 +200,40 @@ int dw_splits(int sms, size_t Kin, size_t Nout, size_t rows) {
 
 size_t dw_stride(size_t Kin, size_t Nout) { return (Kin + 127) / 128 * 128 * Nout; }
 
-// bf16 mode's workspace: bf16 activations and backward signals, fp32 LayerNorm state, residual
-// gradient and partials; offsets in floats.
-void bf16_layout(BertPlan* p) {
+// The 16-bit modes' workspace (the same for bf16 and fp16): 16-bit activations and backward
+// signals, fp32 LayerNorm state, residual gradient and partials; offsets in floats.
+void layout16(BertPlan* p) {
   const size_t M = (size_t)p->M, E = p->E, I = p->I, H = p->H, Sz = (size_t)p->S;
   size_t w = 0;
-  for (int l = 0; l <= p->NL; ++l) { p->xs_off[l] = w; w += bf16_floats(M * E); }
+  for (int l = 0; l <= p->NL; ++l) { p->xs_off[l] = w; w += h16_floats(M * E); }
   p->xhe_off = w; w += al64(M * E);
   p->rse_off = w; w += al64(M);
   p->pos_ids_off = w; w += al64(M);
   for (int l = 0; l < p->NL; ++l) {
-    p->qkv_off[l] = w; w += bf16_floats(M * 3 * E);
-    p->o_off[l] = w; w += bf16_floats(M * E);
+    p->qkv_off[l] = w; w += h16_floats(M * 3 * E);
+    p->o_off[l] = w; w += h16_floats(M * E);
     p->lse_off[l] = w; w += al64(2 * M * H);
     p->xh1_off[l] = w; w += al64(M * E);
     p->rs1_off[l] = w; w += al64(M);
-    p->x1_off[l] = w; w += bf16_floats(M * E);
-    p->u_off[l] = w; w += bf16_floats(M * I);
-    p->a_off[l] = w; w += bf16_floats(M * I);
+    p->x1_off[l] = w; w += h16_floats(M * E);
+    p->u_off[l] = w; w += h16_floats(M * I);
+    p->a_off[l] = w; w += h16_floats(M * I);
     p->xh2_off[l] = w; w += al64(M * E);
     p->rs2_off[l] = w; w += al64(M);
   }
-  p->ytmp_off = w; w += bf16_floats(M * E);
-  p->pre_off = w; w += bf16_floats(Sz * E);
+  p->ytmp_off = w; w += h16_floats(M * E);
+  p->pre_off = w; w += h16_floats(Sz * E);
   p->pooled_off = w; w += al64(Sz * E);
   p->g_off = w; w += al64(M * E);
   p->dres_off = w; w += al64(M * E);
-  p->dy_off = w; w += al64(M * E);   // bf16 in the layers, fp32 for the embedding tables
-  p->tmp_off = w; w += bf16_floats(M * E);
-  p->do_off = w; w += bf16_floats(M * E);
-  p->dqkv_off = w; w += bf16_floats(M * 3 * E);
-  p->da_off = w; w += bf16_floats(M * I);
+  p->dy_off = w; w += al64(M * E);   // 16-bit in the layers, fp32 for the embedding tables
+  p->tmp_off = w; w += h16_floats(M * E);
+  p->do_off = w; w += h16_floats(M * E);
+  p->dqkv_off = w; w += h16_floats(M * 3 * E);
+  p->da_off = w; w += h16_floats(M * I);
   p->dsum_off = w; w += al64(M * H);
-  p->dpre_off = w; w += bf16_floats(Sz * E);
-  p->dcls_off = w; w += bf16_floats(Sz * E);
+  p->dpre_off = w; w += h16_floats(Sz * E);
+  p->dcls_off = w; w += h16_floats(Sz * E);
   const int nsplit = p->splits > p->s_splits ? p->splits : p->s_splits;
   // LayerNorm partials (2E per split) and the dW GEMMs' split partials share one region
   p->part_stride = al64(2 * E);
@@ -243,8 +249,8 @@ void bf16_layout(BertPlan* p) {
   p->emb_ws_off = w; w += p->emb_ws_floats;
   p->sh_layer = 4 * E * E + 2 * E * I;
   p->sh_total = (size_t)p->NL * p->sh_layer + E * E;
-  p->wb_off = w; w += bf16_floats(p->sh_total);
-  p->wbt_off = w; w += bf16_floats(p->sh_total);
+  p->wb_off = w; w += h16_floats(p->sh_total);
+  p->wbt_off = w; w += h16_floats(p->sh_total);
   p->ws_floats = w;
 }
 
@@ -261,9 +267,10 @@ int make_bert_plan(const tfr_bert_cfg* c, int S, int L, BertPlan* p) {
   p->sdrop = c->training ? c->output_dropout : 0.f;
   p->seed = c->seed;
   p->tc = c->precision == TFR_PREC_TF32;
-  p->bf16 = c->precision == TFR_PREC_BF16;
+  p->h16 = c->precision == TFR_PREC_BF16 || c->precision == TFR_PREC_FP16;
+  p->f16 = c->precision == TFR_PREC_FP16;
   p->passes = p->tc ? 1 : 3;
-  if (p->bf16) {
+  if (p->h16) {
     p->sms = num_sms();
     row_splits((size_t)p->M, p->sms, &p->rows_per_split, &p->splits);
     row_splits((size_t)S, p->sms, &p->s_rows_per_split, &p->s_splits);
@@ -274,7 +281,7 @@ int make_bert_plan(const tfr_bert_cfg* c, int S, int L, BertPlan* p) {
       if (b > eb) eb = b;
     }
     p->emb_ws_floats = al64((eb + 3) / 4 + 64);
-    bf16_layout(p);
+    layout16(p);
     return TFR_OK;
   }
   const size_t M = (size_t)p->M, E = p->E, I = p->I, H = p->H, Sz = (size_t)S;
@@ -335,12 +342,20 @@ int make_bert_plan(const tfr_bert_cfg* c, int S, int L, BertPlan* p) {
 
 using bf16 = __nv_bfloat16;
 
-// Element access of the kernels that run on fp32 or (bf16 mode) bf16 rows: fp32 in registers,
-// bf16 stores rounded to nearest even.
+// Element access of the kernels that run on fp32 or (16-bit modes) bf16 / fp16 rows: fp32 in
+// registers, 16-bit stores rounded to nearest even (fp16: subnormals kept, magnitudes past
+// 65504 stored as inf).
 __device__ __forceinline__ float ldf(const float* p) { return *p; }
 __device__ __forceinline__ float ldf(const bf16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ float ldf(const __half* p) { return __half2float(*p); }
 __device__ __forceinline__ void stf(float* p, float v) { *p = v; }
 __device__ __forceinline__ void stf(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ void stf(__half* p, float v) { *p = __float2half_rn(v); }
+template <typename T>
+__device__ __forceinline__ T rn16(float v) {
+  if constexpr (std::is_same_v<T, __half>) return __float2half_rn(v);
+  else return __float2bfloat16_rn(v);
+}
 
 // ---------------------------------------------------------------------------------------------
 // LayerNorm over rows of width E <= 32 * NPL, one warp per row; column c = lane + 32 k.
@@ -773,23 +788,25 @@ int bert_bwd(const int32_t* wid, const uint8_t* mask, const int32_t* tid, const 
 }
 
 // ---------------------------------------------------------------------------------------------
-// bf16 mode (TFR_PREC_BF16).  Activations, GEMM operands and backward signals are bf16 in the
-// workspace; every projection runs on the bf16 wgmma engine (tc_gemm_bf16.cu), the attention
-// core on din_bf16.cu.  Parameters, gradients, LayerNorm state, the residual gradient g / dres
+// 16-bit modes (TFR_PREC_BF16, TFR_PREC_FP16), one code path templated on the element type T
+// (bf16 or fp16).  Activations, GEMM operands and backward signals are T in the workspace; every
+// projection runs on the 16-bit wgmma engine (tc_gemm_bf16.cu), the attention core on
+// din_bf16.cu.  Parameters, gradients, LayerNorm state, the residual gradient g / dres
 // and every partial sum stay fp32:
-//   forward   out = bf16(A W + b)    A K-major, W^T [out, in] shadow K-major (mn = 0)
+//   forward   out = T(A W + b)       A K-major, W^T [out, in] shadow K-major (mn = 0)
 //   backward  dW  = A^T dZ           both as stored, MN-major (mn = 1), fp32 split partials
 //                                    reduced in fixed order
-//             db  = colsum(dZ)       fp32 column sums of the bf16 dZ, per row range
-//             dA  = bf16(dZ W^T)     dZ K-major, W [in, out] shadow K-major (mn = 0)
+//             db  = colsum(dZ)       fp32 column sums of the 16-bit dZ, per row range
+//             dA  = T(dZ W^T)        dZ K-major, W [in, out] shadow K-major (mn = 0)
 // ---------------------------------------------------------------------------------------------
 
-// wb = bf16(W) [in, out] and wbt = bf16(W)^T [out, in] of every projection kernel: blockIdx.y
+// wb = T(W) [in, out] and wbt = T(W)^T [out, in] of every projection kernel: blockIdx.y
 // picks the matrix (Wqkv, Wo, W1, W2 of each layer, then Wp), 32 x 32 tiles through shared
 // memory so both stores are coalesced.
+template <typename T>
 __global__ void __launch_bounds__(256)
-shadow_kernel(const float* __restrict__ params, BertPlan p, bf16* __restrict__ wb,
-              bf16* __restrict__ wbt) {
+shadow_kernel(const float* __restrict__ params, BertPlan p, T* __restrict__ wb,
+              T* __restrict__ wbt) {
   __shared__ float tile[32][33];
   const int e = blockIdx.y, l = e / 4;
   size_t src, dst;
@@ -813,54 +830,59 @@ shadow_kernel(const float* __restrict__ params, BertPlan p, bf16* __restrict__ w
       const int k = k0 + r, n = n0 + tx;
       if (k < kin && n < nout) {
         const float v = params[src + (size_t)k * nout + n];
-        wb[dst + (size_t)k * nout + n] = __float2bfloat16_rn(v);
+        wb[dst + (size_t)k * nout + n] = rn16<T>(v);
         tile[r][tx] = v;
       }
     }
     __syncthreads();
     for (int r = ty; r < 32; r += 8) {
       const int n = n0 + r, k = k0 + tx;
-      if (n < nout && k < kin) wbt[dst + (size_t)n * kin + k] = __float2bfloat16_rn(tile[tx][r]);
+      if (n < nout && k < kin) wbt[dst + (size_t)n * kin + k] = rn16<T>(tile[tx][r]);
     }
     __syncthreads();
   }
 }
 
-// mlp_colsum over bf16 dZ: partial[z][n] = sum of rows [z rows_per, ...) of column n, in row
+// mlp_colsum over 16-bit dZ: partial[z][n] = sum of rows [z rows_per, ...) of column n, in row
 // order.
+template <typename T>
 __global__ void __launch_bounds__(256)
-colsum_bf16_kernel(const bf16* __restrict__ dZ, int M, int N, int rows_per,
+colsum16_kernel(const T* __restrict__ dZ, int M, int N, int rows_per,
                    float* __restrict__ partial, size_t pstride) {
   const int z = blockIdx.x;
   const int mbeg = z * rows_per, mend = min(M, mbeg + rows_per);
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
     float acc = 0.f;
-    for (int m = mbeg; m < mend; ++m) acc += __bfloat162float(dZ[(size_t)m * N + n]);
+    for (int m = mbeg; m < mend; ++m) acc += ldf(dZ + (size_t)m * N + n);
     partial[(size_t)z * pstride + n] = acc;
   }
 }
 
 // g[s L E + c] = dcls[s E + c]: the [CLS] rows' gradient into the (zeroed) residual gradient.
+template <typename T>
 __global__ void __launch_bounds__(256)
-cls_scatter_kernel(const bf16* __restrict__ dcls, int S, int E, int L, float* __restrict__ g) {
+cls_scatter_kernel(const T* __restrict__ dcls, int S, int E, int L, float* __restrict__ g) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)S * E) return;
   const size_t s = i / E, c = i % E;
-  g[s * L * E + c] = __bfloat162float(dcls[i]);
+  g[s * L * E + c] = ldf(dcls + i);
 }
 
-#define TFR_BERT_LN_DISPATCH_BF16(E, kernel, grid, ...)                                      \
-  ((E) <= 128   ? (kernel<4, bf16><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)         \
-   : (E) <= 256 ? (kernel<8, bf16><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)         \
-   : (E) <= 512 ? (kernel<16, bf16><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)        \
-                : (kernel<32, bf16><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0))
+#define TFR_BERT_LN_DISPATCH16(E, kernel, grid, ...)                                      \
+  ((E) <= 128   ? (kernel<4, T><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)         \
+   : (E) <= 256 ? (kernel<8, T><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)         \
+   : (E) <= 512 ? (kernel<16, T><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0)        \
+                : (kernel<32, T><<<grid, kLnWarps * 32, 0, st>>>(__VA_ARGS__), 0))
 
-bf16* bf(float* ws, size_t off) { return reinterpret_cast<bf16*>(ws + off); }
+template <typename T>
+T* h16(float* ws, size_t off) { return reinterpret_cast<T*>(ws + off); }
 
-// C [GM, GN] (ldc) = bf16(A B^T (+ bias)): A [GM, GK] (lda), B [GN, GK] (ldb), both K-major.
-int bgemm(const bf16* A, int lda, const bf16* B, int ldb, bf16* C, int ldc, int GM, int GN,
+// C [GM, GN] (ldc) = T(A B^T (+ bias)): A [GM, GK] (lda), B [GN, GK] (ldb), both K-major.
+template <typename T>
+int bgemm(const T* A, int lda, const T* B, int ldb, T* C, int ldc, int GM, int GN,
           int GK, const float* bias, cudaStream_t st) {
   tcb::GemmDesc g{};
+  g.f16 = std::is_same_v<T, __half>;
   g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
   g.GM = GM; g.GN = GN; g.GK = GK;
   g.mn = 0;
@@ -872,13 +894,14 @@ int bgemm(const bf16* A, int lda, const bf16* B, int ldb, bf16* C, int ldc, int 
 
 // grads_w[0 .. Kin Nout + Nout) = {A^T dZ, column sums of dZ} over M rows of A [M, Kin] (lda)
 // and dZ [M, Nout].
-int dense_grad_bf16(const BertPlan& p, float* ws, const bf16* A, int lda, int Kin,
-                    const bf16* dZ, int Nout, int M, bool seq_rows, float* grads_w,
+template <typename T>
+int dense_grad16(const BertPlan& p, float* ws, const T* A, int lda, int Kin,
+                    const T* dZ, int Nout, int M, bool seq_rows, float* grads_w,
                     cudaStream_t st) {
   const int rows_per = seq_rows ? p.s_rows_per_split : p.rows_per_split;
   const int splits = seq_rows ? p.s_splits : p.splits;
   float* cs = ws + p.cs_off;
-  colsum_bf16_kernel<<<splits, 256, 0, st>>>(dZ, M, Nout, rows_per, cs, p.cs_stride);
+  colsum16_kernel<<<splits, 256, 0, st>>>(dZ, M, Nout, rows_per, cs, p.cs_stride);
   TFR_LAUNCH_OK();
   int rc = mlp_reduce_partials(cs, splits, p.cs_stride, (size_t)Nout,
                                grads_w + (size_t)Kin * Nout, st);
@@ -891,15 +914,17 @@ int dense_grad_bf16(const BertPlan& p, float* ws, const bf16* A, int lda, int Ki
   g.GM = Kin; g.GN = Nout; g.GK = M;
   g.mn = 1; g.epi = tcb::EPI_STORE;
   g.splits = ksplits; g.split_stride = stride;
+  g.f16 = std::is_same_v<T, __half>;
   rc = tcb::gemm(g, st);
   if (rc) return rc;
   return mlp_reduce_partials(ws + p.part_off, ksplits, stride, (size_t)Kin * Nout, grads_w, st);
 }
 
-int ln_bwd_bf16(const BertPlan& p, float* ws, const float* g, size_t xh_off, size_t rs_off,
-                const float* gamma, float ydrop, unsigned long long yseed, float* dres, bf16* dy,
+template <typename T>
+int ln_bwd16(const BertPlan& p, float* ws, const float* g, size_t xh_off, size_t rs_off,
+                const float* gamma, float ydrop, unsigned long long yseed, float* dres, T* dy,
                 float* dgamma, cudaStream_t st) {
-  TFR_BERT_LN_DISPATCH_BF16(p.E, ln_bwd_kernel, p.splits, g, ws + xh_off, ws + rs_off, gamma,
+  TFR_BERT_LN_DISPATCH16(p.E, ln_bwd_kernel, p.splits, g, ws + xh_off, ws + rs_off, gamma,
                             p.M, p.E, p.rows_per_split, 0.f, 0ull, ydrop, yseed, dres, dy,
                             ws + p.part_off, p.part_stride);
   TFR_LAUNCH_OK();
@@ -907,36 +932,37 @@ int ln_bwd_bf16(const BertPlan& p, float* ws, const float* g, size_t xh_off, siz
                              st);
 }
 
-int bert_fwd_bf16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, const BertPlan& p,
+template <typename T>
+int bert_fwd16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, const BertPlan& p,
                   const float* params, float* ws, float* scores, int* bad_ids, cudaStream_t st) {
   const int E = p.E, I = p.I, M = p.M;
   const size_t MI = (size_t)M * I;
-  bf16* wbt = bf(ws, p.wbt_off);
-  shadow_kernel<<<dim3(64, 4 * p.NL + 1), 256, 0, st>>>(params, p, bf(ws, p.wb_off), wbt);
+  T* wbt = h16<T>(ws, p.wbt_off);
+  shadow_kernel<T><<<dim3(64, 4 * p.NL + 1), 256, 0, st>>>(params, p, h16<T>(ws, p.wb_off), wbt);
   TFR_LAUNCH_OK();
   const unsigned ln_grid = blocks_for(M, kLnWarps);
-  TFR_BERT_LN_DISPATCH_BF16(E, emb_ln_fwd_kernel, ln_grid, wid, tid, M, p.L, params, p, p.hdrop,
+  TFR_BERT_LN_DISPATCH16(E, emb_ln_fwd_kernel, ln_grid, wid, tid, M, p.L, params, p, p.hdrop,
                             site_seed(p.seed, p.site_emb()), ws + p.xhe_off, ws + p.rse_off,
-                            bf(ws, p.xs_off[0]), reinterpret_cast<int32_t*>(ws + p.pos_ids_off),
+                            h16<T>(ws, p.xs_off[0]), reinterpret_cast<int32_t*>(ws + p.pos_ids_off),
                             bad_ids);
   TFR_LAUNCH_OK();
-  bf16* y = bf(ws, p.ytmp_off);
+  T* y = h16<T>(ws, p.ytmp_off);
   int rc;
   for (int l = 0; l < p.NL; ++l) {
-    const bf16* x = bf(ws, p.xs_off[l]);
-    bf16* qkv = bf(ws, p.qkv_off[l]);
-    bf16* o = bf(ws, p.o_off[l]);
-    bf16* x1 = bf(ws, p.x1_off[l]);
-    bf16* u = bf(ws, p.u_off[l]);
-    bf16* a = bf(ws, p.a_off[l]);
+    const T* x = h16<T>(ws, p.xs_off[l]);
+    T* qkv = h16<T>(ws, p.qkv_off[l]);
+    T* o = h16<T>(ws, p.o_off[l]);
+    T* x1 = h16<T>(ws, p.x1_off[l]);
+    T* u = h16<T>(ws, p.u_off[l]);
+    T* a = h16<T>(ws, p.a_off[l]);
     rc = bgemm(x, E, wbt + p.sh_wqkv(l), E, qkv, 3 * E, M, 3 * E, E, params + p.bqkv(l), st);
     if (rc) return rc;
-    rc = din_bf16_attn_fwd(qkv, mask, p.S, p.L, p.H, p.dh, p.adrop,
+    rc = din16_attn_fwd(qkv, mask, p.S, p.L, p.H, p.dh, p.adrop,
                            site_seed(p.seed, p.site_attn(l)), o, ws + p.lse_off[l], st);
     if (rc) return rc;
     rc = bgemm(o, E, wbt + p.sh_wo(l), E, y, E, M, E, E, params + p.bo(l), st);
     if (rc) return rc;
-    TFR_BERT_LN_DISPATCH_BF16(E, ln_fwd_kernel, ln_grid, y, x, M, E, params + p.g1(l),
+    TFR_BERT_LN_DISPATCH16(E, ln_fwd_kernel, ln_grid, y, x, M, E, params + p.g1(l),
                               params + p.g1(l) + E, p.hdrop, site_seed(p.seed, p.site_h1(l)),
                               ws + p.xh1_off[l], ws + p.rs1_off[l], x1);
     TFR_LAUNCH_OK();
@@ -946,13 +972,13 @@ int bert_fwd_bf16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, c
     TFR_LAUNCH_OK();
     rc = bgemm(a, I, wbt + p.sh_w2(l), I, y, E, M, E, I, params + p.b2(l), st);
     if (rc) return rc;
-    TFR_BERT_LN_DISPATCH_BF16(E, ln_fwd_kernel, ln_grid, y, x1, M, E, params + p.g2(l),
+    TFR_BERT_LN_DISPATCH16(E, ln_fwd_kernel, ln_grid, y, x1, M, E, params + p.g2(l),
                               params + p.g2(l) + E, p.hdrop, site_seed(p.seed, p.site_h2(l)),
-                              ws + p.xh2_off[l], ws + p.rs2_off[l], bf(ws, p.xs_off[l + 1]));
+                              ws + p.xh2_off[l], ws + p.rs2_off[l], h16<T>(ws, p.xs_off[l + 1]));
     TFR_LAUNCH_OK();
   }
-  bf16* pre = bf(ws, p.pre_off);
-  rc = bgemm(bf(ws, p.xs_off[p.NL]), p.L * E, wbt + p.sh_wp(), E, pre, E, p.S, E, E,
+  T* pre = h16<T>(ws, p.pre_off);
+  rc = bgemm(h16<T>(ws, p.xs_off[p.NL]), p.L * E, wbt + p.sh_wp(), E, pre, E, p.S, E, E,
              params + p.bp(), st);
   if (rc) return rc;
   head_fwd_kernel<<<blocks_for(p.S, 8), 256, 0, st>>>(
@@ -962,28 +988,29 @@ int bert_fwd_bf16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, c
   return TFR_OK;
 }
 
-int bert_bwd_bf16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, const BertPlan& p,
+template <typename T>
+int bert_bwd16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, const BertPlan& p,
                   const float* params, const float* dscores, float* ws, float* grads,
                   cudaStream_t st) {
   const int E = p.E, I = p.I, M = p.M, S = p.S;
   const size_t ME = (size_t)M * E, MI = (size_t)M * I;
   float* g = ws + p.g_off;       // d loss / d (current layer's output), fp32
   float* dres = ws + p.dres_off;
-  bf16* dy = bf(ws, p.dy_off);
-  bf16* tmp = bf(ws, p.tmp_off);
-  bf16* dO = bf(ws, p.do_off);
-  bf16* dqkv = bf(ws, p.dqkv_off);
-  bf16* da = bf(ws, p.da_off);
-  bf16* dpre = bf(ws, p.dpre_off);
-  const bf16* wb = bf(ws, p.wb_off);
+  T* dy = h16<T>(ws, p.dy_off);
+  T* tmp = h16<T>(ws, p.tmp_off);
+  T* dO = h16<T>(ws, p.do_off);
+  T* dqkv = h16<T>(ws, p.dqkv_off);
+  T* da = h16<T>(ws, p.da_off);
+  T* dpre = h16<T>(ws, p.dpre_off);
+  const T* wb = h16<T>(ws, p.wb_off);
   head_bwd_kernel<<<blocks_for(E + 1, 256), 256, 0, st>>>(
       ws + p.pooled_off, dscores, S, E, params + p.ws_(), p.sdrop,
       site_seed(p.seed, p.site_score()), dpre, grads + p.ws_(), grads + p.bs());
   TFR_LAUNCH_OK();
-  const bf16* xl = bf(ws, p.xs_off[p.NL]);
-  int rc = dense_grad_bf16(p, ws, xl, p.L * E, E, dpre, E, S, true, grads + p.wp(), st);
+  const T* xl = h16<T>(ws, p.xs_off[p.NL]);
+  int rc = dense_grad16(p, ws, xl, p.L * E, E, dpre, E, S, true, grads + p.wp(), st);
   if (rc) return rc;
-  bf16* dcls = bf(ws, p.dcls_off);
+  T* dcls = h16<T>(ws, p.dcls_off);
   rc = bgemm(dpre, E, wb + p.sh_wp(), E, dcls, E, S, E, E, nullptr, st);
   if (rc) return rc;
   TFR_CUDA_OK(cudaMemsetAsync(g, 0, ME * sizeof(float), st));
@@ -991,35 +1018,35 @@ int bert_bwd_bf16(const int32_t* wid, const uint8_t* mask, const int32_t* tid, c
   TFR_LAUNCH_OK();
   for (int l = p.NL - 1; l >= 0; --l) {
     // x'' = LN_2(drop(a W2 + b2) + x'):  dres = d x' (residual), dy = d(a W2 + b2)
-    rc = ln_bwd_bf16(p, ws, g, p.xh2_off[l], p.rs2_off[l], params + p.g2(l), p.hdrop,
+    rc = ln_bwd16(p, ws, g, p.xh2_off[l], p.rs2_off[l], params + p.g2(l), p.hdrop,
                      site_seed(p.seed, p.site_h2(l)), dres, dy, grads + p.g2(l), st);
     if (rc) return rc;
-    rc = dense_grad_bf16(p, ws, bf(ws, p.a_off[l]), I, I, dy, E, M, false, grads + p.w2(l), st);
+    rc = dense_grad16(p, ws, h16<T>(ws, p.a_off[l]), I, I, dy, E, M, false, grads + p.w2(l), st);
     if (rc) return rc;
     rc = bgemm(dy, E, wb + p.sh_w2(l), E, da, I, M, I, E, nullptr, st);
     if (rc) return rc;
-    gelu_bwd_kernel<<<blocks_for(MI, 256), 256, 0, st>>>(bf(ws, p.u_off[l]), MI, da);   // du
+    gelu_bwd_kernel<<<blocks_for(MI, 256), 256, 0, st>>>(h16<T>(ws, p.u_off[l]), MI, da);   // du
     TFR_LAUNCH_OK();
-    rc = dense_grad_bf16(p, ws, bf(ws, p.x1_off[l]), E, E, da, I, M, false, grads + p.w1(l), st);
+    rc = dense_grad16(p, ws, h16<T>(ws, p.x1_off[l]), E, E, da, I, M, false, grads + p.w1(l), st);
     if (rc) return rc;
     rc = bgemm(da, I, wb + p.sh_w1(l), I, tmp, E, M, E, I, nullptr, st);
     if (rc) return rc;
     add_kernel<<<blocks_for(ME, 256), 256, 0, st>>>(tmp, dres, ME, g);   // d x'
     TFR_LAUNCH_OK();
     // x' = LN_1(drop(o Wo + bo) + x)
-    rc = ln_bwd_bf16(p, ws, g, p.xh1_off[l], p.rs1_off[l], params + p.g1(l), p.hdrop,
+    rc = ln_bwd16(p, ws, g, p.xh1_off[l], p.rs1_off[l], params + p.g1(l), p.hdrop,
                      site_seed(p.seed, p.site_h1(l)), dres, dy, grads + p.g1(l), st);
     if (rc) return rc;
-    rc = dense_grad_bf16(p, ws, bf(ws, p.o_off[l]), E, E, dy, E, M, false, grads + p.wo(l), st);
+    rc = dense_grad16(p, ws, h16<T>(ws, p.o_off[l]), E, E, dy, E, M, false, grads + p.wo(l), st);
     if (rc) return rc;
     rc = bgemm(dy, E, wb + p.sh_wo(l), E, dO, E, M, E, E, nullptr, st);
     if (rc) return rc;
-    rc = din_bf16_attn_bwd(bf(ws, p.qkv_off[l]), mask, p.S, p.L, p.H, p.dh, p.adrop,
-                           site_seed(p.seed, p.site_attn(l)), bf(ws, p.o_off[l]),
+    rc = din16_attn_bwd(h16<T>(ws, p.qkv_off[l]), mask, p.S, p.L, p.H, p.dh, p.adrop,
+                           site_seed(p.seed, p.site_attn(l)), h16<T>(ws, p.o_off[l]),
                            ws + p.lse_off[l], dO, ws + p.dsum_off, dqkv, st);
     if (rc) return rc;
-    const bf16* x = bf(ws, p.xs_off[l]);
-    rc = dense_grad_bf16(p, ws, x, E, E, dqkv, 3 * E, M, false, grads + p.wqkv(l), st);
+    const T* x = h16<T>(ws, p.xs_off[l]);
+    rc = dense_grad16(p, ws, x, E, E, dqkv, 3 * E, M, false, grads + p.wqkv(l), st);
     if (rc) return rc;
     rc = bgemm(dqkv, 3 * E, wb + p.sh_wqkv(l), 3 * E, tmp, E, M, E, 3 * E, nullptr, st);
     if (rc) return rc;
@@ -1080,9 +1107,12 @@ extern "C" int tfr_bert_fwd(const int32_t* word_ids, const uint8_t* input_mask,
   BertPlan p;
   rc = make_bert_plan(cfg, S, L, &p);
   if (rc) return rc;
-  if (p.bf16)
-    return bert_fwd_bf16(word_ids, input_mask, type_ids, p, params, ws_align(workspace), scores,
-                         bad_ids, (cudaStream_t)stream);
+  if (p.f16)
+    return bert_fwd16<__half>(word_ids, input_mask, type_ids, p, params, ws_align(workspace),
+                              scores, bad_ids, (cudaStream_t)stream);
+  if (p.h16)
+    return bert_fwd16<bf16>(word_ids, input_mask, type_ids, p, params, ws_align(workspace), scores,
+                            bad_ids, (cudaStream_t)stream);
   return bert_fwd(word_ids, input_mask, type_ids, p, params, ws_align(workspace), scores, bad_ids,
                   (cudaStream_t)stream);
 }
@@ -1104,9 +1134,12 @@ extern "C" int tfr_bert_bwd(const int32_t* word_ids, const uint8_t* input_mask,
     TFR_CUDA_OK(cudaMemsetAsync(grads, 0, p.n_params * sizeof(float), (cudaStream_t)stream));
     return TFR_OK;
   }
-  if (p.bf16)
-    return bert_bwd_bf16(word_ids, input_mask, type_ids, p, params, dscores, ws_align(workspace),
-                         grads, (cudaStream_t)stream);
+  if (p.f16)
+    return bert_bwd16<__half>(word_ids, input_mask, type_ids, p, params, dscores,
+                              ws_align(workspace), grads, (cudaStream_t)stream);
+  if (p.h16)
+    return bert_bwd16<bf16>(word_ids, input_mask, type_ids, p, params, dscores,
+                            ws_align(workspace), grads, (cudaStream_t)stream);
   return bert_bwd(word_ids, input_mask, type_ids, p, params, dscores, ws_align(workspace), grads,
                   (cudaStream_t)stream);
 }

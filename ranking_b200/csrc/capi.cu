@@ -232,6 +232,65 @@ adamw_kernel(float* __restrict__ params, const float* __restrict__ grads, float*
   params[i] = p - step_size * mi / (sqrtf(vi) + eps);
 }
 
+// Loss-scaled AdamW (the header's dynamic loss scale rule): the step is skipped -- params, m
+// and v left as they are -- when *norm (the global norm of the scaled gradient) is inf or NaN;
+// otherwise g = grads * (1 / S) with S = *scale, clipped on the unscaled norm when clip_norm > 0,
+// then the update of adamw_kernel.  A kernel of its own, so adamw_kernel's code is unchanged.
+__global__ void __launch_bounds__(256)
+adamw_scaled_kernel(float* __restrict__ params, const float* __restrict__ grads,
+                    float* __restrict__ m, float* __restrict__ v,
+                    const uint8_t* __restrict__ decay_mask, size_t n, float lr, float beta1,
+                    float beta2, float eps, float wd, float step_size, float clip_norm,
+                    const float* __restrict__ norm, const float* __restrict__ scale) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const float nrm = *norm;
+  if (i >= n || !isfinite(nrm)) return;
+  const float S = *scale;
+  float g = grads[i] * (1.f / S);
+  if (clip_norm > 0.f) {
+    const float nu = (float)((double)nrm / (double)S);
+    g *= nu <= clip_norm ? 1.f : clip_norm / nu;
+  }
+  const float mi = beta1 * m[i] + (1.f - beta1) * g;
+  const float vi = beta2 * v[i] + (1.f - beta2) * g * g;
+  m[i] = mi;
+  v[i] = vi;
+  float p = params[i];
+  if (!decay_mask || decay_mask[i]) p -= lr * wd * p;
+  params[i] = p - step_size * mi / (sqrtf(vi) + eps);
+}
+
+// out = x * *scale (out may alias x).
+__global__ void __launch_bounds__(256)
+loss_scale_mul_kernel(const float* x, size_t n, const float* __restrict__ scale, float* out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = x[i] * *scale;
+}
+
+// One thread, after the step that read the old scale: the unscaled norm, then the dynamic
+// rule's new scale and good-step count (growth_steps 0: a fixed scale, left as it is).
+__global__ void __launch_bounds__(32)
+loss_scale_update_kernel(float* scale, int64_t* good_steps, const float* __restrict__ norm,
+                         float* unscaled_norm, int64_t growth_steps) {
+  if (threadIdx.x != 0) return;
+  const float S = *scale, nrm = *norm;
+  if (unscaled_norm) *unscaled_norm = (float)((double)nrm / (double)S);
+  if (growth_steps <= 0) return;
+  if (!isfinite(nrm)) {
+    *scale = fmaxf(S * 0.5f, 1.f);
+    *good_steps = 0;
+    return;
+  }
+  const int64_t c = *good_steps + 1;
+  if (c >= growth_steps) {
+    const float grown = S * 2.f;
+    if (isfinite(grown)) *scale = grown;
+    *good_steps = 0;
+  } else {
+    *good_steps = c;
+  }
+}
+
 // Global L2 norm, in two fixed-order passes.  Pass 1: thread t of block b sums squares (in
 // double) over fixed positions p = b * 256 + t + k * norm_blocks(n) * 256 -- float4 number p
 // when x is 16-byte aligned (the n % 4 tail elements then go to the first threads of block 0),
@@ -555,6 +614,49 @@ extern "C" int tfr_adamw_step_clipped(float* params, const float* grads, float* 
   adamw_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       params, grads, m, v, decay_mask, n, lr, beta1, beta2, eps, weight_decay, step_size,
       grad_scale, clip_norm, norm);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" int tfr_loss_scale_mul(const float* x, size_t n, const float* scale, float* out,
+                                  void* stream) {
+  TFR_REQUIRE(scale && out && (x || n == 0), "NULL argument");
+  if (n == 0) return TFR_OK;
+  loss_scale_mul_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      x, n, scale, out);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" int tfr_adamw_step_scaled(float* params, const float* grads, float* m, float* v,
+                                     const uint8_t* decay_mask, size_t n, float lr, float beta1,
+                                     float beta2, float eps, float weight_decay, int64_t step,
+                                     float clip_norm, const float* norm, const float* scale,
+                                     void* stream) {
+  TFR_REQUIRE(params && grads && m && v && norm && scale, "NULL argument");
+  TFR_REQUIRE(step >= 1, "AdamW step %lld must be >= 1", (long long)step);
+  TFR_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f,
+              "beta1 %g and beta2 %g must be in [0, 1)", (double)beta1, (double)beta2);
+  TFR_REQUIRE(clip_norm == 0.f || (clip_norm > 0.f && std::isfinite(clip_norm)),
+              "clip_norm %g must be 0 (off) or finite and > 0", (double)clip_norm);
+  if (n == 0) return TFR_OK;
+  const double t = (double)step;
+  const float step_size =
+      (float)((double)lr * std::sqrt(1.0 - std::pow((double)beta2, t)) /
+              (1.0 - std::pow((double)beta1, t)));
+  adamw_scaled_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      params, grads, m, v, decay_mask, n, lr, beta1, beta2, eps, weight_decay, step_size,
+      clip_norm, norm, scale);
+  TFR_LAUNCH_OK();
+  return TFR_OK;
+}
+
+extern "C" int tfr_loss_scale_update(float* scale, int64_t* good_steps, const float* norm,
+                                     float* unscaled_norm, int64_t growth_steps, void* stream) {
+  TFR_REQUIRE(scale && norm && (good_steps || growth_steps == 0), "NULL argument");
+  TFR_REQUIRE(growth_steps >= 0, "growth_steps %lld must be >= 0", (long long)growth_steps);
+  loss_scale_update_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(scale, good_steps, norm,
+                                                               unscaled_norm, growth_steps);
   TFR_LAUNCH_OK();
   return TFR_OK;
 }

@@ -4,6 +4,7 @@
 #include <cstdint>
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 namespace tfr {
@@ -38,17 +39,23 @@ int din_tc_attn_bwd(const float* qkv, const uint8_t* lmask, int B, int N, int H,
                     float drop, unsigned long long dseed, const float* O, const float* lse,
                     const float* dO, float* dsum, float* dqkv, cudaStream_t st);
 
-// bf16 tensor-core attention core (din_bf16.cu): qkv, O, dO and dqkv bf16, lse and dsum fp32,
-// same layouts and dropout draws.  P~ is rounded to bf16 after normalisation, before P~ v; dS
-// is rounded to bf16 before dS K and dS^T Q, and dQ / dK are scaled by 1 / sqrt(h) after
-// those products.  dsum = dO . O over the stored bf16 values.  h % 8 == 0, h <= 128.
-int din_bf16_attn_fwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
-                      float drop, unsigned long long dseed, __nv_bfloat16* O, float* lse,
-                      cudaStream_t st);
-int din_bf16_attn_bwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
-                      float drop, unsigned long long dseed, const __nv_bfloat16* O,
-                      const float* lse, const __nv_bfloat16* dO, float* dsum,
-                      __nv_bfloat16* dqkv, cudaStream_t st);
+// 16-bit tensor-core attention core (din_bf16.cu), one overload per element type (bf16, fp16):
+// qkv, O, dO and dqkv 16-bit, lse and dsum fp32, same layouts and dropout draws.  P~ is rounded
+// to 16 bits after normalisation, before P~ v; dS is rounded before dS K and dS^T Q, and dQ / dK
+// are scaled by 1 / sqrt(h) after those products.  dsum = dO . O over the stored 16-bit values.
+// h % 8 == 0, h <= 128.
+int din16_attn_fwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                   float drop, unsigned long long dseed, __nv_bfloat16* O, float* lse,
+                   cudaStream_t st);
+int din16_attn_fwd(const __half* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                   float drop, unsigned long long dseed, __half* O, float* lse, cudaStream_t st);
+int din16_attn_bwd(const __nv_bfloat16* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                   float drop, unsigned long long dseed, const __nv_bfloat16* O,
+                   const float* lse, const __nv_bfloat16* dO, float* dsum,
+                   __nv_bfloat16* dqkv, cudaStream_t st);
+int din16_attn_bwd(const __half* qkv, const uint8_t* lmask, int B, int N, int H, int h,
+                   float drop, unsigned long long dseed, const __half* O, const float* lse,
+                   const __half* dO, float* dsum, __half* dqkv, cudaStream_t st);
 
 // C [GM, GN] (ldc) = A B (+ bias, act) on the scorer GEMM engine, 3xTF32 (passes 3) or TF32
 // (passes 1).  a_mn / b_mn: operand stored MN-major (A^T [GK, GM], B [GK, GN]) instead of

@@ -1,5 +1,5 @@
 // Hopper (sm_90a) warpgroup-MMA GEMM core shared by the TF32 / 3xTF32 engine (tc_gemm.cu) and
-// the bf16 engine (tc_gemm_bf16.cu).
+// the 16-bit engine (tc_gemm_bf16.cu: bf16 or fp16 operands, the same code on either type).
 //
 //   * a CTA owns a 128 x 128 output tile: two consumer warpgroups of 64 rows, each issuing one
 //     wgmma.mma_async m64n128 per k step (m64n64 when the tile's live columns fit in 64).  In
@@ -38,6 +38,7 @@
 #pragma once
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 
 #include <type_traits>
@@ -342,20 +343,32 @@ __device__ __forceinline__ void mma_tf32_n136(float (&d)[2][32], float (&t)[4], 
                  "+f"(t[0]), "+f"(t[1]), "+f"(t[2]), "+f"(t[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
-// bf16 (k = 16): two bf16 per register.  TRANS_B: B is MN-major in shared memory.
-template <int TRANS_B>
-__device__ __forceinline__ void mma_bf16_n64(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
-  asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " TFR_WG_D32
-               ", {%32, %33, %34, %35}, %36, 1, 1, 1, %37;"
-               : TFR_WG_OUT32(d[0])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
+// bf16 / fp16 (k = 16): two elements per register.  TRANS_B: B is MN-major in shared memory.
+template <typename T, int TRANS_B>
+__device__ __forceinline__ void mma16_n64(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (std::is_same_v<T, __half>)
+    asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " TFR_WG_D32
+                 ", {%32, %33, %34, %35}, %36, 1, 1, 1, %37;"
+                 : TFR_WG_OUT32(d[0])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
+  else
+    asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " TFR_WG_D32
+                 ", {%32, %33, %34, %35}, %36, 1, 1, 1, %37;"
+                 : TFR_WG_OUT32(d[0])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
 }
-template <int TRANS_B>
-__device__ __forceinline__ void mma_bf16_n128(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
-  asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " TFR_WG_D64
-               ", {%64, %65, %66, %67}, %68, 1, 1, 1, %69;"
-               : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
+template <typename T, int TRANS_B>
+__device__ __forceinline__ void mma16_n128(float (&d)[2][32], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (std::is_same_v<T, __half>)
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " TFR_WG_D64
+                 ", {%64, %65, %66, %67}, %68, 1, 1, 1, %69;"
+                 : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
+  else
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " TFR_WG_D64
+                 ", {%64, %65, %66, %67}, %68, 1, 1, 1, %69;"
+                 : TFR_WG_OUT32(d[0]), TFR_WG_OUT32(d[1])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TRANS_B));
 }
 #undef TFR_WG_D32
 #undef TFR_WG_D64
@@ -365,6 +378,7 @@ __device__ __forceinline__ void mma_bf16_n128(float (&d)[2][32], const uint32_t 
 template <typename T> struct Elem;
 template <> struct Elem<float> { static constexpr int EPC = 4; static constexpr int BK = 32; };
 template <> struct Elem<__nv_bfloat16> { static constexpr int EPC = 8; static constexpr int BK = 64; };
+template <> struct Elem<__half> { static constexpr int EPC = 8; static constexpr int BK = 64; };
 
 // Byte offset of 16-byte chunk `kc` of row `row` in a K-major 128B-swizzled tile.
 __device__ __forceinline__ int swz_chunk(int row, int kc) { return row * 128 + (((kc ^ row) & 7) << 4); }
@@ -692,11 +706,29 @@ __device__ __forceinline__ void transpose_slab(unsigned char* t, unsigned char* 
   }
 }
 
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+// 16-bit stores of C (H: bf16 or fp16), rounded to nearest even.  fp16 keeps subnormals and
+// rounds magnitudes past its range to inf, which the stores pass on.
+template <typename H>
+__device__ __forceinline__ uint32_t pack16(float lo, float hi) {
   uint32_t r;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  if constexpr (std::is_same_v<H, __half>) asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  else asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+template <typename H>
+__device__ __forceinline__ H to16(float x) {
+  if constexpr (std::is_same_v<H, __half>) return __float2half_rn(x);
+  else return __float2bfloat16_rn(x);
+}
+template <typename H>
+__device__ __forceinline__ float round16(float x) {   // the value a 16-bit store keeps
+  if constexpr (std::is_same_v<H, __half>) return __half2float(__float2half_rn(x));
+  else return __bfloat162float(__float2bfloat16_rn(x));
+}
+// The 16-bit type of C when OUT16: the operand type (bf16 when the operands are fp32, a case
+// no launch instantiates with OUT16).
+template <typename T>
+using Out16 = std::conditional_t<sizeof(T) == 2, T, __nv_bfloat16>;
 
 // The epilogue warpgroup of a staged kernel: walks the CTA's tiles as the MMA warpgroups do and
 // finishes each from the staging tile `stg`.  Warp `ew` takes rows 32 ew .. 32 ew + 31, a lane
@@ -713,7 +745,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 // its running sum in the group's slot in global memory.  Slot and column always meet the same
 // thread, so plain loads and stores keep the running sums; the loads are issued before the row
 // pass, so the tile's tail only stores.
-template <bool OUT_BF16>
+template <typename H, bool OUT16>
 __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg) {
   const int lane = threadIdx.x & 31;
   const int et = threadIdx.x - kThreads, ew = et >> 5;
@@ -771,11 +803,11 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         if (j < live) b4[j] = __ldg(args.bias + col + j);
     }
     float* Cf = static_cast<float*>(args.C) + static_cast<size_t>(z) * args.split_stride;
-    __nv_bfloat16* Cb = static_cast<__nv_bfloat16*>(args.C);
+    H* Cb = static_cast<H*>(args.C);
     // vector stores need a row pitch of a multiple of 4 elements and a 16-byte (bf16: 8-byte)
     // aligned base (C and every split-K slice C + z * split_stride)
-    const uintptr_t cbase = OUT_BF16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
-    const bool vec_ok = (args.ldc % 4) == 0 && (cbase & (OUT_BF16 ? 7u : 15u)) == 0;
+    const uintptr_t cbase = OUT16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
+    const bool vec_ok = (args.ldc % 4) == 0 && (cbase & (OUT16 ? 7u : 15u)) == 0;
     const bool vec4 = live == 4 && vec_ok;
     // this lane's plane of sign words (tile columns 32 mpl .. 32 mpl + 31); every lane of a
     // live plane stores rows in the fast loop, also those whose own columns lie past GN
@@ -800,13 +832,13 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
       constexpr int EPI = decltype(kind)::value;
       constexpr bool PAIR = decltype(paired)::value;
       constexpr int STEP = PAIR ? 2 : 1;
-      using V = std::conditional_t<OUT_BF16, uint2, float4>;
+      using V = std::conditional_t<OUT16, uint2, float4>;
       const bool on = live == 4, relu = args.act == TFR_ACT_RELU;
       const int row0 = m0 + ew * 32;
       const float4* sp =
           reinterpret_cast<const float4*>(stg + (ew * 32 + half) * kStagingPitch + 4 * cl);
       const size_t coff = static_cast<size_t>(row0 + half) * args.ldc + col;
-      V* cp = OUT_BF16 ? reinterpret_cast<V*>(Cb + coff) : reinterpret_cast<V*>(Cf + coff);
+      V* cp = OUT16 ? reinterpret_cast<V*>(Cb + coff) : reinterpret_cast<V*>(Cf + coff);
       const int cstep = args.ldc / 4;
       // sign words: lane q of a group keeps the word of row 8 b + q and stores it once the
       // group's 8 rows are done (with two rows a step, half h keeps the rows of parity h)
@@ -829,10 +861,10 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
           if (!(w & 8u)) v.w = 0.f;
         }
         if (!on) v = make_float4(0.f, 0.f, 0.f, 0.f);
-        const uint2 packed = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+        const uint2 packed = make_uint2(pack16<H>(v.x, v.y), pack16<H>(v.z, v.w));
         if (args.bits_out) {
           auto pos = [](float y) {   // the sign bit is that of the stored value
-            return (OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(y)) : y) > 0.f ? 1u : 0u;
+            return (OUT16 ? round16<H>(y) : y) > 0.f ? 1u : 0u;
           };
           const uint32_t nib = pos(v.x) | pos(v.y) << 1 | pos(v.z) << 2 | pos(v.w) << 3;
           const uint32_t w = sign_word(nib);
@@ -841,7 +873,7 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         }
         if (args.colsum_cols) const_cast<float4*>(sp)[i * (kStagingPitch / 4)] = v;
         if (on) {
-          if (OUT_BF16) *reinterpret_cast<uint2*>(cp + static_cast<size_t>(i) * cstep) = packed;
+          if (OUT16) *reinterpret_cast<uint2*>(cp + static_cast<size_t>(i) * cstep) = packed;
           else *reinterpret_cast<float4*>(cp + static_cast<size_t>(i) * cstep) = v;
         }
       }
@@ -881,7 +913,7 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
         }
         if (!rlive || j >= live) y = 0.f;
         x[j] = y;   // column sums take the fp32 value, sign bits the stored one
-        const float stored = OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(y)) : y;
+        const float stored = OUT16 ? round16<H>(y) : y;
         nib |= (stored > 0.f ? 1u : 0u) << j;
       }
       if (args.bits_out) {
@@ -890,14 +922,14 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
       }
       if (args.colsum_cols) *reinterpret_cast<float4*>(sp) = make_float4(x[0], x[1], x[2], x[3]);
       if (!rlive || live == 0) continue;
-      if (OUT_BF16) {
-        __nv_bfloat16* p = Cb + static_cast<size_t>(row) * args.ldc + col;
+      if (OUT16) {
+        H* p = Cb + static_cast<size_t>(row) * args.ldc + col;
         if (vec4) {
-          *reinterpret_cast<uint2*>(p) = make_uint2(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]));
+          *reinterpret_cast<uint2*>(p) = make_uint2(pack16<H>(x[0], x[1]), pack16<H>(x[2], x[3]));
         } else {
 #pragma unroll
           for (int j = 0; j < 4; ++j)
-            if (j < live) p[j] = __float2bfloat16_rn(x[j]);
+            if (j < live) p[j] = to16<H>(x[j]);
         }
       } else if (args.store_transposed) {
 #pragma unroll
@@ -935,17 +967,19 @@ __device__ __forceinline__ void epilogue_warpgroup(const Args& args, float* stg)
 }
 
 // PASSES: 1 (one product) or 3 (3xTF32: Ahi Bhi + Alo Bhi + Ahi Blo; float only).
-// PRE_B: B comes pre-split (B = hi parts, B_lo = lo parts).  OUT_BF16: C is bf16 (row-major).
+// PRE_B: B comes pre-split (B = hi parts, B_lo = lo parts).  OUT16: C has the operands' 16-bit
+// type (row-major).
 // Staged (K-major A): a third warpgroup runs the epilogue from a staging tile.
 // Shared memory: num_stages x {B hi, [B lo,] A}, then the staging tile (staged) or
 // [8][colsum_cols] floats.  FOLD (launched when GN has a remainder to fold): the last column
 // tile owns it, B tiles have 136 rows and wide tiles issue m64n136.
-template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16, bool FOLD>
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT16, bool FOLD>
 __global__ void __launch_bounds__(block_threads<T, A_MN, B_MN>(), 1)
 gemm_kernel(const Args args) {
   constexpr bool STAGED = !A_MN;
   constexpr bool PROD = has_producer<T, A_MN, B_MN>();   // a producer warpgroup runs the ring
   constexpr bool F32 = sizeof(T) == 4;
+  using H = Out16<T>;
   constexpr int EPC = Elem<T>::EPC;
   constexpr int BK = Elem<T>::BK;
   constexpr int KSTEP = F32 ? 8 : 16;   // k of one wgmma
@@ -979,7 +1013,7 @@ gemm_kernel(const Args args) {
     if (threadIdx.x >= kThreads) {
       setmaxnreg_dec<kEpiRegs>();
       if constexpr (PROD) producer_ring<P3, PRE_B, FOLD>(args, smem, stages, full, empty);
-      else epilogue_warpgroup<OUT_BF16>(args, cacc);
+      else epilogue_warpgroup<Out16<T>, OUT16>(args, cacc);
       return;
     }
     setmaxnreg_inc<kMmaRegs>();
@@ -1035,7 +1069,7 @@ gemm_kernel(const Args args) {
         cp_async16(st + swz_chunk(r, kc), B + off, n * static_cast<int>(sizeof(T)));
         if (PRE_B) cp_async16(st + kBTile + swz_chunk(r, kc), Blo + off, n * static_cast<int>(sizeof(T)));
       }
-    } else if (!F32) {   // bf16 [2 atoms of 64 n][64 k rows][8 chunks of n], swizzled
+    } else if (!F32) {   // 16-bit [2 atoms of 64 n][64 k rows][8 chunks of n], swizzled
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int c = threadIdx.x + i * kThreads;
@@ -1148,7 +1182,7 @@ gemm_kernel(const Args args) {
         const int krem = args.GK - (kb0 + kb) * BK;
         const int ksteps = krem >= BK ? NKS : (krem + KSTEP - 1) / KSTEP;
         // A fragments of every k step (m64 x k, per warp 16 rows): register i holds row
-        // g + 8 (i % 2), k t + 4 (i / 2) (TF32) / k pair 2t + 8 (i / 2) (bf16)
+        // g + 8 (i % 2), k t + 4 (i / 2) (TF32) / k pair 2t + 8 (i / 2) (16-bit)
         const int g = lane >> 2, t = lane & 3;
         const int row = wg * 64 + wq * 16 + g;
         const unsigned char* sa = smem + s * kStage + kAOff;
@@ -1225,12 +1259,12 @@ gemm_kernel(const Args args) {
               }
             } else if (B_MN) {   // 16 k rows (2 KB) per wgmma
               const uint64_t db = desc_sw128_mn(st + ks * 2048, BK * 128);
-              if (W) mma_bf16_n128<1>(acc, ahi[ks], db);
-              else mma_bf16_n64<1>(acc, ahi[ks], db);
+              if (W) mma16_n128<T, 1>(acc, ahi[ks], db);
+              else mma16_n64<T, 1>(acc, ahi[ks], db);
             } else {
               const uint64_t db = desc_sw128(st + ks * 32);
-              if (W) mma_bf16_n128<0>(acc, ahi[ks], db);
-              else mma_bf16_n64<0>(acc, ahi[ks], db);
+              if (W) mma16_n128<T, 0>(acc, ahi[ks], db);
+              else mma16_n64<T, 0>(acc, ahi[ks], db);
             }
           }
           wgmma_commit();
@@ -1285,11 +1319,11 @@ gemm_kernel(const Args args) {
     // ------------------------------------------- epilogue on the accumulator registers ----
     const int rbase = m0 + wg * 64 + wq * 16 + (lane >> 2);
     float* Cf = static_cast<float*>(args.C) + static_cast<size_t>(z) * args.split_stride;
-    __nv_bfloat16* Cb = static_cast<__nv_bfloat16*>(args.C);
+    H* Cb = static_cast<H*>(args.C);
     // paired stores need an even row pitch and a base aligned to two elements (C and every
     // split-K slice C + z * split_stride)
-    const uintptr_t cbase = OUT_BF16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
-    const bool vec2 = (args.ldc % 2) == 0 && (cbase & (OUT_BF16 ? 3u : 7u)) == 0;
+    const uintptr_t cbase = OUT16 ? reinterpret_cast<uintptr_t>(Cb) : reinterpret_cast<uintptr_t>(Cf);
+    const bool vec2 = (args.ldc % 2) == 0 && (cbase & (OUT16 ? 3u : 7u)) == 0;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (h == 1 && !two_n) break;
@@ -1326,7 +1360,7 @@ gemm_kernel(const Args args) {
           }
           if (row >= args.GM || col >= args.GN) x = 0.f;
           acc[h][j] = x;   // column sums take the fp32 value, sign bits the stored one
-          const float stored = OUT_BF16 ? __bfloat162float(__float2bfloat16_rn(x)) : x;
+          const float stored = OUT16 ? round16<H>(x) : x;
           bits_out[rr] |= (stored > 0.f ? 1u : 0u) << (cin & 31);
         }
         if (args.bits_out) {
@@ -1349,13 +1383,13 @@ gemm_kernel(const Args args) {
         if (row >= args.GM || col >= args.GN) continue;
         const float x0 = acc[h][j], x1 = acc[h][j + 1];
         const bool both = col + 1 < args.GN;
-        if (OUT_BF16) {
-          __nv_bfloat16* p = Cb + static_cast<size_t>(row) * args.ldc + col;
+        if (OUT16) {
+          H* p = Cb + static_cast<size_t>(row) * args.ldc + col;
           if (both && vec2) {
-            *reinterpret_cast<uint32_t*>(p) = pack_bf16(x0, x1);
+            *reinterpret_cast<uint32_t*>(p) = pack16<H>(x0, x1);
           } else {
-            p[0] = __float2bfloat16_rn(x0);
-            if (both) p[1] = __float2bfloat16_rn(x1);
+            p[0] = to16<H>(x0);
+            if (both) p[1] = to16<H>(x1);
           }
         } else if (args.store_transposed) {
           Cf[static_cast<size_t>(col) * args.ldc + row] = x0;
@@ -1421,7 +1455,7 @@ gemm_kernel(const Args args) {
   }
 }
 
-template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16, bool FOLD>
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT16, bool FOLD>
 int launch_grid(Args a, cudaStream_t st, int* ctas) {
   a.m_tiles = (a.GM + BM - 1) / BM;
   a.n_tiles = col_tiles(a.GN, FOLD);
@@ -1433,7 +1467,7 @@ int launch_grid(Args a, cudaStream_t st, int* ctas) {
   const int grid = total < sms ? total : sms;
   if (ctas) *ctas = grid;
   const size_t smem = smem_bytes(PASSES, a.colsum_cols, !A_MN, FOLD, has_producer<T, A_MN, B_MN>());
-  auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, FOLD>;
+  auto kern = gemm_kernel<T, A_MN, B_MN, PASSES, PRE_B, OUT16, FOLD>;
   TFR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, block_threads<T, A_MN, B_MN>(), smem, st>>>(a);
   TFR_LAUNCH_OK();
@@ -1443,11 +1477,11 @@ int launch_grid(Args a, cudaStream_t st, int* ctas) {
 // Launches the persistent grid; *ctas receives its size (column-sum slots = 8 x ctas).  A GN
 // with a remainder to fold takes the folding kernel.  Every other GN takes the plain one, whose
 // m64n128 MMAs and 128-row B tiles cost less per k block when no column is folded.
-template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT_BF16>
+template <typename T, bool A_MN, bool B_MN, int PASSES, bool PRE_B, bool OUT16>
 int launch(Args a, cudaStream_t st, int* ctas) {
   if constexpr (folds<T, A_MN, B_MN>())
-    if (folded_cols(a.GN) > 0) return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, true>(a, st, ctas);
-  return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT_BF16, false>(a, st, ctas);
+    if (folded_cols(a.GN) > 0) return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT16, true>(a, st, ctas);
+  return launch_grid<T, A_MN, B_MN, PASSES, PRE_B, OUT16, false>(a, st, ctas);
 }
 
 }  // namespace wg

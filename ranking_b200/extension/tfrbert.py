@@ -5,7 +5,8 @@ document) token sequence of a list, trained end to end with a ranking loss and A
     TFRBertScorer                      Dropout(bert_output_dropout) + Dense(1) on the pooled
                                        [CLS] output
     TFRBertRankingTrainer              one fused step: tfr_bert_fwd, the fused loss kernel,
-                                       tfr_bert_bwd, tfr_adamw_step
+                                       tfr_bert_bwd, tfr_adamw_step (fp16: with dynamic loss
+                                       scaling)
     TFRBertDataConfig, tfrbert_batches ELWC records with `input_ids` / `input_mask` /
                                        `segment_ids` (int64, dim seq_length) and a label
 
@@ -14,8 +15,10 @@ flat parameter layout are written out in include/tfr_b200.h (K15).  `set_weights
 tensors in the documented order (`weight_names`); `BertEncoder.from_pretrained` and
 `load_checkpoint` import a pretrained TF2 BertEncoder or Hugging Face BERT checkpoint
 (bert_checkpoint.py), and `BertEncoderConfig.from_json` reads its `config.json`.
-Precision: 'fp32', 'tf32' or 'bf16' (the reference's 'mixed_bfloat16' policy: fp32 parameters
-and optimizer, bf16 activations, GEMMs and attention core; sizes in multiples of 8).
+Precision: 'fp32', 'tf32', 'bf16' (the reference's 'mixed_bfloat16' policy: fp32 parameters
+and optimizer, bf16 activations, GEMMs and attention core; sizes in multiples of 8) or 'fp16'
+(the reference's 'mixed_float16', its choice for GPUs: the same with fp16, trained with dynamic
+loss scaling).
 """
 import ctypes
 import dataclasses
@@ -29,7 +32,8 @@ from ranking_b200 import data as data_lib
 from ranking_b200 import train as train_lib
 from ranking_b200.extension import bert_checkpoint
 
-_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32, 'bf16': _C.PREC_BF16}
+_PRECISIONS = {'fp32': _C.PREC_FP32, 'tf32': _C.PREC_TF32, 'bf16': _C.PREC_BF16,
+               'fp16': _C.PREC_FP16}
 
 
 @dataclasses.dataclass
@@ -146,10 +150,11 @@ def _truncated_normal(gen, shape, stddev):
 class BertEncoder(object):
   """The encoder's flat parameters and configuration (pooler and score head included, so the
   scorer is one buffer: one gradient, one optimizer launch).  `precision` 'fp32' (default:
-  3xTF32 GEMMs, FP32 attention core), 'tf32' (one TF32 pass, wgmma attention core) or 'bf16'
+  3xTF32 GEMMs, FP32 attention core), 'tf32' (one TF32 pass, wgmma attention core), 'bf16'
   (mixed precision: bf16 activations, GEMMs and attention core on fp32 master weights, as
-  Keras' 'mixed_bfloat16' policy; hidden, intermediate and head sizes must be multiples of 8).
-  The parameters are the same in all three, so `set_precision` can switch a trained encoder.
+  Keras' 'mixed_bfloat16' policy; hidden, intermediate and head sizes must be multiples of 8)
+  or 'fp16' (the same with fp16, as 'mixed_float16'; its trainer scales the loss).  The
+  parameters are the same in all four, so `set_precision` can switch a trained encoder.
   Initialisation (host): truncated normal with stddev `initializer_range` for the tables and
   kernels, zero biases, LayerNorm gamma 1 / beta 0."""
 
@@ -304,15 +309,91 @@ class TFRBertRankingTrainer(train_lib.RankingTrainer):
   default; the recipe's AdamWeightDecay uses 1.0) clips to a global norm first.  Padded items
   (label < 0) are encoded too, as in the reference; the loss ignores them.  fit / evaluate /
   checkpoints are the base class's; batches are ({'input_word_ids', 'input_mask',
-  'input_type_ids'}, y) pairs."""
+  'input_type_ids'}, y) pairs.
+
+  fp16 steps (an encoder in precision 'fp16') scale the loss, as Keras' LossScaleOptimizer
+  does for 'mixed_float16' (the rule is include/tfr_b200.h's, next to AdamW's):
+  `loss_scale` 'dynamic' (default) starts at `initial_loss_scale` (2^15), halves on a step
+  whose scaled gradient holds an inf or NaN (that step is skipped: parameters and moments
+  untouched, `adam_step` still advances) and doubles after `dynamic_growth_steps` (2000)
+  finite steps in a row; a float is a fixed scale.  The step scales d loss / d scores by S on
+  the device (trainer.dscores holds the scaled values), takes the global norm of the scaled
+  gradient, and runs tfr_adamw_step_scaled and tfr_loss_scale_update: no host sync.
+  `loss_scale` (0-d float32) and `good_steps` (0-d int64, the finite steps since the last
+  change) are device tensors; `grad_norm` holds the last fp16 step's unscaled gradient norm,
+  before clipping.  fp16 needs optimizer 'adamw' and one rank (ValueError otherwise).  fp32,
+  tf32 and bf16 steps do not scale; `predict` never does."""
 
   def __init__(self, scorer, loss, optimizer='adamw', learning_rate=3e-5, epsilon=1e-6,
-               weight_decay_rate=0.01, **kw):
+               weight_decay_rate=0.01, loss_scale='dynamic', initial_loss_scale=2 ** 15,
+               dynamic_growth_steps=2000, **kw):
     self.scorer = scorer
     self.encoder = scorer.encoder
+    if loss_scale == 'dynamic':
+      init, growth = float(initial_loss_scale), int(dynamic_growth_steps)
+      if not (1.0 <= init < float('inf')):
+        raise ValueError('initial_loss_scale must be finite and >= 1, got %r' %
+                         (initial_loss_scale,))
+      if growth < 1:
+        raise ValueError('dynamic_growth_steps must be >= 1, got %r' % (dynamic_growth_steps,))
+    else:
+      try:
+        init, growth = float(loss_scale), 0
+      except (TypeError, ValueError):
+        raise ValueError("loss_scale must be 'dynamic' or a number, got %r" % (loss_scale,))
+      if not (0.0 < init < float('inf')):
+        raise ValueError('a fixed loss_scale must be finite and > 0, got %r' % (loss_scale,))
     super().__init__(scorer, loss, optimizer=optimizer, learning_rate=learning_rate,
                      epsilon=epsilon, weight_decay_rate=weight_decay_rate, **kw)
     self.bad_ids = torch.zeros(1, dtype=torch.int32, device=self.device)
+    self.initial_loss_scale = init
+    self.dynamic_growth_steps = growth   # 0: a fixed scale
+    self.loss_scale = torch.full((), init, dtype=torch.float32, device=self.device)
+    self.good_steps = torch.zeros((), dtype=torch.int64, device=self.device)
+    if self.encoder.precision == 'fp16':
+      self._check_fp16()
+
+  def _check_fp16(self):
+    """fp16's loss-scaled update is AdamW on one rank; its norm buffers on first use."""
+    if self.opt_kind != train_lib._OPT['adamw']:
+      raise ValueError("precision 'fp16' needs optimizer 'adamw' (loss scaling is built for "
+                       "AdamW only)")
+    if self.world > 1:
+      raise ValueError('precision fp16 supports one rank only, got world size %d' % self.world)
+    if getattr(self, '_scaled_norm', None) is None:
+      dev, n = self.device, self.scorer.flat.numel()
+      self._scaled_norm = torch.zeros((), dtype=torch.float32, device=dev)
+      if getattr(self, 'grad_norm', None) is None:
+        self.grad_norm = torch.zeros((), dtype=torch.float32, device=dev)
+      if getattr(self, '_norm_ws', None) is None:
+        self._norm_ws = torch.empty(_C.lib.tfr_global_norm_workspace_bytes(n),
+                                    dtype=torch.uint8, device=dev)
+
+  def reset_loss_scale(self):
+    """The loss scale back to its initial value, the good-step count to 0."""
+    self.loss_scale.fill_(self.initial_loss_scale)
+    self.good_steps.zero_()
+
+  def _apply(self, grads):
+    if self.encoder.precision != 'fp16':
+      super()._apply(grads)
+      return
+    # grads are the gradient of S * loss: norm, then the update and the scale's rule
+    t = self.tower
+    lr = self.lr(self.adam_step) if callable(self.lr) else self.lr
+    self.adam_step += 1
+    n = grads.numel()
+    st = _C.stream()
+    _C.check(_C.lib.tfr_global_norm(_C.ptr(grads), n, _C.ptr(self._scaled_norm),
+                                     _C.ptr(self._norm_ws), self._norm_ws.numel(), st))
+    _C.check(_C.lib.tfr_adamw_step_scaled(
+        _C.ptr(t.flat.data), _C.ptr(grads), _C.ptr(self.accum[:n]), _C.ptr(self.accum[n:]),
+        _C.ptr(self.decay_mask), n, lr, self.beta_1, self.beta_2, self.eps,
+        self.weight_decay_rate, self.adam_step, self.gradient_clip_norm or 0.0,
+        _C.ptr(self._scaled_norm), _C.ptr(self.loss_scale), st))
+    _C.check(_C.lib.tfr_loss_scale_update(_C.ptr(self.loss_scale), _C.ptr(self.good_steps),
+                                          _C.ptr(self._scaled_norm), _C.ptr(self.grad_norm),
+                                          self.dynamic_growth_steps, st))
 
   def _ensure_bert(self, b, n, seq):
     if self._shape == (b, n, seq):
@@ -356,6 +437,9 @@ class TFRBertRankingTrainer(train_lib.RankingTrainer):
                  mask=None):
     """ids / mask / type ids [B, N, L] (device or host), y_true [B, N] (label < 0 = padded
     item).  Returns the scalar loss as a 0-d device tensor (no host sync)."""
+    fp16 = self.encoder.precision == 'fp16'
+    if fp16:
+      self._check_fp16()
     wid, msk, tid, s, seq = self._inputs(input_word_ids, input_mask, input_type_ids)
     if mask is not None:
       y_true = torch.where(mask.to(y_true.device), y_true, torch.full_like(y_true, -1.0))
@@ -368,6 +452,9 @@ class TFRBertRankingTrainer(train_lib.RankingTrainer):
                                  _C.ptr(self.bad_ids), st))
     self.loss.fused_fwd_bwd(y_true, self.scores, sample_weight, self.dscores, self.per_list,
                             self.total2)
+    if fp16:   # d loss / d scores times S, in place
+      _C.check(_C.lib.tfr_loss_scale_mul(_C.ptr(self.dscores), self.dscores.numel(),
+                                         _C.ptr(self.loss_scale), _C.ptr(self.dscores), st))
     _C.check(_C.lib.tfr_bert_bwd(_C.ptr(wid), _C.ptr(msk), _C.ptr(tid), s, seq, cfg,
                                  _C.ptr(flat), _C.ptr(self.dscores), _C.ptr(self.ws),
                                  _C.ptr(grads), st))

@@ -13,7 +13,7 @@ from ranking_b200.keras import metrics as keras_metrics
 
 def save_checkpoint(trainer, path, step):
   """Parameters, optimizer accumulator, BN moving statistics and the step counter (and
-  AdamW's update count).
+  AdamW's update count, and a TFR-BERT trainer's loss scale and good-step count).
   Data parallel: rank 0 alone writes (replicas hold identical parameters; BN statistics
   are per replica and rank 0's are the ones kept), every rank waits for the file."""
   tower = trainer.tower
@@ -24,6 +24,9 @@ def save_checkpoint(trainer, path, step):
              'dims': list(tower.dims)}
     if hasattr(trainer, 'adam_step'):   # AdamW's update count t
       state['adam_step'] = int(trainer.adam_step)
+    if hasattr(trainer, 'loss_scale'):   # TFR-BERT's fp16 loss scale and good-step count
+      state['loss_scale'] = trainer.loss_scale.cpu()
+      state['good_steps'] = trainer.good_steps.cpu()
     torch.save(state, tmp)
     os.replace(tmp, path)      # atomic: a crash never leaves a torn file
   if dp.world_size(trainer.group) > 1:
@@ -43,6 +46,13 @@ def load_checkpoint(trainer, path):
       tower.bn_state.copy_(ckpt['bn_state'])
   if 'adam_step' in ckpt:
     trainer.adam_step = int(ckpt['adam_step'])
+  if hasattr(trainer, 'loss_scale'):   # a checkpoint without them: the initial scale, count 0
+    if 'loss_scale' in ckpt:
+      with torch.no_grad():
+        trainer.loss_scale.copy_(ckpt['loss_scale'])
+        trainer.good_steps.copy_(ckpt['good_steps'])
+    else:
+      trainer.reset_loss_scale()
   return int(ckpt['step'])
 
 

@@ -5,12 +5,16 @@ arms within one run:
   ours-fp32    3xTF32 GEMMs, FP32 attention core          (precision 'fp32')
   ours-tf32    TF32 GEMMs, wgmma TF32 attention core      (precision 'tf32')
   ours-bf16    bf16 GEMMs and wgmma attention core on fp32 master weights (precision 'bf16')
+  ours-fp16    the same in fp16 with dynamic loss scaling (precision 'fp16': tfr_loss_scale_mul,
+               tfr_global_norm, tfr_adamw_step_scaled, tfr_loss_scale_update)
   ours-*-clip  the same with gradient_clip_norm 1.0 (the recipe's AdamWeightDecay clipping:
                tfr_global_norm + tfr_adamw_step_clipped), for tf32 and bf16
   torch-fp32   torch autograd + torch.optim.AdamW, TF32 matmul off
   torch-tf32   the same with TF32 matmul on
   torch-bf16   the same under torch.autocast('cuda', dtype=torch.bfloat16): ours-bf16's
                like-for-like competitor (fp32 parameters and optimizer, bf16 compute)
+  torch-fp16   torch.autocast('cuda', dtype=torch.float16) with torch.amp.GradScaler (dynamic
+               loss scale): ours-fp16's competitor
 
 BERT-base (12 layers, E 768, H 12, I 3072), seq 64, lists of 10, at 4 lists (the reference
 yaml) and 32.  Dropout 0.1 everywhere in both.  Then one profiled step of each of our arms,
@@ -97,7 +101,7 @@ def _ours(precision, clip=None):
   return lambda wid, mask, tid, y: tr.train_step(wid, mask, tid, y)
 
 
-def _torch(tf32, bf16=False):
+def _torch(tf32, dtype=None):
   torch.manual_seed(1)
   model = TorchBert().cuda().train()
   decay = [p for n, p in model.named_parameters()
@@ -105,18 +109,20 @@ def _torch(tf32, bf16=False):
   rest = [p for n, p in model.named_parameters() if not any(p is q for q in decay)]
   opt = torch.optim.AdamW([{'params': decay, 'weight_decay': 0.01},
                            {'params': rest, 'weight_decay': 0.0}], lr=3e-5, eps=1e-6)
+  scaler = torch.amp.GradScaler('cuda', enabled=dtype == torch.float16)
 
   def step(wid, mask, tid, y):
     torch.backends.cuda.matmul.allow_tf32 = tf32
     torch.backends.cudnn.allow_tf32 = tf32
     b = wid.shape[0]
-    with torch.autocast('cuda', dtype=torch.bfloat16, enabled=bf16):
+    with torch.autocast('cuda', dtype=dtype or torch.bfloat16, enabled=dtype is not None):
       s = model(wid.reshape(b * N, SEQ), mask.reshape(b * N, SEQ),
                 tid.reshape(b * N, SEQ)).reshape(b, N)
     loss = _softmax_loss(y, s.float())
     opt.zero_grad(set_to_none=True)
-    loss.backward()
-    opt.step()
+    scaler.scale(loss).backward()   # no-ops without fp16
+    scaler.step(opt)
+    scaler.update()
     return loss
   return step
 
@@ -126,7 +132,7 @@ _FAMILIES = [('embedding', ('emb_ln', 'embedding', 'radix', 'segment', 'scatter_
              ('ffn_gelu', ('gelu',)),
              ('layernorm', ('ln_fwd', 'ln_bwd', 'reduce_partials')),
              ('pooler_loss', ('head_', 'loss', 'softmax', 'cls_scatter')),
-             ('optimizer', ('adamw', 'sumsq_partials', 'norm_final')),
+             ('optimizer', ('adamw', 'sumsq_partials', 'norm_final', 'loss_scale')),
              ('gemm', ('gemm', 'wgmma', 'colsum', 'tc_', 'weight_grad', 'split', 'shadow'))]
 
 
@@ -140,8 +146,10 @@ def _family(name):
 
 _ARMS = {'ours-fp32': lambda: _ours('fp32'), 'ours-tf32': lambda: _ours('tf32'),
          'ours-tf32-clip': lambda: _ours('tf32', 1.0), 'ours-bf16': lambda: _ours('bf16'),
-         'ours-bf16-clip': lambda: _ours('bf16', 1.0), 'torch-fp32': lambda: _torch(False),
-         'torch-tf32': lambda: _torch(True), 'torch-bf16': lambda: _torch(True, bf16=True)}
+         'ours-bf16-clip': lambda: _ours('bf16', 1.0), 'ours-fp16': lambda: _ours('fp16'),
+         'torch-fp32': lambda: _torch(False), 'torch-tf32': lambda: _torch(True),
+         'torch-bf16': lambda: _torch(True, torch.bfloat16),
+         'torch-fp16': lambda: _torch(True, torch.float16)}
 
 
 def main():
